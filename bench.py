@@ -20,6 +20,7 @@ download).  Extra objects on the same JSON line:
     python bench.py --gpus N --steps K --warmup W            # torchrun for N > 1
     python bench.py --impl reference ...                       # CPU oracle arm (rank 0 only)
     python bench.py --quick                                    # headline legs only (A/B runs)
+    python bench.py --dump-outputs DIR ...                     # also write the headline window's solution as DIR/*.npy
 """
 import argparse
 import ctypes
@@ -42,11 +43,6 @@ N_KF, N_LM = 10, 4000                # configs[1]
 W20_KF, W20_LM = 20, 8000            # configs[3]'s BA part = north_star's 20-keyframe target
 ICP_K, ICP_P = 120000, 1000000       # configs[2]
 EVAL_KF, EVAL_LM = 5000, 500000      # configs[4] scale
-# dram__bytes_read.sum + dram__bytes_write.sum of one ba_eval_two_frame_kernel launch at that scale, from the `ncu --set full`
-# capture summarised in profiles/eval_r1_v3_summary.txt (75.19 MB + 293.14 MB): a constant from that capture, not measured in-run
-EVAL_DRAM_BYTES_PER_LAUNCH = 368.33e6
-# the same for ba_linearize_kernel<0> at that scale: profiles/global_r2_final_summary.txt (143.74 MB read + 115.21 MB written)
-FUSED_DRAM_BYTES_PER_LAUNCH = 258.95e6
 BYTES_TWO_FRAME = 308                # SURVEY 8(d): 40 const + 12 idx + 16 r + 240 J
 BYTES_FUSED = {0: 52, 1: 52, 2: 44}  # SURVEY 8(d) fused mode: TwoFrame, PoseOnly, TwoCamera
 BYTES_KNN_QUERY = 40                 # query 16 + idx 12 + d2 12, plus 16 B per map point amortised over the queries
@@ -63,7 +59,7 @@ def peaks():
     if os.path.exists(p):
         with open(p) as f:
             return json.load(f)["hbm_gbs"], "MEASURED_PEAKS.json"
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "H100 SXM data sheet (not measured)"
 
 
 class ClockSampler(threading.Thread):
@@ -93,6 +89,17 @@ class ClockSampler(threading.Thread):
                 "reasons": reasons, "samples": len(self.rows)}
 
 
+def gpu_info(device):
+    """Name and power limit of the card the numbers were measured on (read-only query)."""
+    try:
+        out = subprocess.run(["nvidia-smi", "-i", str(device), "--query-gpu=name,power.limit", "--format=csv,noheader"],
+                             capture_output=True, text=True, timeout=10).stdout.strip().split(",")
+        return {"name": out[0].strip(), "power_limit": out[1].strip()}
+    except Exception:
+        import torch
+        return {"name": torch.cuda.get_device_name(device), "power_limit": None}
+
+
 def bench_options(api, iters, threads=1):
     # fixed iteration count: tolerances off so both arms do exactly the same number of LM iterations
     return backend.default_options(api, max_num_iterations=iters, function_tolerance=0.0, gradient_tolerance=0.0,
@@ -101,14 +108,14 @@ def bench_options(api, iters, threads=1):
 
 def run_solves(problem, d, api, total_iters, per_solve, threads=1):
     """Run LM iterations in solves of `per_solve` iterations restarted from the initial guess until
-    `total_iters` iterations have been executed; returns iterations actually executed."""
-    done = 0
+    `total_iters` iterations have been executed; returns (iterations actually executed, last solve's summary)."""
+    done, s = 0, None
     while done < total_iters:
         k = min(per_solve, total_iters - done)
         problem.update_params(d["poses"], d["vec3"], d["rho"])
         s = problem.solve(bench_options(api, k, threads))
         done += max(1, s.num_iterations)
-    return done
+    return done, s
 
 
 def cpu_window(orc, octx, n_kf, n_lm, iters, T):
@@ -116,7 +123,7 @@ def cpu_window(orc, octx, n_kf, n_lm, iters, T):
     p = backend.Problem.from_dict(octx, d)
     run_solves(p, d, orc, PER, PER, T)
     t0 = time.perf_counter()
-    it = run_solves(p, d, orc, iters, PER, T)
+    it, _ = run_solves(p, d, orc, iters, PER, T)
     dt = time.perf_counter() - t0
     return synth.count_rows(d) * it / dt, it, dt
 
@@ -154,7 +161,7 @@ def reference_arm(args):
     p = backend.Problem.from_dict(octx, d)
     run_solves(p, d, orc, max(1, args.warmup), PER, T)
     t0 = time.perf_counter()
-    it = run_solves(p, d, orc, args.steps, PER, T)
+    it, _ = run_solves(p, d, orc, args.steps, PER, T)
     dt = time.perf_counter() - t0
     val = rows * it / dt
     w20, it20, _ = cpu_window(orc, octx, W20_KF, W20_LM, 20, T)
@@ -192,15 +199,15 @@ def kernel_split(lvb, run, iters):
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
-    ap.add_argument("--steps", type=int, default=40)
+    ap.add_argument("--steps", type=int, default=200, help="timed LM iterations of each window leg")
     ap.add_argument("--warmup", type=int, default=10)
-    ap.add_argument("--impl", default="b200")
+    ap.add_argument("--impl", default="cuda")
     ap.add_argument("--quick", action="store_true", help="headline legs only")
     ap.add_argument("--skip-icp", action="store_true")
     ap.add_argument("--skip-roofline", action="store_true")
     ap.add_argument("--skip-global", action="store_true")
     ap.add_argument("--skip-cpu", action="store_true")
-    ap.add_argument("--blocks", type=int, default=0, help="repetitions of the timed region (0: enough for >= 50 solves); profiler runs use 1")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the headline window's solution after its last timed step as DIR/<name>.npy")
     args = ap.parse_args()
     if args.quick:
         args.skip_icp = args.skip_roofline = args.skip_global = args.skip_cpu = True
@@ -270,14 +277,16 @@ def main():
             prob = backend.Problem.from_dict(c, d)
             run_solves(prob, d, lvb, max(3, warmup), PER)
             l0 = c.launch_count()
-            its = run_solves(prob, d, lvb, steps, PER)
+            run_solves(prob, d, lvb, steps, PER)
             launches = c.launch_count() - l0
-            # the K-step timed region, repeated so that >= 50 solves stand behind the number; the median block is reported
-            blocks = args.blocks if args.blocks > 0 else max(5, -(-50 * PER // max(1, steps)))
-            times, its = timed_blocks(lambda: run_solves(prob, d, lvb, steps, PER), blocks)
-            ms = float(np.median(times))
-            res = {"rows": rows, "iters": its, "ms": ms, "launches": int(launches), "blocks": blocks,
-                   "ms_min": float(np.min(times)), "ms_max": float(np.max(times)), "problem": prob, "data": d, "full": full}
+            # the timed region: exactly `steps` LM iterations, in solves of up to PER iterations, each timed with CUDA events
+            times, per_step, iters, last = [], [], 0, None
+            while iters < steps:
+                t, (n, last) = timed_blocks(lambda: run_solves(prob, d, lvb, min(PER, steps - iters), PER), 1)
+                times.append(t[0]); per_step.append(t[0] / n)
+                iters += n
+            res = {"rows": rows, "iters": iters, "ms": float(np.sum(times)), "launches": int(launches), "solves": len(times),
+                   "ms_min": float(np.min(per_step)), "ms_max": float(np.max(per_step)), "problem": prob, "data": d, "full": full, "summary": last}
             # e2e: build + upload + solve + download through the public API, host buffers
             h2d = sum(f[0].nbytes + f[1].nbytes for f in d["factors"].values()) + d["poses"].nbytes + d["vec3"].nbytes + d["rho"].nbytes + 22 * 8
             d2h = d["poses"].nbytes + d["vec3"].nbytes + d["rho"].nbytes
@@ -293,7 +302,7 @@ def main():
                 return n
             one_e2e()
             walls = []
-            for _ in range(max(3, blocks // 4)):
+            for _ in range(3):
                 barrier()
                 t0 = time.perf_counter()
                 n_it = one_e2e()
@@ -313,12 +322,20 @@ def main():
             "ms_per_step": w10["ms"] / w10["iters"], "higher_is_better": True, "scaling": "weak", "vs_baseline": None, "dtype": "f64", "data": "synthetic",
             "config": {"workload": workload_text(w10["rows"]),
                        "blocks": synth.count_blocks(w10["full"]), "iters_per_solve": PER,
-                       "timing": "median of %d repetitions of the %d-step timed region (min %.4f / max %.4f ms per step)" % (w10["blocks"], w10["iters"], w10["ms_min"] / w10["iters"], w10["ms_max"] / w10["iters"]),
-                       "l2": "BA working set (~3 MB) is L2-resident by design; the roofline legs stream 394 MB / 97 MB per launch (> 126 MB L2 together with their outputs)"},
+                       "timing": "%d timed steps in %d solves, CUDA events per solve (min %.4f / max %.4f ms per step)" % (w10["iters"], w10["solves"], w10["ms_min"], w10["ms_max"]),
+                       "l2": "BA working set (~3 MB) is L2-resident by design; the roofline legs stream 394 MB / 97 MB per launch (> 50 MB L2)"},
             "e2e": {"value": w10["rows"] * w10["e2e_iters"] / (w10["e2e_ms"] * 1e-3), "unit": "rows/s", "h2d_bytes_per_step": w10["h2d"], "d2h_bytes_per_step": w10["d2h"],
                     "note": "Problem.from_dict (AoS->SoA, H2D) + solve(%d iterations) + D2H of all parameter blocks, per solve; bytes amortised per iteration" % PER},
             "gpu_launches": w10["launches"],
+            "gpu": gpu_info(local_rank),
         }
+        if args.dump_outputs and rank == 0:
+            # what a caller of the timed path receives after its last step: the solved parameter blocks and the solve summary
+            os.makedirs(args.dump_outputs, exist_ok=True)
+            s10, p10 = w10["summary"], w10["problem"]
+            for name, arr in (("poses", p10.poses()), ("vec3", p10.vec3()), ("inv_depths", p10.inv_depths()),
+                              ("summary", [s10.initial_cost, s10.final_cost, s10.num_iterations])):
+                np.save(os.path.join(args.dump_outputs, name + ".npy"), np.asarray(arr, dtype=np.float64))
         # per-kernel split of one pass (direct launches, CUDA event after every kernel): names the limiter at every N
         p10, d10 = w10["problem"], w10["data"]
         split = kernel_split(lvb, lambda: run_solves(p10, d10, lvb, PER, PER), PER)
@@ -326,7 +343,7 @@ def main():
         line["kernels"] = {"window10_us_per_iteration": {k: round(v, 2) for k, v in sorted(split.items(), key=lambda kv: -kv[1])},
                            "compute_us": round(sum(split.values()) - comm, 2), "allreduce_us": round(comm, 2),
                            "note": "direct launches with an event after each kernel (the timed legs replay a CUDA graph); includes launch gaps"}
-        # the only dense contraction of the path on the tensor cores (north_star: tcgen05 for the Schur reduce): same window, schur_mode = 1
+        # the only dense contraction of the path on the tensor cores: same window, schur_mode = 1
         if world == 1:
             def run_tc(iters):
                 n = 0
@@ -336,7 +353,7 @@ def main():
                     n += max(1, p10.solve(o).num_iterations)
                 return n
             run_tc(3 * PER)
-            t_tc, it_tc = timed_blocks(lambda: run_tc(args.steps), 5)
+            t_tc, it_tc = timed_blocks(lambda: run_tc(args.steps), 1)
             s_fp = p10.solve(bench_options(lvb, PER)); p10.update_params(d10["poses"], d10["vec3"], d10["rho"])
             o = bench_options(lvb, PER); o.schur_mode = 1
             s_tc = p10.solve(o)
@@ -344,7 +361,7 @@ def main():
             line["schur_tc"] = {"ms_per_step": float(np.median(t_tc)) / it_tc, "fp64_ms_per_step": w10["ms"] / w10["iters"],
                                 "final_cost_rel_diff": abs(s_tc.final_cost - s_fp.final_cost) / s_fp.final_cost,
                                 "us_per_iteration": {k: round(v, 2) for k, v in tc_split.items() if "schur" in k},
-                                "note": "ba_schur_tc_kernel: tcgen05.mma kind::f16 on split-bf16 operands (hi/mid/lo), FP32 accumulation in TMEM, FP64 epilogue; "
+                                "note": "ba_schur_tc_kernel: wgmma m64n128k16 on split-bf16 operands (hi/mid/lo), FP32 accumulation in registers, FP64 epilogue; "
                                         "opt-in (schur_mode = 1): the contraction is ~0.2 GFLOP per iteration, so packing + the FP64 scatter cost what the tensor pipe saves"}
         p10.close()
 
@@ -379,8 +396,7 @@ def main():
             torch.cuda.synchronize()
             t_avg = sum(ev[i].elapsed_time(ev[i + 1]) for i in range(reps)) / reps
             ach = nb * BYTES_TWO_FRAME / (t_avg * 1e-3) / 1e9
-            line["roofline"] = {"bound": "hbm", "achieved": ach, "peak": peak, "unit": "GB/s", "frac": ach / peak, "traffic": EVAL_DRAM_BYTES_PER_LAUNCH,
-                                "traffic_source": "profiles/eval_r1_v3_summary.txt (ncu --set full), not measured in-run",
+            line["roofline"] = {"bound": "hbm", "achieved": ach, "peak": peak, "unit": "GB/s", "frac": ach / peak,
                                 "kernel": "ba_eval_two_frame_kernel", "blocks": nb, "bytes_per_block": BYTES_TWO_FRAME,
                                 "us_per_launch": t_avg * 1e3, "peak_source": peak_src, "workload": "configs[4]-scale: %d keyframes, %d landmarks" % (EVAL_KF, EVAL_LM),
                                 "rows_per_s": 2.0 * nb / (t_avg * 1e-3)}
@@ -415,7 +431,6 @@ def main():
                 alg = sum(n * BYTES_FUSED[k] for k, n in zip((0, 1, 2), nblk))
                 if us:
                     line["roofline_fused"] = {"bound": "hbm", "achieved": alg / (us * 1e-6) / 1e9, "peak": peak, "unit": "GB/s", "frac": alg / (us * 1e-6) / 1e9 / peak,
-                                              "traffic": FUSED_DRAM_BYTES_PER_LAUNCH, "traffic_source": "profiles/global_r2_final_summary.txt (ncu --set full), not measured in-run",
                                               "kernel": "ba_linearize_kernel<0>", "blocks": nblk, "bytes_per_block": [BYTES_FUSED[k] for k in (0, 1, 2)],
                                               "us_per_launch": us, "peak_source": peak_src, "total_blocks": g_blocks,
                                               "note": "algorithmic bytes are SURVEY 8(d)'s fused-mode figures; the kernel also writes the per-factor coupling rows the Schur step reads"}
@@ -485,7 +500,6 @@ def main():
                 line["icp"]["knn_only"] = {"value": ICP_K / (us * 1e-6), "unit": "points/s", "us": us,
                                            "note": "icp_associate_kernel alone: float32 transform + exact 3-NN + gate + plane normal"}
                 line["icp"]["roofline"] = {"bound": "hbm", "achieved": alg / (us * 1e-6) / 1e9, "peak": peak, "unit": "GB/s", "frac": alg / (us * 1e-6) / 1e9 / peak,
-                                           "traffic": 17.53e6, "traffic_source": "profiles/icp_r2_final_summary.txt (ncu --set full), not measured in-run",
                                            "kernel": "icp_associate_kernel", "bytes_per_query": BYTES_KNN_QUERY + 16.0 * ICP_P / ICP_K,
                                            "us_per_launch": us, "peak_source": peak_src,
                                            "note": "algorithmic minimum of SURVEY 8(d) (40 B/query + the map read once); the voxel ring scan is L2-latency work on top"}

@@ -1,4 +1,4 @@
-/* lvio_b200.h -- C ABI of the B200-native optimisation backend for lvio_fusion.
+/* lvio_b200.h -- C ABI of the H100-native optimisation backend for lvio_fusion.
  *
  * This is the drop-in boundary (SURVEY.md section 8b).  The reference has no FFI layer: its
  * hot path calls the C++ APIs of Ceres (ceres::Problem / ceres::Solve) and PCL
@@ -13,7 +13,7 @@
  * created from it belong to ONE host thread at a time; use one context per solving thread
  * (Backend thread, global thread, Relocator thread: backend.cpp:19-20, relocator.cpp:188-206) --
  * the C++ shim does (lvb::Runtime is thread_local).  There is NO CPU fallback: every compute entry point fails with
- * LVB_ERR_CUDA when no sm_100 device is usable.
+ * LVB_ERR_CUDA when no sm_90 device is usable.
  *
  * Layouts: pose = Sophus::SE3d::data() = [qx qy qz qw tx ty tz] (include/lvio_fusion/ceres/
  * base.hpp:27-38), T_world_body.  All BA arithmetic is FP64.  Jacobians handed back by the
@@ -83,7 +83,7 @@ typedef struct lvb_solve_options {
     int linear_solver_type;             /* 0 SPARSE_SCHUR, 1 SPARSE_NORMAL_CHOLESKY, 2 DENSE_QR (informational:
                                            the device always eliminates inverse depths exactly) */
     int num_threads;                    /* ignored on the device */
-    int schur_mode;                     /* 0 = FP64 CUDA-core Schur (parity reference), 1 = tcgen05 split-precision */
+    int schur_mode;                     /* 0 = FP64 CUDA-core Schur (parity reference), 1 = tensor-core (wgmma) split-precision */
 } lvb_solve_options;
 
 /* ceres::Solver::Summary fields the reference reads (mapping.cpp:279-280,293-294) + diagnostics. */
@@ -169,7 +169,7 @@ LVB_API int lvb_ba_reduced_system(lvb_ba* ba, double radius, double* S, double* 
 /* ceres::Solve(options, &problem, &summary) (adapt/problem.h:83-88). Parameters are updated
  * on the device; fetch them with the getters (the shim writes them back in place). */
 /* Default Schur mode of the handle (used by lvb_ba_reduced_system and by lvb_ba_solve(options == NULL)): 0 = FP64
- * CUDA-core elimination (parity reference), 1 = tcgen05 split-bf16 contraction with FP32 accumulation in TMEM, taken
+ * CUDA-core elimination (parity reference), 1 = wgmma split-bf16 contraction with FP32 accumulation in registers, taken
  * only when 6 x (free poses) <= 128 on a single GPU, else the handle silently stays on mode 0. */
 LVB_API int lvb_ba_set_schur_mode(lvb_ba* ba, int mode);
 LVB_API int lvb_ba_solve(lvb_ba* ba, const lvb_solve_options* options, lvb_solve_summary* summary);

@@ -334,7 +334,7 @@ inline void Solve(const Solver::Options& options, Problem* problem, Solver::Summ
     // PoseGraphError / PoseError): dense LM on the host, host_solver.h.  A problem with any reprojection / IMU / scan-to-map
     // block never goes there.
     if (has_other) {
-        if (has_device || scan) return fail("generic cost functions cannot be mixed with the device factor kinds of the B200 path");
+        if (has_device || scan) return fail("generic cost functions cannot be mixed with the device factor kinds of the CUDA path");
         return lvb::host::solve(options, problem, summary);
     }
     (void)has_hostable;

@@ -1,6 +1,6 @@
 """ctypes binding of the C ABI in include/lvio_b200.h.
 
-The product library is ``lvio_fusion_b200/csrc/liblvio_b200.so`` (CUDA, sm_100a).  There is
+The product library is ``lvio_fusion_b200/csrc/liblvio_b200.so`` (CUDA, sm_90a).  There is
 no CPU fallback: if the library is missing or no device is usable the calls raise.
 
 The signature table is prefix-agnostic so that ``oracle/binding.py`` (test infrastructure)

@@ -156,7 +156,7 @@ class Problem:
         self.api.check(self.api.ba_set_loss(self.h, kind, float(huber_a)), "ba_set_loss")
 
     def set_schur_mode(self, mode):
-        """0 = FP64 Schur (parity reference), 1 = tcgen05 split-bf16 tensor-core Schur (CUDA library only)."""
+        """0 = FP64 Schur (parity reference), 1 = wgmma split-bf16 tensor-core Schur (CUDA library only)."""
         self.api.check(self.api.ba_set_schur_mode(self.h, int(mode)), "ba_set_schur_mode")
 
     def finalize(self):

@@ -53,8 +53,8 @@ struct BaDev {
     const int *tf_slot;                 // 2 planes: slot of pose_1 / pose_2 inside the landmark's Schur group (-1: constant pose)
     const int *sw_group, *sw_lm, *grp_ns, *grp_off;   // Schur warps: group id, 32 landmark ids (-1 pad); per group: #slots, offsets
     int n_schur_warps, warp_syrk;
-    int tc_mode;                        // 1: Schur contraction on the tensor cores (tcgen05, split bf16), FP64 rhs only here
-    unsigned short* tc_u;               // packed U^T: [chunk of 16 landmarks][3 splits][128 x 16 bf16 UMMA K-major tile]
+    int tc_mode;                        // 1: Schur contraction on the tensor cores (wgmma, split bf16), FP64 rhs only here
+    unsigned short* tc_u;               // packed U^T: [chunk of 16 landmarks][3 splits][128 x 16 bf16 K-major core-matrix tile]
     const int* tc_cdim;                 // camera offset -> compact pose dimension (0..127) or -1
     const int* tc_off;                  // compact pose dimension -> camera offset
     int tc_ndim;                        // 6 * free poses (<= 128)
@@ -749,7 +749,7 @@ __global__ void __launch_bounds__(TPB) ba_schur_kernel(BaDev d, int cols_max) {
     const int* offs = d.grp_off + (size_t)g * MAX_TRACK;
     if (d.tc_mode) {
         // tensor-core mode: this warp only (a) adds its rhs column  sum_l u_l g_l / h_l  in FP64 and (b) writes its 32
-        // rows of U as three bf16 planes (x ~ hi + mid + lo, 24 mantissa bits) into the UMMA K-major tiles of its two
+        // rows of U as three bf16 planes (x ~ hi + mid + lo, 24 mantissa bits) into the K-major wgmma tiles of its two
         // 16-landmark chunks.  Positions outside the group's pose set were zeroed once at finalize and never change.
         for (int b = lane; b < ncol - 1; b += 32) {
             double v = 0.0;
@@ -792,89 +792,78 @@ __global__ void __launch_bounds__(TPB) ba_schur_kernel(BaDev d, int cols_max) {
 }
 
 // K5 on the tensor cores.  S_pose -= U^T U with U^T staged as bf16 split planes (hi, mid, lo); per 16-landmark chunk six
-// 128x128x16 UMMAs (hi.hi, hi.mid, mid.hi, mid.mid, hi.lo, lo.hi) accumulate in FP32 in TMEM, which keeps ~2^-23 of each
-// product; one CTA owns TC_CHUNKS chunks (a 256-landmark slice of K), so the FP32 accumulation stays short and the
-// cross-CTA sum happens in FP64 (red.global.add.f64 on the lower triangle).  The FP64 kernel above remains the parity
-// reference; this path is selected with lvb_solve_options.schur_mode = 1 when 6 * (free poses) <= 128.
+// products (hi.hi, hi.mid, mid.hi, mid.mid, hi.lo, lo.hi) accumulate in FP32 in registers, which keeps ~2^-23 of each
+// product.  One warpgroup issues wgmma.m64n128k16 for the two 64-row halves of the 128 x 128 result in turn (64 accumulator
+// registers per thread instead of 128); one CTA owns TC_CHUNKS chunks (a 256-landmark slice of K), so the FP32 accumulation
+// stays short and the cross-CTA sum happens in FP64 (red.global.add.f64 on the lower triangle).  The FP64 kernel above
+// remains the parity reference; this path is selected with lvb_solve_options.schur_mode = 1 when 6 * (free poses) <= 128.
 enum { TC_CHUNKS = 16, TC_TILE_BYTES = 4096, TC_CHUNK_BYTES = 3 * TC_TILE_BYTES };
 
-__device__ __forceinline__ uint64_t umma_smem_desc(uint32_t smem_addr) {
-    // SmemDescriptor (cute/arch/mma_sm100_desc.hpp): start >> 4 [0,14) | LBO >> 4 [16,30) | SBO >> 4 [32,46) | version 1 [46,48)
-    // | layout_type SWIZZLE_NONE (0) [61,64).  K-major canonical layout ((8,n),2):((1,SBO),LBO) in 16-byte units.
-    return (uint64_t)((smem_addr >> 4) & 0x3FFF) | ((uint64_t)(128 >> 4) << 16) | ((uint64_t)(256 >> 4) << 32) | ((uint64_t)1 << 46);
+__device__ __forceinline__ uint64_t gmma_smem_desc(uint32_t smem_addr) {
+    // sm_90 matrix descriptor: start >> 4 [0,14) | LBO >> 4 [16,30) | SBO >> 4 [32,46) | base offset 0 [49,52) | layout 0 = no
+    // swizzle [62,64).  K-major canonical layout ((8,m),2):((1,SBO),LBO) in 16-byte units: LBO = 128 B between the two 8-wide
+    // K core matrices, SBO = 256 B between 8-row groups.
+    return (uint64_t)((smem_addr >> 4) & 0x3FFF) | ((uint64_t)(128 >> 4) << 16) | ((uint64_t)(256 >> 4) << 32);
 }
-__device__ __forceinline__ void umma_bf16_ss(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\ttcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}\n"
-                 ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate) : "memory");
+// D[64 x 128] += A[64 x 16] . B[128 x 16]^T, both operands K-major bf16 in shared memory, D in FP32 registers, overwritten when accumulate == 0 (warpgroup layout:
+// thread t holds rows 16 (t / 32) + (t % 32) / 4 + {0, 8}, columns 8 n + 2 (t % 4) + {0, 1} in c[4 n + {0, 1}] / c[4 n + {2, 3}])
+__device__ __forceinline__ void wgmma_bf16_m64n128(float (&c)[64], uint64_t adesc, uint64_t bdesc, int accumulate) {
+    asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %66, 0;\nwgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, 0, 0;\n}\n"
+                 : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3]), "+f"(c[4]), "+f"(c[5]), "+f"(c[6]), "+f"(c[7]), "+f"(c[8]), "+f"(c[9]), "+f"(c[10]), "+f"(c[11]), "+f"(c[12]), "+f"(c[13]), "+f"(c[14]), "+f"(c[15]), "+f"(c[16]), "+f"(c[17]), "+f"(c[18]), "+f"(c[19]), "+f"(c[20]), "+f"(c[21]), "+f"(c[22]), "+f"(c[23]), "+f"(c[24]), "+f"(c[25]), "+f"(c[26]), "+f"(c[27]), "+f"(c[28]), "+f"(c[29]), "+f"(c[30]), "+f"(c[31]), "+f"(c[32]), "+f"(c[33]), "+f"(c[34]), "+f"(c[35]), "+f"(c[36]), "+f"(c[37]), "+f"(c[38]), "+f"(c[39]), "+f"(c[40]), "+f"(c[41]), "+f"(c[42]), "+f"(c[43]), "+f"(c[44]), "+f"(c[45]), "+f"(c[46]), "+f"(c[47]), "+f"(c[48]), "+f"(c[49]), "+f"(c[50]), "+f"(c[51]), "+f"(c[52]), "+f"(c[53]), "+f"(c[54]), "+f"(c[55]), "+f"(c[56]), "+f"(c[57]), "+f"(c[58]), "+f"(c[59]), "+f"(c[60]), "+f"(c[61]), "+f"(c[62]), "+f"(c[63])
+                 : "l"(adesc), "l"(bdesc), "r"(accumulate) : "memory");
 }
 
 __global__ void __launch_bounds__(128) ba_schur_tc_kernel(BaDev d, int n_chunks) {
     extern __shared__ __align__(1024) unsigned char smem_raw[];
-    __shared__ __align__(8) uint64_t bar_load, bar_mma;
-    __shared__ uint32_t tmem_base_slot;
+    __shared__ __align__(8) uint64_t bar_load;
     if (d.st->done) return;
-    const int tid = threadIdx.x, warp = tid >> 5;
+    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int c0 = blockIdx.x * TC_CHUNKS;
     const int nc = min(TC_CHUNKS, n_chunks - c0);
-    if (tid == 0) { mbar_init(&bar_load, 1); mbar_init(&bar_mma, 1); }
-    if (warp == 0) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&tmem_base_slot)), "r"(128) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
+    if (tid == 0) mbar_init(&bar_load, 1);
     __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const uint32_t tmem_d = tmem_base_slot;
     if (tid == 0) {
         // TMA 1-D bulk copies of this CTA's chunks (contiguous in HBM), one mbarrier transaction
         mbar_expect_tx(&bar_load, (uint32_t)nc * TC_CHUNK_BYTES);
         const unsigned char* src = reinterpret_cast<const unsigned char*>(d.tc_u) + (size_t)c0 * TC_CHUNK_BYTES;
         for (int c = 0; c < nc; ++c) bulk_load_1d(smem_raw + (size_t)c * TC_CHUNK_BYTES, src + (size_t)c * TC_CHUNK_BYTES, TC_CHUNK_BYTES, &bar_load);
-        mbar_wait(&bar_load, 0);
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        // InstrDescriptor: D = F32 (1 << 4), A = B = BF16 (1 << 7, 1 << 10), both K-major, N = 128 (>> 3 at bit 17), M = 128 (>> 4 at bit 24)
-        const uint32_t idesc = (1u << 4) | (1u << 7) | (1u << 10) | ((128u >> 3) << 17) | ((128u >> 4) << 24);
-        const uint32_t base = smem_u32(smem_raw);
-        uint32_t acc = 0;
-        for (int c = 0; c < nc; ++c) {
-            const uint64_t hi = umma_smem_desc(base + c * TC_CHUNK_BYTES), mid = umma_smem_desc(base + c * TC_CHUNK_BYTES + TC_TILE_BYTES),
-                           lo = umma_smem_desc(base + c * TC_CHUNK_BYTES + 2 * TC_TILE_BYTES);
-            umma_bf16_ss(tmem_d, hi, hi, idesc, acc); acc = 1;
-            umma_bf16_ss(tmem_d, hi, mid, idesc, 1); umma_bf16_ss(tmem_d, mid, hi, idesc, 1);
-            umma_bf16_ss(tmem_d, mid, mid, idesc, 1);
-            umma_bf16_ss(tmem_d, hi, lo, idesc, 1); umma_bf16_ss(tmem_d, lo, hi, idesc, 1);
-        }
-        asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(&bar_mma)) : "memory");
     }
-    // epilogue: thread t owns accumulator row t (TMEM lane t): FP32 -> FP64, subtract from the lower triangle of S
-    mbar_wait(&bar_mma, 0);
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const int a = tid;
-    const int ga = a < d.tc_ndim ? d.tc_off[a] : -1;
-    for (int cb = 0; cb < 128; cb += 32) {
-        uint32_t v[32];
-        const uint32_t taddr = tmem_d + ((uint32_t)(warp * 32) << 16) + (uint32_t)cb;
-        asm volatile("tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-                     : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]),
-                       "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]), "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]),
-                       "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-                     : "r"(taddr) : "memory");
-        asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-        if (ga >= 0) {
+    mbar_wait(&bar_load, 0);
+    const uint32_t base = smem_u32(smem_raw);
+    const int ndim = d.tc_ndim;
+    for (int mh = 0; mh < 2 && 64 * mh < ndim; ++mh) {
+        float acc[64];                                  // the first product overwrites it (scale-d = 0)
+        asm volatile("wgmma.fence.sync.aligned;" ::: "memory");
+        for (int c = 0; c < nc; ++c) {
+            const uint32_t cb = base + c * TC_CHUNK_BYTES, ab = cb + mh * 2048;      // rows 64 mh.. of the tile: 8 row groups of 256 B
+            const uint64_t a_hi = gmma_smem_desc(ab), a_mid = gmma_smem_desc(ab + TC_TILE_BYTES), a_lo = gmma_smem_desc(ab + 2 * TC_TILE_BYTES);
+            const uint64_t b_hi = gmma_smem_desc(cb), b_mid = gmma_smem_desc(cb + TC_TILE_BYTES), b_lo = gmma_smem_desc(cb + 2 * TC_TILE_BYTES);
+            wgmma_bf16_m64n128(acc, a_hi, b_hi, c > 0);
+            wgmma_bf16_m64n128(acc, a_hi, b_mid, 1); wgmma_bf16_m64n128(acc, a_mid, b_hi, 1);
+            wgmma_bf16_m64n128(acc, a_mid, b_mid, 1);
+            wgmma_bf16_m64n128(acc, a_hi, b_lo, 1); wgmma_bf16_m64n128(acc, a_lo, b_hi, 1);
+        }
+        asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory");
+        asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory");
+        // epilogue: FP32 -> FP64, subtract from the lower triangle of S (compact order)
 #pragma unroll
-            for (int j = 0; j < 32; ++j) {
-                const int b = cb + j;
-                if (b > a || b >= d.tc_ndim) continue;              // lower triangle in compact order
-                const float f = __uint_as_float(v[j]);
-                if (f == 0.0f) continue;
-                const int gb = d.tc_off[b];
-                if (ga >= gb) atomicAdd(&d.S[SIDX(d, ga, gb)], -(double)f); else atomicAdd(&d.S[SIDX(d, gb, ga)], -(double)f);
+        for (int i = 0; i < 2; ++i) {
+            const int a = 64 * mh + 16 * warp + (lane >> 2) + 8 * i;
+            if (a >= ndim) continue;
+            const int ga = d.tc_off[a];
+#pragma unroll
+            for (int n = 0; n < 16; ++n) {
+#pragma unroll
+                for (int j = 0; j < 2; ++j) {
+                    const int b = 8 * n + 2 * (lane & 3) + j;
+                    const float f = acc[4 * n + 2 * i + j];
+                    if (b > a || b >= ndim || f == 0.0f) continue;
+                    const int gb = d.tc_off[b];
+                    if (ga >= gb) atomicAdd(&d.S[SIDX(d, ga, gb)], -(double)f); else atomicAdd(&d.S[SIDX(d, gb, ga)], -(double)f);
+                }
             }
         }
     }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    if (warp == 0) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_d), "r"(128) : "memory");
 }
 
 __global__ void ba_pack_scalars_kernel(BaDev d) {
@@ -2480,7 +2469,7 @@ int lvb_ba_solve(lvb_ba* ba, const lvb_solve_options* options, lvb_solve_summary
 }
 
 int lvb_ba_set_schur_mode(lvb_ba* ba, int mode) {
-    if (mode != 0 && mode != 1) { set_error("schur_mode must be 0 (FP64) or 1 (tcgen05)"); return LVB_ERR_INVALID; }
+    if (mode != 0 && mode != 1) { set_error("schur_mode must be 0 (FP64) or 1 (tensor cores)"); return LVB_ERR_INVALID; }
     ba->schur_mode = mode;
     return LVB_OK;
 }

@@ -227,7 +227,7 @@ int lvb_ctx_create(int device, void* cuda_stream, lvb_ctx** out) {
     LVB_CUDA(cudaSetDevice(device));
     cudaDeviceProp prop;
     LVB_CUDA(cudaGetDeviceProperties(&prop, device));
-    if (prop.major < 10) { set_error("device %d is sm_%d%d; this library is built for sm_100a only", device, prop.major, prop.minor); return LVB_ERR_CUDA; }
+    if (prop.major != 9 || prop.minor != 0) { set_error("device %d is sm_%d%d; this library is built for sm_90a (H100) only", device, prop.major, prop.minor); return LVB_ERR_CUDA; }
     lvb_ctx* c = new lvb_ctx();
     c->device = device;
     c->sm_count = prop.multiProcessorCount;

@@ -27,7 +27,7 @@ struct lvb_ctx {
     cudaEvent_t ev_fork = nullptr, ev_join = nullptr;
     bool use_side = true;               // env LVB_NO_SIDE=1 disables
     long long launches = 0;
-    int sm_count = 148;
+    int sm_count = 132;
     bool use_tma = true;          // cp.async.bulk staging of the pose array (env LVB_NO_TMA=1 disables)
     bool use_graph = true;        // replay the LM pass as a CUDA graph (env LVB_NO_GRAPH=1 disables)
     int eval_variant = 0;         // A/B switch of the Jacobian-eval kernel (env LVB_EVAL_VARIANT)

@@ -1,4 +1,4 @@
-// lvb_math.cuh -- per-factor residual / Jacobian arithmetic of the B200 backend.
+// lvb_math.cuh -- per-factor residual / Jacobian arithmetic of the CUDA backend.
 //
 // Hand-derived closed forms (no autodiff on the hot path).  Everything is
 // __host__ __device__ so that tests/hostcheck can compile the very same functions with g++

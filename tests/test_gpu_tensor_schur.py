@@ -1,5 +1,5 @@
-"""schur_mode = 1: the landmark marginalisation S -= W^T D W on the tcgen05 tensor cores (bf16 x3 split operands, FP32
-accumulation in TMEM over 256-landmark slices, FP64 across slices), checked against the FP64 CUDA-core path that
+"""schur_mode = 1: the landmark marginalisation S -= W^T D W on the tensor cores (wgmma, bf16 x3 split operands, FP32
+accumulation in registers over 256-landmark slices, FP64 across slices), checked against the FP64 CUDA-core path that
 carries the parity claims.  Stated tolerance: 2e-5 of max|S| on the reduced system (2^-23 per product plus FP32
 accumulation), 1e-5 relative on the converged cost, 1e-5 on poses -- the gradient side (rhs) stays FP64, so the
 fixed point of the LM iteration is unchanged and only the step direction is perturbed."""

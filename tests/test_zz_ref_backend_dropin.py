@@ -214,7 +214,7 @@ def test_reference_mapping_optimize_drives_the_cuda_path(tmp_path):
 @pytest.mark.gpu
 @pytest.mark.parametrize("mode", [0, 1, 2, 3, 4])
 def test_reference_backend_drives_the_cuda_path(mode, tmp_path):
-    """The same binaries on the B200: the reference's Backend::BuildProblem / adapt::Solve / imu::FullBA through the shim on
+    """The same binaries on the GPU: the reference's Backend::BuildProblem / adapt::Solve / imu::FullBA through the shim on
     liblvio_b200.so, against the oracle-served run of the identical problem."""
     fo, fg = str(tmp_path / "orc.bin"), str(tmp_path / "lvb.bin")
     o, g = _run("ref_backend_orc", mode, fo), _run("ref_backend_lvb", mode, fg)
@@ -244,7 +244,7 @@ def test_reference_backend_drives_the_cuda_path(mode, tmp_path):
 
 @pytest.mark.gpu
 def test_shim_solves_from_two_threads_on_the_device(tmp_path):
-    """tests/test_capi_cpu.py::test_shim_solves_from_several_threads_at_once on the B200: two host threads, each with its own
+    """tests/test_capi_cpu.py::test_shim_solves_from_several_threads_at_once on the GPU: two host threads, each with its own
     per-thread context and stream (graph capture is thread-local), solve the same window at once; both must equal the single-threaded
     result.  Bounded by a timeout so that a wedged run cannot hold the box."""
     import shim_util

@@ -1,5 +1,5 @@
 // Cycles and accuracy of the 32 x 32 diagonal-block factorisations in lvb_chol.cuh (one warp), and of the panel-row solve.
-// build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o diag_probe diag_probe.cu
+// build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o diag_probe diag_probe.cu
 #include <cstdio>
 #include <cmath>
 #include <vector>

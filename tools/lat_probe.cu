@@ -1,5 +1,5 @@
-// Dependent-issue latencies of the instructions in the pivot chain of the diagonal-block Cholesky (one warp, sm_100a).
-// build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o lat_probe lat_probe.cu ; run on the GPU box
+// Dependent-issue latencies of the instructions in the pivot chain of the diagonal-block Cholesky (one warp, sm_90a).
+// build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o lat_probe lat_probe.cu ; run on the GPU box
 #include <cstdio>
 #include <cmath>
 #include <cuda_runtime.h>
