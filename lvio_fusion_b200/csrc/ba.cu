@@ -18,10 +18,10 @@
 #include <math.h>
 #include <algorithm>
 #include <chrono>
-#include <functional>
 #include <map>
 #include <string.h>
 #include <cuda_bf16.h>
+#include "ba_plan.h"
 #include "lvb_internal.cuh"
 #include "lvb_math.cuh"
 #include "lvb_imu_warp.cuh"
@@ -32,7 +32,7 @@ using namespace lvb;
 
 namespace {
 
-enum { TPB = 128, IMU_STRIDE = 17 + 45 + 225 + 1, IMU_RAW = 469, MAX_DIMC = 736, MAX_STAGE_POSES = 512, MAX_TRACK = 16, CHOL_T = 256, SYRK_ROWS = 64, SYRK_LD = 14 };
+enum { TPB = 128, IMU_STRIDE = 17 + 45 + 225 + 1, MAX_STAGE_POSES = 512, SYRK_ROWS = 64, SYRK_LD = 14 };
 
 __device__ long long g_chol_dbg[8];     // accumulated SM clocks per Cholesky phase (diag, panel, trailing, backward, total)
 __device__ unsigned char c_tri_a[465];   // lower-triangle enumeration e -> (a, b), a >= b; global (not __constant__):
@@ -1007,7 +1007,6 @@ __global__ void lm_control_pre_kernel(LmState* st) { lm_control_pre(*st); }
 //                everything but diagonal block k + 1
 // so the pivot chain of block k + 1 overlaps the panel and the trailing update of step k instead of following them.
 #define SA(i_, j_) S[(size_t)(i_) * (size_t)srow + (size_t)(j_) + (size_t)soff]
-enum { CHOL_DT = 32 * 34 + 32, CHOL_HDR = 2 * CHOL_DT };        // doubles: (Dt, invd) twice, then the panel
 __global__ void __launch_bounds__(CHOL_T) ba_cholesky_kernel(double* __restrict__ S, double* __restrict__ rhs, int n, long long srow, long long soff,
                                                                   double* __restrict__ invd_g, LmState* st, int run_control_pre,
                                                                   const int* __restrict__ env_rmax, const int* __restrict__ env_cmin) {
@@ -1367,9 +1366,7 @@ __global__ void ba_reproj_error_kernel(BaDev d, int n, const double* __restrict_
 // ====================================================================================== host side
 struct lvb_ba {
     lvb_ctx* ctx = nullptr;
-    bool finalized = false, solvable = false;
-    const char* unsolvable_why = "the problem has no free camera parameter";
-    long long srow = 0, soff = 0; size_t nS = 1, chol_smem = 0; int band = 0, panel_rows = 2;
+    bool finalized = false;
     DevBuf<double> chol_invd;
     double cam[22];
     bool have_cam = false;
@@ -1379,24 +1376,15 @@ struct lvb_ba {
     std::vector<double> h_fc[6];
     std::vector<int32_t> h_fi[6];
     int n[6] = {0, 0, 0, 0, 0, 0};      // blocks as added by the caller
-    int nd[6] = {0, 0, 0, 0, 0, 0};     // blocks in the device layout (kinds 0/1: sorted by pose key, each key padded to 32)
-    std::vector<int> order[6];          // device position -> caller index, -1 for padding
     double huber[6] = {0, 0, 0, 0, 0, 0};
-    int dimc = 0, n_pose_free = 0, n_vec3_free = 0, n_rho_free = 0;
-    std::vector<int> canon;             // internal camera-system offset -> canonical (poses first, then vec3) offset
+    BaPlan plan;                        // structure, device order, storage and solver of the last finalize (ba_plan.h)
     DevBuf<int> chol_rmax, chol_cmin;   // envelope of S per 32-column block step
-    // multifrontal tree over the banded system (ba_tree.cuh); tree_levels == 0: single-CTA envelope Cholesky
-    DevBuf<Front> fronts; DevBuf<double> front_pool;
-    std::vector<int> level_first, level_count;
-    int tree_levels = 0; size_t tree_factor_smem = 0, tree_back_smem = 0;
-    bool wide_solver = false;           // envelope too wide for the one-CTA panel and no tree: per-phase grids over S in global memory (ba_wide.cuh)
-    std::vector<int> h_rmax;            // host copy of the envelope (launch geometry of the wide solver)
+    DevBuf<Front> fronts; DevBuf<double> front_pool;      // multifrontal tree over the banded system (ba_tree.cuh)
     // device
     DevBuf<unsigned char> upload_arena;      // one allocation for everything finalize uploads (the buffers below are views into it)
     DevBuf<double> poses, vec3, rho, c_poses, c_vec3, c_rho;
     DevBuf<int> pose_off, vec3_off, rho_slot, lm_start, lm_fac;
     DevBuf<int> tf_slot, sw_group, sw_lm, grp_ns, grp_off;
-    int n_schur_warps = 0, schur_cols_max = 0;
     size_t schur_smem = 0, lin_smem = 0;
     cudaGraphExec_t pass_graph = nullptr;
     bool graph_borrowed = false;        // pass_graph is the context's cached exec (never destroyed from here)
@@ -1404,7 +1392,7 @@ struct lvb_ba {
     bool capturing = false;
     bool imu_checked = true;
     // tensor-core Schur (schur_mode 1)
-    bool tc_ok = false; int schur_mode = 0, graph_mode = -1, n_tc_chunks = 0;
+    int schur_mode = 0, graph_mode = -1, n_tc_chunks = 0;
     DevBuf<unsigned short> tc_u; DevBuf<int> tc_cdim, tc_off;
     int solves_done = 0;
     DevBuf<double> fc[6];
@@ -1427,8 +1415,6 @@ static void drop_graph(lvb_ba* ba) {
     ba->pass_graph = nullptr; ba->graph_borrowed = false;
 }
 
-static const int kConstStride[6] = {5, 6, 5, IMU_RAW, 8, 9};
-static const int kIdxStride[6] = {3, 1, 1, 8, 2, 1};
 static const int kResDim[6] = {2, 2, 2, 15, 6, 6};
 static const int kJacCols[6] = {15, 7, 1, 32, 14, 7};
 
@@ -1439,8 +1425,8 @@ static int init_tables() {
     for (int i = 0; i < 30; ++i) for (int j = 0; j <= i; ++j) { a[e] = (unsigned char)i; b[e] = (unsigned char)j; ++e; }
     LVB_CUDA(cudaMemcpyToSymbol(c_tri_a, a, sizeof(a)));
     LVB_CUDA(cudaMemcpyToSymbol(c_tri_b, b, sizeof(b)));
-    LVB_CUDA(cudaFuncSetAttribute(ba_cholesky_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024 - 256));
-    LVB_CUDA(cudaFuncSetAttribute(ba_front_factor_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024 - 256));
+    LVB_CUDA(cudaFuncSetAttribute(ba_cholesky_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, MAX_CTA_SMEM));
+    LVB_CUDA(cudaFuncSetAttribute(ba_front_factor_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, MAX_CTA_SMEM));
     LVB_CUDA(cudaFuncSetAttribute(ba_front_backward_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 64 * 1024));
     LVB_CUDA(cudaFuncSetAttribute(ba_eval_two_frame_kernel<1, 5>, cudaFuncAttributeMaxDynamicSharedMemorySize, (TPB * 31 + MAX_STAGE_POSES * 7 + 2) * 8));
     LVB_CUDA(cudaFuncSetAttribute(ba_eval_two_frame_kernel<1, 6>, cudaFuncAttributeMaxDynamicSharedMemorySize, (TPB * 31 + MAX_STAGE_POSES * 7 + 2) * 8));
@@ -1460,64 +1446,9 @@ static inline int nblk(size_t n, int per) { return (int)((n + per - 1) / per); }
 static void mark(struct lvb_ba* ba, const char* name);
 #define LAUNCH_ON(ba, stream_, kernel, grid, block, smem, ...)                             \
     do { if ((grid) > 0) { kernel<<<(grid), (block), (smem), (stream_)>>>(__VA_ARGS__); (ba)->ctx->launches++; } } while (0)
-#define LAUNCH(ba, kernel, grid, block, smem, ...)                                        \
-    do { if ((grid) > 0) { kernel<<<(grid), (block), (smem), (ba)->ctx->stream>>>(__VA_ARGS__); (ba)->ctx->launches++; mark(ba, #kernel); } } while (0)
-
-// Separator tree of the banded reduced system (see ba_tree.cuh): complete binary tree with 2^D leaves, separators of width
-// w = true half bandwidth.  Leaves keep >= 2w unknowns so that a separator is coupled to nothing beyond its two neighbouring subtrees.
-static int build_front_tree(int n, int band, int sep, int max_leaves, std::vector<Front>& out, std::vector<int>& level_first, std::vector<int>& level_count,
-                            size_t& pool_doubles, int& max_panel_rows, int& max_nb) {
-    out.clear(); level_first.clear(); level_count.clear(); pool_doubles = 0; max_panel_rows = 0; max_nb = 0;
-    // separator width: the TRUE half bandwidth is enough to separate (the storage band carries up to 31 columns of block-step slack);
-    // a front's cost grows with the cube of it
-    static const bool sep_is_band = getenv("LVB_TREE_SEP_BAND") && getenv("LVB_TREE_SEP_BAND")[0] == '1';      // A/B switch
-    const int w = sep_is_band ? band : std::max(1, std::min(sep, band));
-    int D = 0;
-    while ((1 << (D + 1)) <= max_leaves) {
-        const long long P = 1ll << (D + 1);
-        const long long leaf = ((long long)n - (P - 1) * w) / P;
-        if (leaf < 2ll * w || leaf < 64) break;
-        ++D;
-    }
-    if (D == 0) return 0;
-    struct Node { int o0, m, bL0, wL, bR0, wR, c0, c1, h; };
-    std::vector<Node> nodes;
-    std::function<int(int, int, int, int, int, int, int)> rec = [&](int a, int b, int depth, int bL0, int wL, int bR0, int wR) -> int {
-        if (depth == D) { nodes.push_back({a, b - a, bL0, wL, bR0, wR, -1, -1, 0}); return (int)nodes.size() - 1; }
-        const int s0 = a + (b - a - w) / 2;
-        const int c0 = rec(a, s0, depth + 1, bL0, wL, s0, w);
-        const int c1 = rec(s0 + w, b, depth + 1, s0, w, bR0, wR);
-        nodes.push_back({s0, w, bL0, wL, bR0, wR, c0, c1, D - depth});
-        return (int)nodes.size() - 1;
-    };
-    rec(0, n, 0, 0, 0, 0, 0);
-    std::vector<int> ids(nodes.size()), new_id(nodes.size());
-    for (size_t i = 0; i < ids.size(); ++i) ids[i] = (int)i;
-    std::stable_sort(ids.begin(), ids.end(), [&](int a, int b) { return nodes[a].h != nodes[b].h ? nodes[a].h < nodes[b].h : nodes[a].o0 < nodes[b].o0; });
-    for (size_t i = 0; i < ids.size(); ++i) new_id[ids[i]] = (int)i;
-    level_first.assign(D + 1, 0); level_count.assign(D + 1, 0);
-    for (size_t i = 0; i < ids.size(); ++i) {
-        const Node& nd = nodes[ids[i]];
-        Front F;
-        F.o0 = nd.o0; F.m = nd.m; F.wL = nd.wL; F.wR = nd.wR; F.bL0 = nd.bL0; F.bR0 = nd.bR0;
-        F.actR = nd.h == 0 ? std::max(0, nd.m - band) : 0;
-        F.child0 = nd.c0 < 0 ? -1 : new_id[nd.c0]; F.child1 = nd.c1 < 0 ? -1 : new_id[nd.c1];
-        F.parent = -1; F.side = 0;
-        F.nb = nd.wL + nd.wR; F.ld = (nd.m + F.nb + 1) & ~1;
-        F.bd = (long long)pool_doubles;
-        pool_doubles += ((size_t)(F.nb + 1) * F.ld + 1) & ~(size_t)1;
-        if (level_count[nd.h] == 0) level_first[nd.h] = (int)i;
-        level_count[nd.h]++;
-        max_nb = std::max(max_nb, F.nb);
-        max_panel_rows = std::max(max_panel_rows, std::min(nd.m, band) + F.nb + 1);
-        out.push_back(F);
-    }
-    for (size_t i = 0; i < out.size(); ++i) {
-        if (out[i].child0 >= 0) { out[out[i].child0].parent = (int)i; out[out[i].child0].side = 0; }
-        if (out[i].child1 >= 0) { out[out[i].child1].parent = (int)i; out[out[i].child1].side = 1; }
-    }
-    return D + 1;
-}
+#define LAUNCH_AS(ba, name, kernel, grid, block, smem, ...)                               \
+    do { if ((grid) > 0) { kernel<<<(grid), (block), (smem), (ba)->ctx->stream>>>(__VA_ARGS__); (ba)->ctx->launches++; mark(ba, name); } } while (0)
+#define LAUNCH(ba, kernel, grid, block, smem, ...) LAUNCH_AS(ba, #kernel, kernel, grid, block, smem, __VA_ARGS__)
 
 static void mark(lvb_ba* ba, const char* name) { lvb::timing_mark(ba->ctx->stream, name); }
 #define g_timing lvb::g_timing
@@ -1668,6 +1599,21 @@ int lvb_ba_set_loss(lvb_ba* ba, int kind, double a) {
     return LVB_OK;
 }
 
+// the plan-shaping A/B switches, read once per process
+static bool no_tree_switch() { static const bool on = getenv("LVB_NO_TREE") && getenv("LVB_NO_TREE")[0] == '1'; return on; }
+static bool tree_sep_band_switch() { static const bool on = getenv("LVB_TREE_SEP_BAND") && getenv("LVB_TREE_SEP_BAND")[0] == '1'; return on; }
+
+// element-wise collective over a host array of a sharded problem: through the device, like every all-reduce
+static int allreduce_host_i32(lvb_ctx* ctx, std::vector<int>& v, int (*op)(lvb_ctx*, int*, size_t)) {
+    cudaStream_t s = ctx->stream;
+    DevBuf<int> tmp;
+    LVB_TRY(tmp.upload(v.data(), v.size(), s));
+    LVB_TRY(op(ctx, tmp.p, v.size()));
+    LVB_CUDA(cudaMemcpyAsync(v.data(), tmp.p, v.size() * sizeof(int), cudaMemcpyDeviceToHost, s));
+    LVB_CUDA(cudaStreamSynchronize(s));
+    return LVB_OK;
+}
+
 int lvb_ba_finalize(lvb_ba* ba) {
     static const bool prof_on = getenv("LVB_PROFILE") != nullptr;
     auto prof_t = std::chrono::steady_clock::now();
@@ -1676,340 +1622,63 @@ int lvb_ba_finalize(lvb_ba* ba) {
     ba->host_fresh = false;
     LVB_CUDA(cudaSetDevice(ctx->device)); lvb::g_alloc_stream = ctx->stream;
     cudaStream_t s = ctx->stream;
+    if (!ba->have_cam) { set_error("cameras not set"); return LVB_ERR_STATE; }
+    const int np = (int)ba->h_poses.size() / 7, nv = (int)ba->h_vec3.size() / 3, nr = (int)ba->h_rho.size();
+    // ---- plan (ba_plan.h): host arithmetic on the index arrays
+    BaProblemView in;
+    in.np = np; in.nv = nv; in.nr = nr;
+    in.pose_const = ba->h_pose_const.data(); in.vec3_const = ba->h_vec3_const.data(); in.rho_const = ba->h_rho_const.data();
+    for (int k = 0; k < 6; ++k) { in.n[k] = ba->n[k]; in.fc[k] = ba->h_fc[k].data(); in.fi[k] = ba->h_fi[k].data(); }
+    PlanHooks hooks;
+    hooks.max_reduce = [ctx](std::vector<int>& v) { return allreduce_host_i32(ctx, v, comm_allreduce_max_i32); };
+    hooks.min_reduce = [ctx](std::vector<int>& v) { return allreduce_host_i32(ctx, v, comm_allreduce_min_i32); };
+    hooks.phase_done = [&](const char* name) { PROF(name); };
+    BaPlan& P = ba->plan;
+    std::string err;
+    if (int rc = plan_ba(in, ctx->sm_count, ctx->world, no_tree_switch(), tree_sep_band_switch(), hooks, P, err)) {
+        if (!err.empty()) set_error("%s", err.c_str());
+        return rc;
+    }
+    const int npf = P.n_pose_free;
+
+    // ---- upload
     size_t stage_estimate = (ba->h_poses.size() + ba->h_vec3.size() + ba->h_rho.size()) * 24;
     for (int k = 0; k < 6; ++k) stage_estimate += ba->h_fc[k].size() * 8 + ba->h_fi[k].size() * 12;
     Stager stg(ctx, stage_estimate);
     LVB_TRY(stg.begin());
-    if (!ba->have_cam) { set_error("cameras not set"); return LVB_ERR_STATE; }
-    const int np = (int)ba->h_poses.size() / 7, nv = (int)ba->h_vec3.size() / 3, nr = (int)ba->h_rho.size();
-    // validate indices (the TwoFrame list is the long one: a branch-free pass; the other kinds through the general rule)
-    {
-        const int32_t* ix = ba->h_fi[0].data();
-        int bad = 0;
-        for (int f = 0; f < ba->n[0]; ++f, ix += 3) bad |= ((unsigned)ix[0] >= (unsigned)nr) | ((unsigned)ix[1] >= (unsigned)np) | ((unsigned)ix[2] >= (unsigned)np);
-        for (int k = bad ? 0 : 1; k < 6; ++k) for (int f = 0; f < ba->n[k]; ++f) for (int j = 0; j < kIdxStride[k]; ++j) {
-            const int v = ba->h_fi[k][(size_t)f * kIdxStride[k] + j];
-            int lim = np;
-            if ((k == 0 && j == 0) || k == 2) lim = nr;
-            if (k == 3 && j != 0 && j != 4) lim = nv;
-            if (k == 3 && (j == 6 || j == 7) && v == -1 && ba->h_fc[3][(size_t)f * IMU_RAW + 467] >= 0.0) continue;     // ImuInitError has no j-side bias blocks
-            if (v < 0 || v >= lim) { set_error("factor kind %d block %d: index %d out of range [0,%d)", k, f, v, lim); return LVB_ERR_INVALID; }
-        }
-    }
-    PROF("validate");
-    // slots / offsets.  Unknowns of the reduced camera system are ordered keyframe by keyframe
-    // (pose_i, then the velocity / bias blocks an ImuError ties to pose_i): co-visibility and the IMU chain only
-    // couple neighbouring keyframes, so S is block-banded and the Cholesky works inside its envelope.
-    // `canon` is the caller-visible order (all poses, then all vec3 blocks) used by lvb_ba_reduced_system.
-    std::vector<int> pose_off(np, -1), vec3_off(nv, -1), rho_slot(nr);
-    int npf = 0, nvf = 0, nrf = 0;
-    for (int i = 0; i < np; ++i) if (!ba->h_pose_const[i]) ++npf;
-    for (int i = 0; i < nv; ++i) if (!ba->h_vec3_const[i]) ++nvf;
-    for (int i = 0; i < nr; ++i) rho_slot[i] = ba->h_rho_const[i] ? -1 : nrf++;
-    ba->n_pose_free = npf; ba->n_vec3_free = nvf; ba->n_rho_free = nrf; ba->dimc = 6 * npf + 3 * nvf;
-    struct Blk { long long key; int type, idx, width; };
-    std::vector<Blk> blks;
-    {
-        std::vector<int> vkey(nv, -1);
-        if ((long long)np * 8 >= (1ll << 31)) { set_error("too many poses"); return LVB_ERR_UNSUPPORTED; }
-        for (int f = 0; f < ba->n[3]; ++f) {
-            const int32_t* ix = &ba->h_fi[3][8 * (size_t)f];
-            for (int b = 1; b < 8; ++b) { if (b == 4) continue; const int v = ix[b]; if (v < 0) continue; const int p = ix[b < 4 ? 0 : 4]; if (vkey[v] < 0) vkey[v] = p * 8 + (b & 3); }
-        }
-        // sharded problems: a rank only sees the IMU factors it owns, but the order of the unknowns (= the layout of the
-        // all-reduced system) must be the same on every rank: take the key any rank found (collective, like the envelope)
-        if (ctx->world > 1 && nv > 0) {
-            DevBuf<int> tmp;
-            LVB_TRY(tmp.upload(vkey.data(), vkey.size(), s));
-            LVB_TRY(comm_allreduce_max_i32(ctx, tmp.p, vkey.size()));
-            LVB_CUDA(cudaMemcpyAsync(vkey.data(), tmp.p, vkey.size() * sizeof(int), cudaMemcpyDeviceToHost, s));
-            LVB_CUDA(cudaStreamSynchronize(s));
-        }
-        for (int i = 0; i < np; ++i) if (!ba->h_pose_const[i]) blks.push_back({(long long)i * 8, 0, i, 6});
-        for (int i = 0; i < nv; ++i) if (!ba->h_vec3_const[i]) blks.push_back({vkey[i] >= 0 ? (long long)vkey[i] : (long long)np * 8 + i, 1, i, 3});
-        std::stable_sort(blks.begin(), blks.end(), [](const Blk& a, const Blk& b) { return a.key < b.key; });
-    }
-    std::vector<int> blk_of_off(ba->dimc, 0), blk_start(blks.size() + 1, 0);
-    ba->canon.assign(ba->dimc, 0);
-    {
-        int off = 0, ps = 0, vs = 0;
-        std::vector<int> pslot(np, -1), vslot(nv, -1);
-        for (int i = 0; i < np; ++i) if (!ba->h_pose_const[i]) pslot[i] = ps++;
-        for (int i = 0; i < nv; ++i) if (!ba->h_vec3_const[i]) vslot[i] = vs++;
-        for (size_t b = 0; b < blks.size(); ++b) {
-            blk_start[b] = off;
-            const int c0 = blks[b].type == 0 ? 6 * pslot[blks[b].idx] : 6 * npf + 3 * vslot[blks[b].idx];
-            if (blks[b].type == 0) pose_off[blks[b].idx] = off; else vec3_off[blks[b].idx] = off;
-            for (int k = 0; k < blks[b].width; ++k) { blk_of_off[off + k] = (int)b; ba->canon[off + k] = c0 + k; }
-            off += blks[b].width;
-        }
-        blk_start[blks.size()] = off;
-    }
-    PROF("block order");
-    // camera systems up to MAX_DIMC use dense lower-triangular storage, larger ones banded storage (decided below)
-    const bool dense_layout = ba->dimc <= MAX_DIMC;
-    ba->solvable = ba->dimc > 0;
-    // ---- device order of the blocks.  TwoFrame blocks sorted by (pose_1, pose_2), PoseOnly blocks by pose, so that
-    // a warp of the linearize kernel owns one key (or a few key segments) and can reduce its J^T J in shared memory
-    // before touching HBM.  Dense-layout (window-sized) problems also pad every key run to a multiple of 32 with
-    // weight-0 copies: one segment per warp.  Large problems stay unpadded (their runs are short, padding would
-    // inflate the block arrays).
-    for (int k = 0; k < 6; ++k) {
-        std::vector<int>& ord = ba->order[k];
-        ord.clear();
-        const int n = ba->n[k];
-        if (ba->solvable && (k == 0 || k == 1) && n > 0) {
-            // stable order by key: counting sort when the key space is small (window-sized problems), else a pair sort
-            std::vector<long long> keys(n);
-            const long long key_space = (k == 0) ? (long long)np * np : (long long)np;
-            for (int f = 0; f < n; ++f) keys[f] = (k == 0) ? (long long)ba->h_fi[0][3 * (size_t)f + 1] * np + ba->h_fi[0][3 * (size_t)f + 2] : (long long)ba->h_fi[1][f];
-            std::vector<int> ids(n);
-            if (key_space <= (1 << 16)) {
-                std::vector<int> start((size_t)key_space + 1, 0);
-                for (int f = 0; f < n; ++f) start[keys[f] + 1]++;
-                for (long long c = 0; c < key_space; ++c) start[c + 1] += start[c];
-                for (int f = 0; f < n; ++f) ids[start[keys[f]]++] = f;
-            } else {
-                std::vector<std::pair<long long, int>> kv(n);
-                for (int f = 0; f < n; ++f) kv[f] = {keys[f], f};
-                std::sort(kv.begin(), kv.end());
-                for (int f = 0; f < n; ++f) ids[f] = kv[f].second;
-            }
-            ord.reserve((size_t)n + 32 * 64);
-            for (int i = 0; i < n;) {
-                int j = i; while (j < n && keys[ids[j]] == keys[ids[i]]) ++j;
-                for (int t = i; t < j; ++t) ord.push_back(ids[t]);
-                while (dense_layout && ord.size() % 32) ord.push_back(-1 - ids[i]);     // padding: encoded source block
-                i = j;
-            }
-        } else { ord.resize(n); for (int f = 0; f < n; ++f) ord[f] = f; }
-        ba->nd[k] = (int)ord.size();
-    }
-    PROF("factor sort + pad");
-    const int n_tf = ba->nd[0];
-    // landmark CSR over device positions: TwoFrame i -> i, TwoCamera f -> -(f+1); padding is skipped.  The count runs over the caller's
-    // order (sequential); the fill has to follow the device order, so its gather is prefetched, and it also notes the two free-pose
-    // offsets of every entry (lm_off) so that the grouping below never goes back to the factor records.
-    std::vector<int> lm_start(nr + 1, 0);
-    {
-        const int32_t* ix = ba->h_fi[0].data();
-        for (int f = 0; f < ba->n[0]; ++f) lm_start[ix[3 * (size_t)f] + 1]++;
-    }
-    for (int f = 0; f < ba->n[2]; ++f) lm_start[ba->h_fi[2][f] + 1]++;
-    for (int i = 0; i < nr; ++i) lm_start[i + 1] += lm_start[i];
-    std::vector<int> lm_fac(std::max(1, lm_start[nr])), lm_off(2 * (size_t)std::max(1, lm_start[nr]), -1), fill(lm_start.begin(), lm_start.end() - 1);
-    {
-        const int32_t* hi = ba->h_fi[0].data();
-        const int* ord = ba->order[0].data();
-        for (int i = 0; i < n_tf; ++i) {
-            if (i + 16 < n_tf && ord[i + 16] >= 0) __builtin_prefetch(hi + 3 * (size_t)ord[i + 16]);
-            if (ord[i] < 0) continue;
-            const int32_t* ix = hi + 3 * (size_t)ord[i];
-            const int pos = fill[ix[0]]++;
-            lm_fac[pos] = i; lm_off[2 * (size_t)pos] = pose_off[ix[1]]; lm_off[2 * (size_t)pos + 1] = pose_off[ix[2]];
-        }
-    }
-    for (int f = 0; f < ba->n[2]; ++f) lm_fac[fill[ba->h_fi[2][f]]++] = -(f + 1);
-
-    PROF("landmark CSR");
-    // ---- Schur groups: landmarks with the same sorted set of free pose offsets share a warp-sized work item
-    std::vector<int> tf_slot((size_t)std::max(1, n_tf) * 2, -1), sw_group, sw_lm, grp_ns, grp_off;
-    int cols_max = 0;
-    {
-        // signature = sorted set of free pose offsets of a landmark; groups found through an open-addressing hash table
-        // over the signatures (no per-landmark heap traffic), numbered in order of first appearance
-        std::vector<std::vector<int>> members;
-        size_t tsize = 64; while (tsize < 4 * (size_t)std::max(1, nrf)) tsize <<= 1;
-        if (tsize > ((size_t)1 << 20)) tsize = (size_t)1 << 20;
-        std::vector<int> table(tsize, -1);
-        for (int l = 0; l < nr; ++l) {
-            if (rho_slot[l] < 0) continue;
-            int sig[MAX_TRACK + 1], ns = 0;
-            for (int e = lm_start[l]; e < lm_start[l + 1]; ++e) {
-                if (lm_fac[e] < 0) continue;
-                for (int side = 1; side <= 2; ++side) {
-                    const int off = lm_off[2 * (size_t)e + side - 1];
-                    if (off < 0) continue;
-                    int p = 0; while (p < ns && sig[p] < off) ++p;
-                    if (p < ns && sig[p] == off) continue;
-                    if (ns == MAX_TRACK) { set_error("landmark %d is observed from more than %d keyframes", l, (int)MAX_TRACK); return LVB_ERR_UNSUPPORTED; }
-                    for (int q = ns; q > p; --q) sig[q] = sig[q - 1];
-                    sig[p] = off; ++ns;
-                }
-            }
-            unsigned long long h = 1469598103934665603ull ^ (unsigned long long)ns;
-            for (int q = 0; q < ns; ++q) { h ^= (unsigned long long)(unsigned)sig[q]; h *= 1099511628211ull; }
-            size_t slot = (size_t)(h ^ (h >> 29)) & (tsize - 1);
-            int g = -1;
-            for (;;) {
-                const int cand = table[slot];
-                if (cand < 0) break;
-                if (grp_ns[cand] == ns) {
-                    bool same = true;
-                    for (int q = 0; q < ns && same; ++q) same = grp_off[(size_t)cand * MAX_TRACK + q] == sig[q];
-                    if (same) { g = cand; break; }
-                }
-                slot = (slot + 1) & (tsize - 1);
-            }
-            if (g < 0) {
-                g = (int)members.size();
-                if ((size_t)g * 2 >= tsize) {      // keep the load factor below 1/2: rebuild a larger table
-                    tsize <<= 1; table.assign(tsize, -1);
-                    for (int c = 0; c < g; ++c) {
-                        unsigned long long hc = 1469598103934665603ull ^ (unsigned long long)grp_ns[c];
-                        for (int q = 0; q < grp_ns[c]; ++q) { hc ^= (unsigned long long)(unsigned)grp_off[(size_t)c * MAX_TRACK + q]; hc *= 1099511628211ull; }
-                        size_t sc = (size_t)(hc ^ (hc >> 29)) & (tsize - 1);
-                        while (table[sc] >= 0) sc = (sc + 1) & (tsize - 1);
-                        table[sc] = c;
-                    }
-                    slot = (size_t)(h ^ (h >> 29)) & (tsize - 1);
-                    while (table[slot] >= 0) slot = (slot + 1) & (tsize - 1);
-                }
-                table[slot] = g;
-                members.emplace_back(); grp_ns.push_back(ns);
-                for (int k2 = 0; k2 < MAX_TRACK; ++k2) grp_off.push_back(k2 < ns ? sig[k2] : -1);
-            }
-            members[g].push_back(l);
-            for (int e = lm_start[l]; e < lm_start[l + 1]; ++e) {
-                const int i = lm_fac[e]; if (i < 0) continue;
-                for (int side = 1; side <= 2; ++side) {
-                    const int off = lm_off[2 * (size_t)e + side - 1];
-                    if (off < 0) continue;
-                    int p = 0; while (sig[p] != off) ++p;
-                    tf_slot[(size_t)(side - 1) * n_tf + i] = p;
-                }
-            }
-        }
-        for (size_t g = 0; g < members.size(); ++g) {
-            cols_max = std::max(cols_max, 6 * grp_ns[g] + 1);
-            for (size_t i = 0; i < members[g].size(); i += 32) {
-                sw_group.push_back((int)g);
-                for (size_t t = i; t < i + 32; ++t) sw_lm.push_back(t < members[g].size() ? members[g][t] : -1);
-            }
-        }
-    }
-    ba->n_schur_warps = (int)sw_group.size(); ba->schur_cols_max = cols_max;
-    PROF("schur groups");
-    // ---- envelope of S: first structurally non-zero column per row, from every coupling the assembly can create
-    std::vector<int> chol_rmax(ba->dimc / 32 + 2, 0), chol_cmin(ba->dimc / 32 + 2, 0);
-    int band = 0, panel_rows = 2, true_band = 0;
-    if (ba->solvable) {
-        std::vector<int> first(ba->dimc);
-        std::vector<int> fb(blks.size());
-        for (size_t b = 0; b < blks.size(); ++b) fb[b] = blk_start[b];
-        auto couple = [&](int offA, int offB) {
-            if (offA < 0 || offB < 0) return;
-            const int a = blk_of_off[offA], b = blk_of_off[offB];
-            const int lo = std::min(a, b), hi = std::max(a, b);
-            fb[hi] = std::min(fb[hi], blk_start[lo]);
-        };
-        for (size_t g = 0; g < grp_ns.size(); ++g) for (int a = 0; a < grp_ns[g]; ++a) for (int b = 0; b < a; ++b) couple(grp_off[g * MAX_TRACK + a], grp_off[g * MAX_TRACK + b]);
-        for (int f = 0; f < ba->n[0]; ++f) couple(pose_off[ba->h_fi[0][3 * (size_t)f + 1]], pose_off[ba->h_fi[0][3 * (size_t)f + 2]]);
-        for (int f = 0; f < ba->n[3]; ++f) {
-            const int32_t* ix = &ba->h_fi[3][8 * (size_t)f];
-            int offs[8];
-            for (int b = 0; b < 8; ++b) offs[b] = ix[b] < 0 ? -1 : ((b == 0 || b == 4) ? pose_off[ix[b]] : vec3_off[ix[b]]);
-            for (int a = 0; a < 8; ++a) for (int b = 0; b < a; ++b) couple(offs[a], offs[b]);
-        }
-        for (int f = 0; f < ba->n[4]; ++f) couple(pose_off[ba->h_fi[4][2 * (size_t)f]], pose_off[ba->h_fi[4][2 * (size_t)f + 1]]);
-        // sharded problems: the other ranks' couplings arrive with the all-reduce, so the envelope must be the global one
-        if (ctx->world > 1) {
-            DevBuf<int> tmp;
-            LVB_TRY(tmp.upload(fb.data(), fb.size(), s));
-            LVB_TRY(comm_allreduce_min_i32(ctx, tmp.p, fb.size()));
-            LVB_CUDA(cudaMemcpyAsync(fb.data(), tmp.p, fb.size() * sizeof(int), cudaMemcpyDeviceToHost, s));
-            LVB_CUDA(cudaStreamSynchronize(s));
-        }
-        for (int r = 0; r < ba->dimc; ++r) { first[r] = fb[blk_of_off[r]]; true_band = std::max(true_band, r - first[r]); }
-        // rmax per 32-column step by a backward sweep: rows whose first column lies left of the end of the step
-        {
-            const int nstep = (ba->dimc + 31) / 32;
-            std::vector<int> last_row_of_col(ba->dimc, 0);      // largest row r with first[r] <= c, via prefix max over c
-            for (int c = 0; c < ba->dimc; ++c) last_row_of_col[c] = c;
-            for (int r = 0; r < ba->dimc; ++r) last_row_of_col[first[r]] = std::max(last_row_of_col[first[r]], r);
-            for (int c = 1; c < ba->dimc; ++c) last_row_of_col[c] = std::max(last_row_of_col[c], last_row_of_col[c - 1]);
-            for (int step = 0; step < nstep; ++step) {
-                const int kb = step * 32, bs = std::min(32, ba->dimc - kb);
-                int cmin = kb;
-                for (int r = kb; r < kb + bs; ++r) cmin = std::min(cmin, first[r]);
-                const int rmax = std::max(kb + bs - 1, last_row_of_col[kb + bs - 1]);
-                chol_rmax[step] = rmax; chol_cmin[step] = cmin;
-                band = std::max(band, std::max(rmax - kb, kb + bs - 1 - cmin));
-                panel_rows = std::max(panel_rows, rmax - (kb + bs) + 2);
-            }
-        }
-    }
-    // ---- storage of Hpp / S
-    // the envelope above is the one of GLOBAL 32-column steps; the fronts of the separator tree step through 32 columns from their
-    // own first unknown, and for an arbitrary start a block column needs rows up to true_band + 31 below its first column
-    if (!dense_layout) band = std::max(band, true_band + 31);
-    band = std::min(std::max(band, 31), std::max(31, ba->dimc - 1));
-    if (dense_layout) { ba->srow = ba->dimc; ba->soff = 0; ba->nS = (size_t)ba->dimc * ba->dimc; }
-    else              { ba->srow = band; ba->soff = band; ba->nS = (size_t)ba->dimc * (size_t)(band + 1); }
-    ba->band = band; ba->panel_rows = panel_rows;
-    ba->chol_smem = (size_t)(CHOL_HDR + std::max(panel_rows + 2, 34) * 34) * 8;      // two diagonal-block buffers + the panel (>= 34 rows; later the backward partial sums)
-    // banded systems: split the chain by a separator tree when the band leaves room for at least two leaves (ba_tree.cuh)
-    ba->tree_levels = 0;
-    std::vector<Front> h_fronts;
-    size_t pool_doubles = 0;
-    {
-        static const bool no_tree = getenv("LVB_NO_TREE") && getenv("LVB_NO_TREE")[0] == '1';
-        int rows = 0, mnb = 0, max_leaves = 1;
-        while (max_leaves * 2 <= std::max(2, ctx->sm_count)) max_leaves *= 2;
-        if (ba->solvable && !dense_layout && !no_tree) {
-            const int lv = build_front_tree(ba->dimc, band, true_band, max_leaves, h_fronts, ba->level_first, ba->level_count, pool_doubles, rows, mnb);
-            const size_t fs = (size_t)(32 * 33 + 32 + 128 + (rows + 2) * 34) * 8, bs_ = (size_t)(((mnb + 1) & ~1) + (CHOL_T / 32) * 32) * 8;
-            if (lv > 0 && fs <= 227 * 1024 - 256 && pool_doubles < ((size_t)1 << 31)) { ba->tree_levels = lv; ba->tree_factor_smem = fs; ba->tree_back_smem = bs_; }
-        }
-    }
-    // loop-closure shaped envelopes: neither a tree nor a panel that fits in shared memory -- the per-phase grids of ba_wide.cuh
-    ba->wide_solver = ba->solvable && ba->tree_levels == 0 && ba->chol_smem > 227 * 1024 - 256;
-    ba->h_rmax = chol_rmax;
-    if (ba->solvable && ba->nS > ((size_t)3 << 30)) { ba->solvable = false; ba->unsolvable_why = "the banded reduced camera system exceeds 24 GB"; }
-    if (!ba->solvable) ba->nS = 1;
-    if (sw_group.empty()) { sw_group.push_back(0); sw_lm.assign(32, -1); }
-    if (grp_ns.empty()) { grp_ns.push_back(0); grp_off.assign(MAX_TRACK, -1); }
-
-    PROF("envelope");
     LVB_TRY(stg.put(ba->poses, ba->h_poses.data(), ba->h_poses.size()));
     LVB_TRY(stg.put(ba->vec3, ba->h_vec3.data(), ba->h_vec3.size()));
     LVB_TRY(stg.put(ba->rho, ba->h_rho.data(), ba->h_rho.size()));
     LVB_TRY(stg.put(ba->c_poses, ba->h_poses.data(), ba->h_poses.size()));
     LVB_TRY(stg.put(ba->c_vec3, ba->h_vec3.data(), ba->h_vec3.size()));
     LVB_TRY(stg.put(ba->c_rho, ba->h_rho.data(), ba->h_rho.size()));
-    LVB_TRY(stg.put(ba->pose_off, pose_off.data(), np));
-    LVB_TRY(stg.put(ba->vec3_off, vec3_off.data(), nv));
-    LVB_TRY(stg.put(ba->rho_slot, rho_slot.data(), nr));
-    LVB_TRY(stg.put(ba->lm_start, lm_start.data(), nr + 1));
-    LVB_TRY(stg.put(ba->lm_fac, lm_fac.data(), lm_fac.size()));
-    LVB_TRY(stg.put(ba->tf_slot, tf_slot.data(), tf_slot.size()));
-    LVB_TRY(stg.put(ba->sw_group, sw_group.data(), sw_group.size()));
-    LVB_TRY(stg.put(ba->sw_lm, sw_lm.data(), sw_lm.size()));
-    LVB_TRY(stg.put(ba->grp_ns, grp_ns.data(), grp_ns.size()));
-    LVB_TRY(stg.put(ba->grp_off, grp_off.data(), grp_off.size()));
-    LVB_TRY(stg.put(ba->chol_rmax, chol_rmax.data(), chol_rmax.size()));
-    LVB_TRY(stg.put(ba->chol_cmin, chol_cmin.data(), chol_cmin.size()));
-    if (ba->tree_levels > 0) { LVB_TRY(stg.put(ba->fronts, h_fronts.data(), h_fronts.size())); LVB_TRY(ba->front_pool.ensure(pool_doubles)); }
-    // tensor-core Schur operands: compact pose dimensions (<= 128) and the zero-initialised split-bf16 U^T tiles
-    ba->tc_ok = ba->solvable && dense_layout && 6 * npf <= 128 && npf > 0 && ctx->world == 1;
-    {
-        std::vector<int> cdim(std::max(1, ba->dimc), -1), coff(128, -1);
-        int c = 0;
-        for (size_t b = 0; b < blks.size(); ++b) if (blks[b].type == 0 && c + 6 <= 128) { for (int k = 0; k < 6; ++k) { cdim[blk_start[b] + k] = c + k; coff[c + k] = blk_start[b] + k; } c += 6; }
-        LVB_TRY(stg.put(ba->tc_cdim, cdim.data(), cdim.size()));
-        LVB_TRY(stg.put(ba->tc_off, coff.data(), coff.size()));
-        ba->n_tc_chunks = ba->tc_ok ? ((2 * ba->n_schur_warps + TC_CHUNKS - 1) / TC_CHUNKS) * TC_CHUNKS : 0;
-        LVB_TRY(ba->tc_u.ensure((size_t)std::max(1, ba->n_tc_chunks) * 3 * 2048));
-        LVB_CUDA(cudaMemsetAsync(ba->tc_u.p, 0, (size_t)std::max(1, ba->n_tc_chunks) * 3 * 2048 * sizeof(unsigned short), s));
-    }
+    LVB_TRY(stg.put(ba->pose_off, P.pose_off.data(), np));
+    LVB_TRY(stg.put(ba->vec3_off, P.vec3_off.data(), nv));
+    LVB_TRY(stg.put(ba->rho_slot, P.rho_slot.data(), nr));
+    LVB_TRY(stg.put(ba->lm_start, P.lm_start.data(), nr + 1));
+    LVB_TRY(stg.put(ba->lm_fac, P.lm_fac.data(), P.lm_fac.size()));
+    LVB_TRY(stg.put(ba->tf_slot, P.tf_slot.data(), P.tf_slot.size()));
+    LVB_TRY(stg.put(ba->sw_group, P.sw_group.data(), P.sw_group.size()));
+    LVB_TRY(stg.put(ba->sw_lm, P.sw_lm.data(), P.sw_lm.size()));
+    LVB_TRY(stg.put(ba->grp_ns, P.grp_ns.data(), P.grp_ns.size()));
+    LVB_TRY(stg.put(ba->grp_off, P.grp_off.data(), P.grp_off.size()));
+    LVB_TRY(stg.put(ba->chol_rmax, P.chol_rmax.data(), P.chol_rmax.size()));
+    LVB_TRY(stg.put(ba->chol_cmin, P.chol_cmin.data(), P.chol_cmin.size()));
+    if (P.solver.tree_levels > 0) { LVB_TRY(stg.put(ba->fronts, P.solver.fronts.data(), P.solver.fronts.size())); LVB_TRY(ba->front_pool.ensure(P.solver.pool_doubles)); }
+    // tensor-core Schur operands: the compaction maps and the zero-initialised split-bf16 U^T tiles
+    LVB_TRY(stg.put(ba->tc_cdim, P.tc_cdim.data(), P.tc_cdim.size()));
+    LVB_TRY(stg.put(ba->tc_off, P.tc_off.data(), P.tc_off.size()));
+    ba->n_tc_chunks = P.tc_ok ? ((2 * P.n_schur_warps + TC_CHUNKS - 1) / TC_CHUNKS) * TC_CHUNKS : 0;
+    LVB_TRY(ba->tc_u.ensure((size_t)std::max(1, ba->n_tc_chunks) * 3 * 2048));
+    LVB_CUDA(cudaMemsetAsync(ba->tc_u.p, 0, (size_t)std::max(1, ba->n_tc_chunks) * 3 * 2048 * sizeof(unsigned short), s));
 
     PROF("uploads (params, structure)");
     // factor planes in device order (AoS -> SoA transpose on the host, written straight into the staging area; IMU stays AoS and
     // is packed on the device).  The one copy to the device is issued when the last array is in place; the IMU kernel follows it.
     {
         for (int k = 0; k < 6; ++k) {
-            const int n = ba->nd[k];
-            const std::vector<int>& ord = ba->order[k];
+            const int n = P.nd[k];
+            const std::vector<int>& ord = P.order[k];
             const int is = kIdxStride[k];
             int* iplanes = nullptr;
             LVB_TRY(stg.reserve(ba->fi[k], (size_t)std::max(1, n) * is, &iplanes));
@@ -2037,7 +1706,7 @@ int lvb_ba_finalize(lvb_ba* ba) {
             }
             LVB_TRY(stg.finish());
         }
-        const int n = ba->nd[3];
+        const int n = P.nd[3];
         LVB_TRY(stg.put(ba->imu_raw, ba->h_fc[3].data(), ba->h_fc[3].size()));
         LVB_TRY(stg.commit(ba->upload_arena));      // everything uploaded so far: one copy
         LVB_TRY(ba->fc[3].ensure((size_t)std::max(1, n) * IMU_STRIDE));
@@ -2051,29 +1720,29 @@ int lvb_ba_finalize(lvb_ba* ba) {
     }
     PROF("planes + uploads");
 
-    const size_t nH = ba->nS;
-    LVB_TRY(ba->chol_invd.ensure(ba->dimc + 32));
-    LVB_TRY(ba->Hpp.ensure(nH)); LVB_TRY(ba->gc.ensure(ba->dimc));
+    const size_t nH = P.nS;
+    LVB_TRY(ba->chol_invd.ensure(P.dimc + 32));
+    LVB_TRY(ba->Hpp.ensure(nH)); LVB_TRY(ba->gc.ensure(P.dimc));
     LVB_TRY(ba->Hll.ensure(std::max(1, nr))); LVB_TRY(ba->gl.ensure(std::max(1, nr)));
-    LVB_TRY(ba->tf_w.ensure((size_t)std::max(1, ba->nd[0]) * 12));
-    LVB_TRY(ba->arena.ensure(nH + 3 * (size_t)ba->dimc + 16));
-    LVB_TRY(ba->scale_c.ensure(ba->dimc)); LVB_TRY(ba->lam_c.ensure(ba->dimc));
+    LVB_TRY(ba->tf_w.ensure((size_t)std::max(1, P.nd[0]) * 12));
+    LVB_TRY(ba->arena.ensure(nH + 3 * (size_t)P.dimc + 16));
+    LVB_TRY(ba->scale_c.ensure(P.dimc)); LVB_TRY(ba->lam_c.ensure(P.dimc));
     LVB_TRY(ba->scale_l.ensure(std::max(1, nr))); LVB_TRY(ba->lam_l.ensure(std::max(1, nr)));
     LVB_TRY(ba->st.ensure(1));
 
     PROF("sync + alloc");
     BaDev& d = ba->dev;
-    d.n_poses = np; d.n_vec3 = nv; d.n_rho = nr; d.dimc = ba->dimc; d.n_pose_free = npf;
-    d.srow = ba->srow; d.soff = ba->soff; d.nS = ba->nS;
+    d.n_poses = np; d.n_vec3 = nv; d.n_rho = nr; d.dimc = P.dimc; d.n_pose_free = npf;
+    d.srow = P.srow; d.soff = P.soff; d.nS = P.nS;
     d.poses = ba->poses.p; d.vec3 = ba->vec3.p; d.rho = ba->rho.p; d.c_poses = ba->c_poses.p; d.c_vec3 = ba->c_vec3.p; d.c_rho = ba->c_rho.p;
     d.pose_off = ba->pose_off.p; d.vec3_off = ba->vec3_off.p; d.rho_slot = ba->rho_slot.p;
-    for (int k = 0; k < 6; ++k) { d.n[k] = ba->nd[k]; d.fc[k] = ba->fc[k].p; d.fi[k] = ba->fi[k].p; d.huber[k] = ba->huber[k]; }
+    for (int k = 0; k < 6; ++k) { d.n[k] = P.nd[k]; d.fc[k] = ba->fc[k].p; d.fi[k] = ba->fi[k].p; d.huber[k] = ba->huber[k]; }
     d.lm_start = ba->lm_start.p; d.lm_fac = ba->lm_fac.p;
     d.tf_slot = ba->tf_slot.p; d.sw_group = ba->sw_group.p; d.sw_lm = ba->sw_lm.p; d.grp_ns = ba->grp_ns.p; d.grp_off = ba->grp_off.p;
-    d.n_schur_warps = ba->n_schur_warps; d.warp_syrk = 1;
+    d.n_schur_warps = P.n_schur_warps; d.warp_syrk = 1;
     d.tc_mode = 0; d.tc_u = ba->tc_u.p; d.tc_cdim = ba->tc_cdim.p; d.tc_off = ba->tc_off.p; d.tc_ndim = 6 * npf;
     d.Hpp = ba->Hpp.p; d.gc = ba->gc.p; d.Hll = ba->Hll.p; d.gl = ba->gl.p; d.tf_w = ba->tf_w.p;
-    d.S = ba->arena.p; d.rhs = d.S + nH; d.gcr = d.rhs + ba->dimc; d.diagH = d.gcr + ba->dimc; d.scal = d.diagH + ba->dimc;
+    d.S = ba->arena.p; d.rhs = d.S + nH; d.gcr = d.rhs + P.dimc; d.diagH = d.gcr + P.dimc; d.scal = d.diagH + P.dimc;
     d.scale_c = ba->scale_c.p; d.scale_l = ba->scale_l.p; d.lam_c = ba->lam_c.p; d.lam_l = ba->lam_l.p;
     d.st = ba->st.p;
     d.rank = ctx->rank; d.world = ctx->world; d.rank0 = (ctx->rank == 0) ? 1 : 0;
@@ -2082,19 +1751,19 @@ int lvb_ba_finalize(lvb_ba* ba) {
 
     BlockRanges& R = ba->ranges;
     R.b[0] = 0;
-    R.b[1] = R.b[0] + nblk(ba->nd[0], TPB);
-    R.b[2] = R.b[1] + nblk(ba->nd[1], TPB);
-    R.b[3] = R.b[2] + nblk(ba->nd[2], TPB);
-    d.imu_cta = dense_layout ? 1 : 0;
-    R.b[4] = R.b[3] + (d.imu_cta ? ba->nd[3] : nblk(ba->nd[3], 4));
-    R.b[5] = R.b[4] + nblk(ba->nd[4], TPB);
-    R.b[6] = R.b[5] + nblk(ba->nd[5], TPB);
+    R.b[1] = R.b[0] + nblk(P.nd[0], TPB);
+    R.b[2] = R.b[1] + nblk(P.nd[1], TPB);
+    R.b[3] = R.b[2] + nblk(P.nd[2], TPB);
+    d.imu_cta = P.dense ? 1 : 0;
+    R.b[4] = R.b[3] + (d.imu_cta ? P.nd[3] : nblk(P.nd[3], 4));
+    R.b[5] = R.b[4] + nblk(P.nd[4], TPB);
+    R.b[6] = R.b[5] + nblk(P.nd[5], TPB);
     const size_t smem_imu = d.imu_cta ? (size_t)(480 * 2 + 32 + IMU_STRIDE) * 8 + 32 * 4 : (size_t)(4 * 480 * 2 + 4 * 32) * 8 + 4 * 32 * 4;
     const size_t smem_pose = d.stage_poses ? ((size_t)np * 56 + 16) : 0;
     drop_graph(ba);
     ba->pose_smem = smem_pose; ba->imu_smem = smem_imu;
     ba->lin_smem = ((smem_pose + 15) & ~(size_t)15) + (size_t)(TPB / 32) * SYRK_ROWS * SYRK_LD * 8;
-    ba->schur_smem = (size_t)(TPB / 32) * 32 * (size_t)std::max(1, cols_max) * 8;
+    ba->schur_smem = (size_t)(TPB / 32) * 32 * (size_t)std::max(1, P.schur_cols_max) * 8;
     PROF("tail");
 #undef PROF
     ba->finalized = true;
@@ -2103,8 +1772,8 @@ int lvb_ba_finalize(lvb_ba* ba) {
 
 int lvb_ba_dims(lvb_ba* ba, int* dimc, int* nrf, int* rows) {
     if (!ba->finalized) { set_error("finalize first"); return LVB_ERR_STATE; }
-    if (dimc) *dimc = ba->dimc;
-    if (nrf) *nrf = ba->n_rho_free;
+    if (dimc) *dimc = ba->plan.dimc;
+    if (nrf) *nrf = ba->plan.n_rho_free;
     if (rows) { int r = 0; for (int k = 0; k < 6; ++k) r += ba->n[k] * kResDim[k]; *rows = r; }
     return LVB_OK;
 }
@@ -2122,8 +1791,8 @@ int lvb_ba_update_params(lvb_ba* ba, const double* P, const double* V, const dou
 }
 
 static int check_imu_status(lvb_ba* ba) {
-    if (ba->imu_checked || ba->nd[3] == 0) { ba->imu_checked = true; return LVB_OK; }
-    std::vector<int> status(ba->nd[3]);
+    if (ba->imu_checked || ba->plan.nd[3] == 0) { ba->imu_checked = true; return LVB_OK; }
+    std::vector<int> status(ba->plan.nd[3]);
     LVB_TRY(ba->imu_status.download(status.data(), status.size(), ba->ctx->stream));
     LVB_CUDA(cudaStreamSynchronize(ba->ctx->stream));
     for (size_t f = 0; f < status.size(); ++f) if (status[f]) { set_error("ImuError %d: covariance is singular or not finite (code %d)", (int)f, status[f]); return LVB_ERR_NUMERIC; }
@@ -2132,7 +1801,7 @@ static int check_imu_status(lvb_ba* ba) {
 }
 
 static int launch_eval(lvb_ba* ba, int kind, double* r_dev, double* J_dev) {
-    const int n = ba->nd[kind];
+    const int n = ba->plan.nd[kind];
     if (n == 0) return LVB_OK;
     BaDev& d = ba->dev;
     switch (kind) {
@@ -2153,7 +1822,7 @@ static int launch_eval(lvb_ba* ba, int kind, double* r_dev, double* J_dev) {
 }
 
 static int ensure_eval_buffers(lvb_ba* ba, int kind) {
-    const size_t n = ba->nd[kind];
+    const size_t n = ba->plan.nd[kind];
     LVB_TRY(ba->eval_r.ensure(std::max<size_t>(1, n * kResDim[kind])));
     LVB_TRY(ba->eval_J.ensure(std::max<size_t>(1, n * kResDim[kind] * kJacCols[kind])));
     return LVB_OK;
@@ -2166,8 +1835,8 @@ int lvb_ba_eval(lvb_ba* ba, int kind, double* r, double* J) {
     LVB_TRY(check_imu_status(ba));
     LVB_TRY(ensure_eval_buffers(ba, kind));
     LVB_TRY(launch_eval(ba, kind, ba->eval_r.p, ba->eval_J.p));
-    const size_t nd = ba->nd[kind], rd = kResDim[kind], jd = (size_t)kResDim[kind] * kJacCols[kind];
-    const std::vector<int>& ord = ba->order[kind];
+    const size_t nd = ba->plan.nd[kind], rd = kResDim[kind], jd = (size_t)kResDim[kind] * kJacCols[kind];
+    const std::vector<int>& ord = ba->plan.order[kind];
     bool identity = (nd == (size_t)ba->n[kind]);
     for (size_t i = 0; identity && i < nd; ++i) identity = (ord[i] == (int)i);
     cudaStream_t s = ba->ctx->stream;
@@ -2200,7 +1869,7 @@ int lvb_ba_eval_device(lvb_ba* ba, int kind) {
 
 static bool merged_linearize(lvb_ba* ba) {
     static const bool off = getenv("LVB_NO_MERGED_LINEARIZE") && getenv("LVB_NO_MERGED_LINEARIZE")[0] == '1';
-    return !off && ba->srow == ba->dimc && ba->soff == 0 && ba->ranges.b[3] > 0 && ba->ranges.b[6] > ba->ranges.b[3];      // dense layout = window-sized
+    return !off && ba->plan.srow == ba->plan.dimc && ba->plan.soff == 0 && ba->ranges.b[3] > 0 && ba->ranges.b[6] > ba->ranges.b[3];      // dense layout = window-sized
 }
 
 static bool use_side_branch(lvb_ba* ba) {
@@ -2208,6 +1877,30 @@ static bool use_side_branch(lvb_ba* ba) {
     // pass on the same build), a linear graph is stable
     return ba->ctx->use_side && ba->ctx->side && !g_timing && !ba->capturing && ba->ranges.b[3] > 0 && ba->ranges.b[6] > ba->ranges.b[3];
 }
+
+// The visual and the IMU / prior linearisations, MODE 0 at the current parameters (start of a pass), MODE 1 at the candidate (after
+// the update).  They are independent (both only add into the accumulators): one grid for both at window size, two kernels (parallel
+// branches when launched directly) at map scale.  The timing marks keep the names of the instantiations.
+extern "C++" {
+template <int MODE> static int launch_linearize(lvb_ba* ba) {
+    static const char* const kName[2][3] = {{"ba_linearize_all_kernel<0>", "ba_linearize_kernel<0>", "ba_linearize_other_kernel<0>"},
+                                            {"ba_linearize_all_kernel<1>", "ba_linearize_kernel<1>", "ba_linearize_other_kernel<1>"}};
+    BaDev& d = ba->dev;
+    lvb_ctx* ctx = ba->ctx;
+    const bool one_grid = merged_linearize(ba);
+    const bool fork = !one_grid && use_side_branch(ba);
+    if (one_grid) LAUNCH_AS(ba, kName[MODE][0], ba_linearize_all_kernel<MODE>, ba->ranges.b[6], TPB, std::max(ba->lin_smem, ba->imu_smem), d, ba->ranges);
+    else {
+    if (fork) { LVB_CUDA(cudaEventRecord(ctx->ev_fork, ctx->stream)); LVB_CUDA(cudaStreamWaitEvent(ctx->side, ctx->ev_fork, 0)); }
+    LAUNCH_AS(ba, kName[MODE][1], ba_linearize_kernel<MODE>, ba->ranges.b[3], TPB, ba->lin_smem, d, ba->ranges);
+    if (fork) {
+        LAUNCH_ON(ba, ctx->side, ba_linearize_other_kernel<MODE>, ba->ranges.b[6] - ba->ranges.b[3], TPB, ba->imu_smem, d, ba->ranges);
+        LVB_CUDA(cudaEventRecord(ctx->ev_join, ctx->side)); LVB_CUDA(cudaStreamWaitEvent(ctx->stream, ctx->ev_join, 0));
+    } else LAUNCH_AS(ba, kName[MODE][2], ba_linearize_other_kernel<MODE>, ba->ranges.b[6] - ba->ranges.b[3], TPB, ba->imu_smem, d, ba->ranges);
+    }
+    return LVB_OK;
+}
+}  // extern "C++"
 
 // one pass = one LM iteration attempt (all decisions on the device), 10 launches (the two linearise kernels and the two
 // cost kernels run as parallel branches on a second stream):
@@ -2217,23 +1910,11 @@ static int launch_linearize_and_reduce(lvb_ba* ba, bool standalone) {
     BaDev& d = ba->dev;
     lvb_ctx* ctx = ba->ctx;
     const size_t nH = d.nS;
-    // the visual and the IMU / prior linearisations are independent (both only add into the accumulators): one grid for both at
-    // window size, two kernels (parallel branches when launched directly) at map scale
-    const bool one_grid = merged_linearize(ba);
-    const bool fork = !one_grid && use_side_branch(ba);
-    if (one_grid) LAUNCH(ba, ba_linearize_all_kernel<0>, ba->ranges.b[6], TPB, std::max(ba->lin_smem, ba->imu_smem), d, ba->ranges);
-    else {
-    if (fork) { LVB_CUDA(cudaEventRecord(ctx->ev_fork, ctx->stream)); LVB_CUDA(cudaStreamWaitEvent(ctx->side, ctx->ev_fork, 0)); }
-    LAUNCH(ba, ba_linearize_kernel<0>, ba->ranges.b[3], TPB, ba->lin_smem, d, ba->ranges);
-    if (fork) {
-        LAUNCH_ON(ba, ctx->side, ba_linearize_other_kernel<0>, ba->ranges.b[6] - ba->ranges.b[3], TPB, ba->imu_smem, d, ba->ranges);
-        LVB_CUDA(cudaEventRecord(ctx->ev_join, ctx->side)); LVB_CUDA(cudaStreamWaitEvent(ctx->stream, ctx->ev_join, 0));
-    } else LAUNCH(ba, ba_linearize_other_kernel<0>, ba->ranges.b[6] - ba->ranges.b[3], TPB, ba->imu_smem, d, ba->ranges);
-    }
+    LVB_TRY(launch_linearize<0>(ba));
     const bool fuse_damp = ctx->world == 1;
     if (fuse_damp) LAUNCH(ba, ba_build_S_kernel<1>, std::min(1024, nblk(nH, 256)), 256, 0, d);
     else LAUNCH(ba, ba_build_S_kernel<0>, std::min(1024, nblk(nH, 256)), 256, 0, d);
-    LAUNCH(ba, ba_schur_kernel, nblk(d.n_schur_warps, TPB / 32), TPB, ba->schur_smem, d, std::max(1, ba->schur_cols_max));
+    LAUNCH(ba, ba_schur_kernel, nblk(d.n_schur_warps, TPB / 32), TPB, ba->schur_smem, d, std::max(1, ba->plan.schur_cols_max));
     if (d.tc_mode) LAUNCH(ba, ba_schur_tc_kernel, ba->n_tc_chunks / TC_CHUNKS, 128, (size_t)TC_CHUNKS * TC_CHUNK_BYTES, d, ba->n_tc_chunks);
     const size_t n_arena = nH + 3 * (size_t)d.dimc + 16;
     P2PArgs pa;
@@ -2259,7 +1940,7 @@ static int launch_wide_solve(lvb_ba* ba) {
     if (!attr_set) { LVB_CUDA(cudaFuncSetAttribute(ba_wide_update_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, WIDE_WARPS * 2 * 32 * 34 * 8)); attr_set = true; }
     for (int kb = 0; kb < n; kb += 32) {
         const int bs = std::min(32, n - kb);
-        const int m = ba->h_rmax[kb >> 5] - (kb + bs) + 2;
+        const int m = ba->plan.chol_rmax[kb >> 5] - (kb + bs) + 2;
         const int ntile = (m + 31) / 32, total = m > 1 ? ntile * (ntile + 1) / 2 : 0;
         LAUNCH(ba, ba_wide_diag_kernel, 1, 32, 0, d.S, n, d.srow, d.soff, kb, ba->chol_invd.p, d.st, kb == 0 ? 1 : 0);
         LAUNCH(ba, ba_wide_panel_kernel, nblk(m, 128), 128, 0, d.S, d.rhs, n, d.srow, d.soff, kb, ba->chol_invd.p, d.st, ba->chol_rmax.p);
@@ -2273,21 +1954,23 @@ static int launch_wide_solve(lvb_ba* ba) {
 static int launch_reduced_solve(lvb_ba* ba) {
     BaDev& d = ba->dev;
     lvb_ctx* ctx = ba->ctx;
-    if (ba->tree_levels > 0) {
+    const SolverPlan& sp = ba->plan.solver;
+    const int band = ba->plan.band;
+    if (sp.tree_levels > 0) {
         // multifrontal tree: leaves (all SMs) -> ... -> root, then the back-substitution root -> leaves; 2 (levels + 1) launches
         const Front* fr = ba->fronts.p;
         LAUNCH(ba, lm_control_pre_kernel, 1, 1, 0, d.st);
-        const int n_fronts = ba->level_first[ba->tree_levels - 1] + ba->level_count[ba->tree_levels - 1];
-        ba_front_init_kernel<<<dim3(16, n_fronts), 256, 0, ctx->stream>>>(fr, n_fronts, d.S, d.rhs, ba->front_pool.p, d.srow, d.soff, ba->band, d.st);
+        const int n_fronts = sp.level_first[sp.tree_levels - 1] + sp.level_count[sp.tree_levels - 1];
+        ba_front_init_kernel<<<dim3(16, n_fronts), 256, 0, ctx->stream>>>(fr, n_fronts, d.S, d.rhs, ba->front_pool.p, d.srow, d.soff, band, d.st);
         ctx->launches++; mark(ba, "ba_front_init_kernel");
-        for (int l = 0; l < ba->tree_levels; ++l)
-            LAUNCH(ba, ba_front_factor_kernel, ba->level_count[l], CHOL_T, ba->tree_factor_smem, fr, ba->level_first[l], d.S, d.rhs, ba->front_pool.p, d.srow, d.soff, ba->band, ba->chol_invd.p, d.st);
-        for (int l = ba->tree_levels - 1; l >= 0; --l)
-            LAUNCH(ba, ba_front_backward_kernel, ba->level_count[l], CHOL_T, ba->tree_back_smem, fr, ba->level_first[l], d.S, d.rhs, ba->front_pool.p, d.srow, d.soff, ba->band, ba->chol_invd.p, d.st);
-    } else if (ba->wide_solver) {
+        for (int l = 0; l < sp.tree_levels; ++l)
+            LAUNCH(ba, ba_front_factor_kernel, sp.level_count[l], CHOL_T, sp.tree_factor_smem, fr, sp.level_first[l], d.S, d.rhs, ba->front_pool.p, d.srow, d.soff, band, ba->chol_invd.p, d.st);
+        for (int l = sp.tree_levels - 1; l >= 0; --l)
+            LAUNCH(ba, ba_front_backward_kernel, sp.level_count[l], CHOL_T, sp.tree_back_smem, fr, sp.level_first[l], d.S, d.rhs, ba->front_pool.p, d.srow, d.soff, band, ba->chol_invd.p, d.st);
+    } else if (sp.wide) {
         LVB_TRY(launch_wide_solve(ba));
     } else
-    LAUNCH(ba, ba_cholesky_kernel, 1, CHOL_T, ba->chol_smem, d.S, d.rhs, d.dimc, d.srow, d.soff, ba->chol_invd.p, d.st, 1, ba->chol_rmax.p, ba->chol_cmin.p);
+    LAUNCH(ba, ba_cholesky_kernel, 1, CHOL_T, sp.chol_smem, d.S, d.rhs, d.dimc, d.srow, d.soff, ba->chol_invd.p, d.st, 1, ba->chol_rmax.p, ba->chol_cmin.p);
     return LVB_OK;
 }
 
@@ -2296,17 +1979,7 @@ static int launch_step(lvb_ba* ba) {
     lvb_ctx* ctx = ba->ctx;
     LVB_TRY(launch_reduced_solve(ba));
     LAUNCH(ba, ba_update_kernel, nblk((size_t)d.n_poses + d.n_vec3 + d.n_rho, TPB), TPB, 0, d);
-    const bool one_grid = merged_linearize(ba);
-    const bool fork = !one_grid && use_side_branch(ba);
-    if (one_grid) LAUNCH(ba, ba_linearize_all_kernel<1>, ba->ranges.b[6], TPB, std::max(ba->lin_smem, ba->imu_smem), d, ba->ranges);
-    else {
-    if (fork) { LVB_CUDA(cudaEventRecord(ctx->ev_fork, ctx->stream)); LVB_CUDA(cudaStreamWaitEvent(ctx->side, ctx->ev_fork, 0)); }
-    LAUNCH(ba, ba_linearize_kernel<1>, ba->ranges.b[3], TPB, ba->lin_smem, d, ba->ranges);
-    if (fork) {
-        LAUNCH_ON(ba, ctx->side, ba_linearize_other_kernel<1>, ba->ranges.b[6] - ba->ranges.b[3], TPB, ba->imu_smem, d, ba->ranges);
-        LVB_CUDA(cudaEventRecord(ctx->ev_join, ctx->side)); LVB_CUDA(cudaStreamWaitEvent(ctx->stream, ctx->ev_join, 0));
-    } else LAUNCH(ba, ba_linearize_other_kernel<1>, ba->ranges.b[6] - ba->ranges.b[3], TPB, ba->imu_smem, d, ba->ranges);
-    }
+    LVB_TRY(launch_linearize<1>(ba));
     if (ctx->world > 1) LVB_TRY(comm_allreduce_sum_f64(ctx, &d.st->cand_cost_acc, 5));
     const bool wide = d.nS > ((size_t)1 << 20) || (size_t)d.n_poses * 7 + (size_t)d.n_vec3 * 3 + d.n_rho > ((size_t)1 << 17);
     LAUNCH(ba, ba_post_kernel, 1, wide ? 32 : 1024, 0, d, wide ? 1 : 0);
@@ -2333,7 +2006,7 @@ static int upload_state(lvb_ba* ba, const lvb_solve_options* o, double radius_ov
 }
 
 static void apply_schur_mode(lvb_ba* ba, int mode) {
-    const int m = (mode == 1 && ba->tc_ok) ? 1 : 0;
+    const int m = (mode == 1 && ba->plan.tc_ok) ? 1 : 0;
     ba->dev.tc_mode = m;
     if (ba->pass_graph && ba->graph_mode != m) drop_graph(ba);
     ba->graph_mode = m;
@@ -2341,7 +2014,7 @@ static void apply_schur_mode(lvb_ba* ba, int mode) {
 
 static int require_solvable(lvb_ba* ba) {
     if (!ba->finalized) { set_error("finalize first"); return LVB_ERR_STATE; }
-    if (!ba->solvable) { set_error("camera system of dimension %d cannot be solved: %s", ba->dimc, ba->unsolvable_why); return LVB_ERR_UNSUPPORTED; }
+    if (!ba->plan.solvable) { set_error("camera system of dimension %d cannot be solved: %s", ba->plan.dimc, ba->plan.unsolvable_why); return LVB_ERR_UNSUPPORTED; }
     return check_imu_status(ba);
 }
 
@@ -2352,10 +2025,10 @@ int lvb_ba_reduced_system(lvb_ba* ba, double radius, double* S, double* b, doubl
     LVB_TRY(upload_state(ba, nullptr, radius));
     LVB_TRY(launch_clear(ba));
     LVB_TRY(launch_linearize_and_reduce(ba, true));
-    const int n = ba->dimc;
+    const int n = ba->plan.dimc;
     if ((size_t)n > 8192) { set_error("lvb_ba_reduced_system: dimension %d is too large for a dense download", n); return LVB_ERR_UNSUPPORTED; }
-    std::vector<double> hS(ba->nS);
-    const size_t srow = (size_t)ba->srow, soff = (size_t)ba->soff; const int band = (ba->soff == 0) ? n : ba->band;
+    std::vector<double> hS(ba->plan.nS);
+    const size_t srow = (size_t)ba->plan.srow, soff = (size_t)ba->plan.soff; const int band = (ba->plan.soff == 0) ? n : ba->plan.band;
     auto at = [&](int i, int j) { return (i - j <= band) ? hS[(size_t)i * srow + j + soff] : 0.0; };   // i >= j
     LmState h;
     cudaStream_t s = ba->ctx->stream;
@@ -2364,7 +2037,7 @@ int lvb_ba_reduced_system(lvb_ba* ba, double radius, double* S, double* b, doubl
     LVB_CUDA(cudaMemcpyAsync(&h, ba->st.p, sizeof(h), cudaMemcpyDeviceToHost, s));
     LVB_CUDA(cudaStreamSynchronize(s));
     // hand the system back in the caller-visible order (all poses, then all vec3 blocks)
-    const std::vector<int>& cn = ba->canon;
+    const std::vector<int>& cn = ba->plan.canon;
     if (S) for (int i = 0; i < n; ++i) for (int j = 0; j < n; ++j) S[(size_t)cn[i] * n + cn[j]] = (j <= i) ? at(i, j) : at(j, i);
     if (b) { std::vector<double> hb(b, b + n); for (int i = 0; i < n; ++i) b[cn[i]] = hb[i]; }
     if (cost) *cost = h.x_cost;
@@ -2392,7 +2065,7 @@ int lvb_ba_solve(lvb_ba* ba, const lvb_solve_options* options, lvb_solve_summary
     // The pass is a fixed sequence of launches whose kernels all read their control flags from the device state,
     // so it is captured once into a CUDA graph and replayed; the host looks at the state only every
     // `check_every` passes (kernels of a finished solve return immediately).
-    const bool graph_ok = comm_graph_safe(ba->ctx, ba->nS + 3 * (size_t)ba->dimc + 16) && ba->ctx->use_graph && !g_timing;
+    const bool graph_ok = comm_graph_safe(ba->ctx, ba->plan.nS + 3 * (size_t)ba->plan.dimc + 16) && ba->ctx->use_graph && !g_timing;
     const int check_every = std::max(1, ba->ctx->check_every);
     const bool capped = opt.max_solver_time_in_seconds < 1e8;
     int pass = 0;
@@ -2490,40 +2163,25 @@ LVB_API int lvb_debug_band_solve(lvb_ctx* ctx, int n, int band, const double* S_
     lvb_ba ba;
     ba.ctx = ctx;
     cudaStream_t s = ctx->stream;
-    ba.dimc = n; ba.band = band; ba.srow = band; ba.soff = band; ba.nS = (size_t)n * (band + 1);
-    LVB_TRY(ba.arena.ensure(ba.nS + n));
-    LVB_CUDA(cudaMemcpyAsync(ba.arena.p, S_band, ba.nS * sizeof(double), cudaMemcpyHostToDevice, s));
-    LVB_CUDA(cudaMemcpyAsync(ba.arena.p + ba.nS, b, (size_t)n * sizeof(double), cudaMemcpyHostToDevice, s));
+    BaPlan& P = ba.plan;
+    P.dimc = n; P.band = band; P.srow = band; P.soff = band; P.nS = (size_t)n * (band + 1);
+    LVB_TRY(ba.arena.ensure(P.nS + n));
+    LVB_CUDA(cudaMemcpyAsync(ba.arena.p, S_band, P.nS * sizeof(double), cudaMemcpyHostToDevice, s));
+    LVB_CUDA(cudaMemcpyAsync(ba.arena.p + P.nS, b, (size_t)n * sizeof(double), cudaMemcpyHostToDevice, s));
     LVB_TRY(ba.chol_invd.ensure(n + 32));
     LVB_TRY(ba.st.ensure(1));
     lvb_solve_options opt; lvb_default_options(&opt);
     LmState h; lm_init(h, opt);
     const double one = 1.0; memcpy(&h.grad_max_bits, &one, sizeof(double));        // not converged: the pre-check lets the solve run
     LVB_CUDA(cudaMemcpyAsync(ba.st.p, &h, sizeof(h), cudaMemcpyHostToDevice, s));
-    const int nstep = (n + 31) / 32;
-    std::vector<int> rmax(nstep + 2, 0), cmin(nstep + 2, 0);
-    int panel_rows = 2;
-    for (int st = 0; st < nstep; ++st) {
-        const int kb = st * 32, bs = std::min(32, n - kb);
-        rmax[st] = std::min(n - 1, kb + band); cmin[st] = std::max(0, kb + bs - 1 - band);
-        panel_rows = std::max(panel_rows, rmax[st] - (kb + bs) + 2);
-    }
-    LVB_TRY(ba.chol_rmax.upload(rmax.data(), rmax.size(), s)); LVB_TRY(ba.chol_cmin.upload(cmin.data(), cmin.size(), s));
-    ba.chol_smem = (size_t)(CHOL_HDR + std::max(panel_rows + 2, 34) * 34) * 8;
-    std::vector<Front> fr; size_t pool = 0; int rows = 0, mnb = 0, max_leaves = 1;
-    while (max_leaves * 2 <= std::max(2, ctx->sm_count)) max_leaves *= 2;
-    ba.tree_levels = 0;
-    if (use_tree) {
-        const int lv = build_front_tree(n, band, band - 31, max_leaves, fr, ba.level_first, ba.level_count, pool, rows, mnb);
-        ba.tree_factor_smem = (size_t)(32 * 33 + 32 + 128 + (rows + 2) * 34) * 8; ba.tree_back_smem = (size_t)(((mnb + 1) & ~1) + (CHOL_T / 32) * 32) * 8;
-        if (lv > 0 && ba.tree_factor_smem <= 227 * 1024 - 256) { ba.tree_levels = lv; LVB_TRY(ba.fronts.upload(fr.data(), fr.size(), s)); LVB_TRY(ba.front_pool.ensure(pool)); }
-    }
-    if (levels_out) *levels_out = ba.tree_levels;
-    ba.wide_solver = ba.tree_levels == 0 && ba.chol_smem > 227 * 1024 - 256;      // ba_wide.cuh
-    ba.h_rmax = rmax;
+    uniform_band_envelope(n, band, P.chol_rmax, P.chol_cmin);
+    LVB_TRY(ba.chol_rmax.upload(P.chol_rmax.data(), P.chol_rmax.size(), s)); LVB_TRY(ba.chol_cmin.upload(P.chol_cmin.data(), P.chol_cmin.size(), s));
+    P.solver = plan_reduced_solver(n, band, tree_sep_band_switch() ? band : band - 31, P.chol_rmax, ctx->sm_count, !use_tree);
+    if (P.solver.tree_levels > 0) { LVB_TRY(ba.fronts.upload(P.solver.fronts.data(), P.solver.fronts.size(), s)); LVB_TRY(ba.front_pool.ensure(P.solver.pool_doubles)); }
+    if (levels_out) *levels_out = P.solver.tree_levels;
     BaDev& d = ba.dev;
     memset(&d, 0, sizeof(d));
-    d.dimc = n; d.srow = ba.srow; d.soff = ba.soff; d.nS = ba.nS; d.S = ba.arena.p; d.rhs = ba.arena.p + ba.nS; d.st = ba.st.p;
+    d.dimc = n; d.srow = P.srow; d.soff = P.soff; d.nS = P.nS; d.S = ba.arena.p; d.rhs = ba.arena.p + P.nS; d.st = ba.st.p;
     LVB_TRY(launch_reduced_solve(&ba));
     LVB_TRY(check_launch("band solve"));
     LVB_CUDA(cudaMemcpyAsync(x, d.rhs, (size_t)n * sizeof(double), cudaMemcpyDeviceToHost, s));

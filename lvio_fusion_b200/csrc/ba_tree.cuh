@@ -16,17 +16,7 @@
 // the same number of launches, root first, back-substitute.  Own x own blocks are factored in place in the banded storage of S
 // (a separator of width w = B fits inside the band), border rows live in a pool.
 #pragma once
-
-struct Front {
-    int o0, m;              // own unknowns [o0, o0 + m)
-    int wL, wR;             // widths of the bounding ancestor separators (0 at the ends of the trajectory)
-    int bL0, bR0;           // their first unknowns
-    int actR;               // own column from which the right-border rows can be non-zero (leaves: m - band; internal: 0)
-    int child0, child1;     // front ids, -1 for leaves
-    int parent, side;       // parent front id (-1: root) and which child this is (0: left, 1: right)
-    int ld, nb;             // border array: (nb + 1) rows (borders, then the rhs row) x ld (= m own columns + nb border columns)
-    long long bd;           // offset of the border array in the pool (doubles)
-};
+#include "ba_plan.h"        // struct Front, CHOL_T; the tree itself is built there (build_front_tree)
 
 #define SG(i_, j_) S[(size_t)(i_) * (size_t)srow + (size_t)(j_) + (size_t)soff]
 
