@@ -223,8 +223,8 @@ inline void solve(const ceres::Solver::Options& options, ceres::Problem* problem
     if (gradient_max_norm() <= options.gradient_tolerance) { summary->termination_type = ceres::CONVERGENCE; return; }
     while (true) {
         if (elapsed() >= options.max_solver_time_in_seconds) break;
+        if (iter >= options.max_num_iterations) break;        // before the gradient rule, as in Ceres and the device loop
         if (iter > 0 && last_successful && gradient_max_norm() <= options.gradient_tolerance) { summary->termination_type = ceres::CONVERGENCE; break; }
-        if (iter >= options.max_num_iterations) break;
         if (radius <= 1e-32) { summary->termination_type = ceres::CONVERGENCE; break; }
         ++iter;
         last_successful = false;

@@ -2101,7 +2101,10 @@ int lvb_ba_solve(lvb_ba* ba, const lvb_solve_options* options, lvb_solve_summary
             const bool own = ba->solves_done >= 1 || !cx->use_graph_cache;      // a reused problem keeps a graph of its own
             if (!own && cx->graph_cache) {
                 cudaGraphExecUpdateResultInfo info;
-                if (cudaGraphExecUpdate(cx->graph_cache, g, &info) == cudaSuccess) { ba->pass_graph = cx->graph_cache; ba->graph_borrowed = true; cx->graph_owner = ba; }
+                if (cudaGraphExecUpdate(cx->graph_cache, g, &info) == cudaSuccess) {
+                    ba->pass_graph = cx->graph_cache; ba->graph_borrowed = true; cx->graph_owner = ba;
+                    if (prof_on) fprintf(stderr, "[solve] cached graph re-targeted\n");
+                }
                 else { cudaGetLastError(); cudaGraphExecDestroy(cx->graph_cache); cx->graph_cache = nullptr; cx->graph_owner = nullptr; }
             }
             if (!ba->pass_graph) {

@@ -145,8 +145,11 @@ __device__ inline void lm_control_pre(LmState& s) {
     if (s.need_linearize) { s.x_cost = s.cost_acc; if (s.iter == 0 && s.num_successful == 0 && s.scale_valid == 0) s.initial_cost = s.x_cost; }
     s.scale_valid = 1;
     const double gmax = __longlong_as_double((long long)*(volatile unsigned long long*)&s.grad_max_bits);   // written with atomics: read at L2
-    if ((s.iter == 0 || s.last_successful) && gmax <= s.g_tol) { s.done = 1; s.termination = 0; return; }
+    // the gradient at the start point is checked before any limit; after a step, Ceres checks the iteration limit first
+    // (time, iterations, gradient, radius), so a solve capped on the step that also reaches gradient_tolerance is NO_CONVERGENCE
+    if (s.iter == 0 && gmax <= s.g_tol) { s.done = 1; s.termination = 0; return; }
     if (s.iter >= s.max_iter) { s.done = 1; return; }
+    if (s.last_successful && gmax <= s.g_tol) { s.done = 1; s.termination = 0; return; }
     if (s.radius <= s.min_radius) { s.done = 1; s.termination = 0; return; }
     s.iter += 1;
     s.last_successful = 0;
