@@ -34,7 +34,9 @@ namespace {
 
 enum { TPB = 128, IMU_STRIDE = 17 + 45 + 225 + 1, MAX_STAGE_POSES = 512, SYRK_ROWS = 64, SYRK_LD = 14 };
 
-__device__ long long g_chol_dbg[8];     // accumulated SM clocks per Cholesky phase (diag, panel, trailing, backward, total)
+// accumulated SM clocks per Cholesky phase: diag, panel, trailing, backward, total, calls; then the resident kernel's load phase
+// (warps 1..7, overlapping warp 0's first diagonal block) and its calls
+__device__ long long g_chol_dbg[8];
 __device__ unsigned char c_tri_a[465];   // lower-triangle enumeration e -> (a, b), a >= b; global (not __constant__):
 __device__ unsigned char c_tri_b[465];   // the index differs per lane and would serialise on the constant cache
 
@@ -1006,27 +1008,71 @@ __global__ void lm_control_pre_kernel(LmState* st) { lm_control_pre(*st); }
 //                the rhs row;  named barrier (warp 0 only arrives, once its head rows are in shared memory);  trailing update of
 //                everything but diagonal block k + 1
 // so the pivot chain of block k + 1 overlaps the panel and the trailing update of step k instead of following them.
+//
+// The schedule runs on one of two storages of S.  kResident = false: S in global memory (in practice L2), each panel copied to the
+// shared buffer P.  kResident = true (the windows, whenever plan_reduced_solver finds that the envelope fits): warps 1..7 load the
+// envelope into shared memory once (chol_resident_columns, ba_plan.h) while warp 0 factors diagonal block 0 from global memory;
+// the panel of step k is then block column k itself, the rhs a shared vector, and only x goes back to global memory.  Nothing reads
+// the factor after the solve (S is rebuilt from Hpp on every pass), so the two storages compute the same x with the same arithmetic.
 #define SA(i_, j_) S[(size_t)(i_) * (size_t)srow + (size_t)(j_) + (size_t)soff]
+struct CholGlobal {               // element (i, j) of S in global memory
+    double* S; long long srow, soff;
+    __device__ __forceinline__ double* at(int i, int j) const { return S + ((size_t)i * (size_t)srow + (size_t)j + (size_t)soff); }
+};
+struct CholResident {             // element (i, j) of block column k = j / 32 in shared memory: rows kb .. rmax[k], row stride 34
+    double* col; const int* boff;
+    __device__ __forceinline__ double* at(int i, int j) const { const int k = j >> 5; return col + boff[k] + (i - (k << 5)) * 34 + (j & 31); }
+};
+
+template <bool kResident>
 __global__ void __launch_bounds__(CHOL_T) ba_cholesky_kernel(double* __restrict__ S, double* __restrict__ rhs, int n, long long srow, long long soff,
                                                                   double* __restrict__ invd_g, LmState* st, int run_control_pre,
                                                                   const int* __restrict__ env_rmax, const int* __restrict__ env_cmin) {
     if (run_control_pre) { if (threadIdx.x == 0) lm_control_pre(*st); __syncthreads(); }
     if (st->done) return;
     extern __shared__ __align__(16) double sm[];
-    double* P = sm + CHOL_HDR;         // rows x 34 panel (16 B aligned rows for broadcast double2 loads)
     __shared__ int fail;
-    const int tid = threadIdx.x, nt = blockDim.x, lane = tid & 31, warp = tid >> 5, nw = nt >> 5;
+    __shared__ int boff[CHOL_RES_STEPS];
+    __shared__ long long t_load;
+    constexpr int nt = CHOL_T, nw = CHOL_T / 32;       // launched with CHOL_T threads; constants keep registers free
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    // global memory: P is the rows x 34 panel (16 B aligned rows for broadcast double2 loads), later the backward partial sums.
+    // resident: the partial sums (nw x 32), the rhs, then the block columns.
+    double* const part = sm + CHOL_HDR;
+    double* const R = kResident ? part + CHOL_T : rhs;
+    const CholGlobal G{S, srow, soff};
+    const auto W = [&] { if constexpr (kResident) return CholResident{R + ((n + 1) & ~1), boff}; else return G; }();   // chol_resident_rhs
     if (tid == 0) fail = 0;
     long long t_diag = 0, t_panel = 0, t_trail = 0, t0 = clock64(), tA;
     const long long t_begin = t0;
-    // ---- diagonal block 0: warp 0, one row per lane in registers (lvb_chol.cuh)
+    // ---- diagonal block 0: warp 0, one row per lane in registers (lvb_chol.cuh), from global memory in both storages
     if (warp == 0) {
         const int b0 = min(32, n);
         double a[32];
 #pragma unroll
-        for (int j = 0; j < 32; ++j) a[j] = (lane < b0 && j <= lane) ? SA(lane, j) : ((j == lane) ? 1.0 : 0.0);
+        for (int j = 0; j < 32; ++j) a[j] = (lane < b0 && j <= lane) ? *G.at(lane, j) : ((j == lane) ? 1.0 : 0.0);
         const int bad = chol_diag32_pair(a, lane, sm, sm + 32 * 34);
         if (bad && lane == 0) fail = 1;
+    } else if constexpr (kResident) {
+        // ---- load: the rhs and the envelope, all of S the solve touches (upper triangles of the diagonal blocks and columns past n
+        // as zeros); batches of 8 independent loads per thread
+        const int t1 = tid - 32, n1 = nt - 32;
+        for (int i = t1; i < n; i += n1) R[i] = rhs[i];
+        int o = 0;
+        for (int kb = 0; kb < n; kb += 32) {
+            const int cnt = (env_rmax[kb >> 5] - kb + 1) * 32;
+            if (t1 == 0) boff[kb >> 5] = o;
+            double* dst = W.col + o;
+            for (int e0 = t1; e0 < cnt; e0 += 8 * n1) {
+                double v[8];
+#pragma unroll
+                for (int u = 0; u < 8; ++u) { const int e = e0 + u * n1, r = e >> 5, c = e & 31; v[u] = (e < cnt && c <= r && kb + c < n) ? *G.at(kb + r, kb + c) : 0.0; }
+#pragma unroll
+                for (int u = 0; u < 8; ++u) { const int e = e0 + u * n1; if (e < cnt) dst[(e >> 5) * 34 + (e & 31)] = v[u]; }
+            }
+            o += cnt / 32 * 34;
+        }
+        if (t1 == 0) t_load = clock64() - t0;
     }
     __syncthreads();
     tA = clock64(); t_diag += tA - t0; t0 = tA;
@@ -1039,15 +1085,18 @@ __global__ void __launch_bounds__(CHOL_T) ba_cholesky_kernel(double* __restrict_
         // panel rows: the rows below the block inside the envelope of this block column (S is block-banded by construction) + the rhs row (last)
         const int m = env_rmax[kb >> 5] - (kb + bs) + 1 + 1;
         const int mh = min(hb, m - 1);                             // head rows inside the envelope
+        // panel row rr < m - 1 at P + rr * 34, the rhs row at Prhs (resident: the panel is block column k below its diagonal block)
+        double* const P = kResident ? W.at(kb + bs, kb) : part;
+        double* const Prhs = kResident ? R + kb : P + (m - 1) * 34;
         if (warp == 0 && hb > 0) {
             double x[32], a[32];
 #pragma unroll
-            for (int j = 0; j < 32; ++j) x[j] = (lane < mh && j < bs) ? SA(kn + lane, kb + j) : 0.0;
+            for (int j = 0; j < 32; ++j) x[j] = (lane < mh && j < bs) ? W.at(kn + lane, kb)[j] : 0.0;
 #pragma unroll
-            for (int j = 0; j < 32; ++j) a[j] = (lane < hb && j <= lane) ? SA(kn + lane, kn + j) : ((j == lane) ? 1.0 : 0.0);
+            for (int j = 0; j < 32; ++j) a[j] = (lane < hb && j <= lane) ? W.at(kn + lane, kn)[j] : ((j == lane) ? 1.0 : 0.0);
             chol_panel_row(x, Dt, invd);
 #pragma unroll
-            for (int j = 0; j < 32; ++j) if (lane < mh) { P[lane * 34 + j] = x[j]; if (j < bs) SA(kn + lane, kb + j) = x[j]; }
+            for (int j = 0; j < 32; ++j) if (lane < mh) { P[lane * 34 + j] = x[j]; if (!kResident && j < bs) W.at(kn + lane, kb)[j] = x[j]; }
             __syncwarp();
             asm volatile("bar.arrive 1, %0;" :: "r"(nt) : "memory");
             tA = clock64(); t_panel += tA - t0; t0 = tA;
@@ -1103,18 +1152,18 @@ __global__ void __launch_bounds__(CHOL_T) ba_cholesky_kernel(double* __restrict_
                 for (int j = 0; j < 32; ++j) e[j] = (j == lane) ? 1.0 : 0.0;
                 chol_panel_row(e, Dt, invd);
 #pragma unroll
-                for (int j = 0; j < 32; ++j) if (j >= lane && j < bs) SA(kb + j, kb + lane) = e[j];
+                for (int j = 0; j < 32; ++j) if (j >= lane && j < bs) W.at(kb + j, kb)[lane] = e[j];
             }
             // ---- panel, the rows warp 0 does not take:  x L^T = a, right-looking, no divisions
             for (int rr = mh + t2; rr < m; rr += nt2) {
                 const bool is_rhs = (rr == m - 1);
-                double* src = is_rhs ? (rhs + kb) : &SA(kb + bs + rr, kb);
+                double* src = is_rhs ? (R + kb) : W.at(kb + bs + rr, kb);
                 double a[32];
     #pragma unroll
                 for (int j = 0; j < 32; ++j) a[j] = (j < bs) ? src[j] : 0.0;
                 chol_panel_row(a, Dt, invd);
     #pragma unroll
-                for (int j = 0; j < 32; ++j) { P[rr * 34 + j] = a[j]; if (j < bs) src[j] = a[j]; }
+                for (int j = 0; j < 32; ++j) { if (!kResident) P[rr * 34 + j] = a[j]; if (j < bs) src[j] = a[j]; }
             }
             asm volatile("bar.sync 1, %0;" :: "r"(nt) : "memory");
             // ---- trailing update A22 -= P P^T on the lower triangle.  One warp per 32x32 tile, each lane a 4x8
@@ -1140,9 +1189,9 @@ __global__ void __launch_bounds__(CHOL_T) ba_cholesky_kernel(double* __restrict_
                 // rows / columns beyond the panel read row 0 (valid memory) and are masked at the store
                 const double2* rp[4]; const double2* cp[8];
     #pragma unroll
-                for (int i = 0; i < 4; ++i) rp[i] = reinterpret_cast<const double2*>(P + (size_t)min(r0 + 8 * i, m - 1) * 34);
+                for (int i = 0; i < 4; ++i) { const int ri = min(r0 + 8 * i, m - 1); rp[i] = reinterpret_cast<const double2*>(ri == m - 1 ? Prhs : P + (size_t)ri * 34); }
     #pragma unroll
-                for (int j = 0; j < 8; ++j) cp[j] = reinterpret_cast<const double2*>(P + (size_t)min(c0 + 4 * j, m - 1) * 34);
+                for (int j = 0; j < 8; ++j) { const int ci = min(c0 + 4 * j, m - 1); cp[j] = reinterpret_cast<const double2*>(ci == m - 1 ? Prhs : P + (size_t)ci * 34); }
     #pragma unroll 2
                 for (int k = 0; k < 16; ++k) {
                     double2 rv[4], cv[8];
@@ -1155,22 +1204,24 @@ __global__ void __launch_bounds__(CHOL_T) ba_cholesky_kernel(double* __restrict_
     #pragma unroll
                         for (int j = 0; j < 8; ++j) { acc[i][j] += rv[i].x * cv[j].x; acc[i][j] += rv[i].y * cv[j].y; }
                 }
-                // read-modify-write of the tile: all loads first (one round trip), then the stores
+                // read-modify-write of the tile: all loads first (one round trip), then the stores.  src / dst point at the tile's
+                // first column (tj * 32 past the panel): the tile lies in one block column of the resident storage.
                 double cur[4][8];
+                const int tc = kb + bs + tj * 32;
     #pragma unroll
                 for (int i = 0; i < 4; ++i) {
                     const int ip = min(r0 + 8 * i, m - 1);
-                    const double* src = (ip == m - 1) ? (rhs + kb + bs) : &SA(kb + bs + ip, kb + bs);
+                    const double* src = (ip == m - 1) ? (R + tc) : W.at(kb + bs + ip, tc);
     #pragma unroll
-                    for (int j = 0; j < 8; ++j) { const int jp = c0 + 4 * j; cur[i][j] = (r0 + 8 * i < m && r0 + 8 * i >= row_lo && jp < m - 1 && jp <= ip) ? src[jp] : 0.0; }
+                    for (int j = 0; j < 8; ++j) { const int jp = c0 + 4 * j; cur[i][j] = (r0 + 8 * i < m && r0 + 8 * i >= row_lo && jp < m - 1 && jp <= ip) ? src[cx + 4 * j] : 0.0; }
                 }
     #pragma unroll
                 for (int i = 0; i < 4; ++i) {
                     const int ip = r0 + 8 * i;
                     if (ip >= m || ip < row_lo) continue;
-                    double* dst = (ip == m - 1) ? (rhs + kb + bs) : &SA(kb + bs + ip, kb + bs);
+                    double* dst = (ip == m - 1) ? (R + tc) : W.at(kb + bs + ip, tc);
     #pragma unroll
-                    for (int j = 0; j < 8; ++j) { const int jp = c0 + 4 * j; if (jp < m - 1 && jp <= ip) dst[jp] = cur[i][j] - acc[i][j]; }
+                    for (int j = 0; j < 8; ++j) { const int jp = c0 + 4 * j; if (jp < m - 1 && jp <= ip) dst[cx + 4 * j] = cur[i][j] - acc[i][j]; }
                 }
             }
         }
@@ -1182,7 +1233,6 @@ __global__ void __launch_bounds__(CHOL_T) ba_cholesky_kernel(double* __restrict_
     // the sum is a GEMV over the envelope rows spread over all warps (independent coalesced loads, one L2 round trip per
     // batch), then warp 0 applies the inverse diagonal block: 32 independent FMAs per lane, no substitution chain.  x overwrites rhs.
     const int last = ((n - 1) / 32) * 32;
-    double* part = P;                                 // nw x 32 partial sums
     for (int kb = last; kb >= 0; kb -= 32) {
         const int bs = min(32, n - kb);
         const int rend = env_rmax[kb >> 5];
@@ -1190,15 +1240,15 @@ __global__ void __launch_bounds__(CHOL_T) ba_cholesky_kernel(double* __restrict_
         double t = 0.0;
         if (warp == 0) {
 #pragma unroll
-            for (int i = 0; i < 32; ++i) col[i] = (i < bs && lane < bs && i >= lane) ? SA(kb + i, kb + lane) : 0.0;
-            if (lane < bs) t = rhs[kb + lane];
+            for (int i = 0; i < 32; ++i) col[i] = (i < bs && lane < bs && i >= lane) ? W.at(kb + i, kb)[lane] : 0.0;
+            if (lane < bs) t = R[kb + lane];
         }
         double acc = 0.0;
         if (lane < bs) {
             for (int r0 = kb + bs + warp; r0 <= rend; r0 += 16 * nw) {
                 double lv[16], xv[16];
 #pragma unroll
-                for (int u = 0; u < 16; ++u) { const int r = r0 + u * nw; const bool ok = r <= rend; lv[u] = ok ? SA(r, kb + lane) : 0.0; xv[u] = ok ? rhs[r] : 0.0; }
+                for (int u = 0; u < 16; ++u) { const int r = r0 + u * nw; const bool ok = r <= rend; lv[u] = ok ? W.at(r, kb)[lane] : 0.0; xv[u] = ok ? R[r] : 0.0; }
 #pragma unroll
                 for (int u = 0; u < 16; ++u) acc += lv[u] * xv[u];
             }
@@ -1217,12 +1267,16 @@ __global__ void __launch_bounds__(CHOL_T) ba_cholesky_kernel(double* __restrict_
                 y3 = fma(col[j + 3], __shfl_sync(0xffffffffu, t, j + 3), y3);
             }
             t = (y0 + y1) + (y2 + y3);
-            if (lane < bs) rhs[kb + lane] = t;
+            if (lane < bs) R[kb + lane] = t;
         }
         __syncthreads();
     }
+    if (kResident) for (int i = tid; i < n; i += nt) rhs[i] = R[i];
     if (tid == 0 && fail) st->solve_fail = 1;
-    if (tid == 0) { tA = clock64(); g_chol_dbg[0] += t_diag; g_chol_dbg[1] += t_panel; g_chol_dbg[2] += t_trail; g_chol_dbg[3] += tA - t0; g_chol_dbg[4] += tA - t_begin; g_chol_dbg[5] += 1; }
+    if (tid == 0) {
+        tA = clock64(); g_chol_dbg[0] += t_diag; g_chol_dbg[1] += t_panel; g_chol_dbg[2] += t_trail; g_chol_dbg[3] += tA - t0; g_chol_dbg[4] += tA - t_begin; g_chol_dbg[5] += 1;
+        if (kResident) { g_chol_dbg[6] += t_load; g_chol_dbg[7] += 1; }
+    }
 }
 
 #include "ba_tree.cuh"
@@ -1425,7 +1479,8 @@ static int init_tables() {
     for (int i = 0; i < 30; ++i) for (int j = 0; j <= i; ++j) { a[e] = (unsigned char)i; b[e] = (unsigned char)j; ++e; }
     LVB_CUDA(cudaMemcpyToSymbol(c_tri_a, a, sizeof(a)));
     LVB_CUDA(cudaMemcpyToSymbol(c_tri_b, b, sizeof(b)));
-    LVB_CUDA(cudaFuncSetAttribute(ba_cholesky_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, MAX_CTA_SMEM));
+    LVB_CUDA(cudaFuncSetAttribute(ba_cholesky_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, MAX_CTA_SMEM));
+    LVB_CUDA(cudaFuncSetAttribute(ba_cholesky_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, MAX_CTA_SMEM));
     LVB_CUDA(cudaFuncSetAttribute(ba_front_factor_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, MAX_CTA_SMEM));
     LVB_CUDA(cudaFuncSetAttribute(ba_front_backward_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 64 * 1024));
     LVB_CUDA(cudaFuncSetAttribute(ba_eval_two_frame_kernel<1, 5>, cudaFuncAttributeMaxDynamicSharedMemorySize, (TPB * 31 + MAX_STAGE_POSES * 7 + 2) * 8));
@@ -1969,8 +2024,10 @@ static int launch_reduced_solve(lvb_ba* ba) {
             LAUNCH(ba, ba_front_backward_kernel, sp.level_count[l], CHOL_T, sp.tree_back_smem, fr, sp.level_first[l], d.S, d.rhs, ba->front_pool.p, d.srow, d.soff, band, ba->chol_invd.p, d.st);
     } else if (sp.wide) {
         LVB_TRY(launch_wide_solve(ba));
+    } else if (sp.resident) {
+        LAUNCH_AS(ba, "ba_cholesky_kernel", ba_cholesky_kernel<true>, 1, CHOL_T, sp.resident_smem, d.S, d.rhs, d.dimc, d.srow, d.soff, ba->chol_invd.p, d.st, 1, ba->chol_rmax.p, ba->chol_cmin.p);
     } else
-    LAUNCH(ba, ba_cholesky_kernel, 1, CHOL_T, sp.chol_smem, d.S, d.rhs, d.dimc, d.srow, d.soff, ba->chol_invd.p, d.st, 1, ba->chol_rmax.p, ba->chol_cmin.p);
+    LAUNCH_AS(ba, "ba_cholesky_kernel", ba_cholesky_kernel<false>, 1, CHOL_T, sp.chol_smem, d.S, d.rhs, d.dimc, d.srow, d.soff, ba->chol_invd.p, d.st, 1, ba->chol_rmax.p, ba->chol_cmin.p);
     return LVB_OK;
 }
 

@@ -19,8 +19,20 @@
 namespace lvb {
 
 // MAX_CTA_SMEM: the 227 KB of dynamic shared memory one CTA may opt into on sm_90, less 256 B of headroom
+// CHOL_RES_STEPS: most 32-column steps of the resident single-CTA solve (its table of block-column offsets)
 enum { MAX_DIMC = 736, MAX_TRACK = 16, IMU_RAW = 469, CHOL_T = 256, CHOL_DT = 32 * 34 + 32, CHOL_HDR = 2 * CHOL_DT,      // doubles: (Dt, invd) twice, then the panel
-       MAX_CTA_SMEM = 227 * 1024 - 256 };
+       MAX_CTA_SMEM = 227 * 1024 - 256, CHOL_RES_STEPS = 32 };
+
+// Shared memory of the resident single-CTA solve, in doubles after the (Dt, invd) pair: the backward partial sums (CHOL_T), the rhs
+// (n, padded to an even count), then block column k = rows kb .. rmax[k] x 32 columns at a row stride of 34 doubles (16-byte rows, as
+// the panel of the global-memory kernel).  rmax is non-decreasing and >= the step's last column, so every trailing tile of step k
+// lands inside the stored rows of its block column.  Returns the block-column area's size in doubles.
+inline long long chol_resident_columns(int n, const int* rmax) {
+    long long d = 0;
+    for (int kb = 0; kb < n; kb += 32) d += (long long)(rmax[kb >> 5] - kb + 1) * 34;
+    return d;
+}
+inline int chol_resident_rhs(int n) { return (n + 1) & ~1; }
 
 // per factor kind: doubles of one constant record and int32 indices of one block, as the caller adds them
 constexpr int kConstStride[6] = {5, 6, 5, IMU_RAW, 8, 9};
@@ -37,10 +49,13 @@ struct Front {
     long long bd;           // offset of the border array in the pool (doubles)
 };
 
-// How the reduced camera system is factored: the separator tree when it has levels (ba_tree.cuh), else the per-phase grids of
-// ba_wide.cuh when the single-CTA envelope kernel's panel does not fit in shared memory, else that kernel.
+// How the reduced camera system is factored: the separator tree when it has levels (ba_tree.cuh), else the single-CTA kernel with
+// the whole envelope resident in shared memory when it fits, else the single-CTA kernel on S in global memory when its panel fits,
+// else the per-phase grids of ba_wide.cuh.
 struct SolverPlan {
-    size_t chol_smem = 0;               // single-CTA kernel: two diagonal-block buffers + the panel (>= 34 rows; later the backward partial sums)
+    size_t chol_smem = 0;               // single-CTA kernel on S in global memory: two diagonal-block buffers + the panel (>= 34 rows; later the backward partial sums)
+    bool resident = false;              // single-CTA kernel with the envelope in shared memory
+    size_t resident_smem = 0;           // its dynamic shared memory (chol_resident_layout)
     int tree_levels = 0;                // 0: no separator tree
     std::vector<Front> fronts;
     std::vector<int> level_first, level_count;
@@ -437,16 +452,18 @@ inline int build_front_tree(int n, int band, int sep, int max_leaves, std::vecto
 
 // The one rule that picks the solver of an n x n system in banded storage of half bandwidth `band` with the envelope rmax (last
 // row per 32-column step): the single-CTA kernel's shared memory, then -- unless no_tree -- a separator tree with separators of
-// width `sep` when it has at least two leaves and its fronts and pool fit, then the wide solver when neither the tree nor the
-// single-CTA panel does.
+// width `sep` when it has at least two leaves and its fronts and pool fit; without a tree, the resident single-CTA solve when the
+// whole envelope fits in shared memory, the single-CTA solve on S in global memory when its panel fits, else the wide solver.
 inline SolverPlan plan_reduced_solver(int n, int band, int sep, const std::vector<int>& rmax, int sm_count, bool no_tree) {
     SolverPlan s;
     int panel_rows = 2;
-    for (int step = 0; step < (n + 31) / 32; ++step) {
+    const int nstep = (n + 31) / 32;
+    for (int step = 0; step < nstep; ++step) {
         const int kb = step * 32, bs = std::min(32, n - kb);
         panel_rows = std::max(panel_rows, rmax[step] - (kb + bs) + 2);
     }
     s.chol_smem = (size_t)(CHOL_HDR + std::max(panel_rows + 2, 34) * 34) * 8;
+    s.resident_smem = (size_t)(CHOL_HDR + CHOL_T + chol_resident_rhs(n) + chol_resident_columns(n, rmax.data())) * 8;
     if (!no_tree) {
         int rows = 0, mnb = 0, max_leaves = 1;
         while (max_leaves * 2 <= std::max(2, sm_count)) max_leaves *= 2;
@@ -454,7 +471,8 @@ inline SolverPlan plan_reduced_solver(int n, int band, int sep, const std::vecto
         const size_t fs = (size_t)(32 * 33 + 32 + 128 + (rows + 2) * 34) * 8, bs = (size_t)(((mnb + 1) & ~1) + (CHOL_T / 32) * 32) * 8;
         if (lv > 0 && fs <= MAX_CTA_SMEM && s.pool_doubles < ((size_t)1 << 31)) { s.tree_levels = lv; s.tree_factor_smem = fs; s.tree_back_smem = bs; }
     }
-    s.wide = s.tree_levels == 0 && s.chol_smem > MAX_CTA_SMEM;
+    s.resident = s.tree_levels == 0 && nstep <= CHOL_RES_STEPS && s.resident_smem <= MAX_CTA_SMEM;
+    s.wide = s.tree_levels == 0 && !s.resident && s.chol_smem > MAX_CTA_SMEM;
     return s;
 }
 

@@ -21,5 +21,6 @@ for n, tb in ((150, 149), (300, 299), (300, 91), (47, 46), (95, 20), (129, 128),
     lvb.check(lvb.debug_cholesky_clocks(out, 1), "clocks")
     err = np.max(np.abs(x - want)) / np.max(np.abs(want)); res = np.max(np.abs(s @ x - b)) / np.max(np.abs(b))
     worst = max(worst, err)
-    print("n=%4d band=%4d  err %.1e resid %.1e   warp0: diag %6d panel %6d wait %6d   backward %6d  total %6d cycles %s" % (n, tb, err, res, out[0], out[1], out[2], out[3], out[4], "" if err < 1e-8 else "  <-- WRONG"))
+    print("n=%4d band=%4d %s err %.1e resid %.1e   load %6d  warp0: diag %6d panel %6d wait %6d   backward %6d  total %6d cycles %s"
+          % (n, tb, "resident" if out[7] else "global  ", err, res, out[6], out[0], out[1], out[2], out[3], out[4], "" if err < 1e-8 else "  <-- WRONG"))
 print("worst", worst)
