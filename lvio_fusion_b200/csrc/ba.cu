@@ -14,7 +14,7 @@
 //   K1  ba_eval_*            residual + ambient Jacobian materialised (parity / roofline entry)
 //   K1-K4 ba_linearize       fused evaluate + robustify + J^T J / J^T r assembly (atomics on the lower triangle)
 //   K5  ba_schur             eliminate the 1-dim inverse-depth blocks into S
-//   K6  ba_cholesky + ba_update + lm control   reduced solve, back-substitution, (+) update, LM decisions
+//   K6  reduced solve (ba_solve.cu) + ba_update + lm control   back-substitution, (+) update, LM decisions
 #include <math.h>
 #include <algorithm>
 #include <chrono>
@@ -25,7 +25,7 @@
 #include "lvb_internal.cuh"
 #include "lvb_math.cuh"
 #include "lvb_imu_warp.cuh"
-#include "lvb_chol.cuh"
+#include "ba_solve.h"
 #include "lvb_p2p.cuh"
 
 using namespace lvb;
@@ -34,9 +34,6 @@ namespace {
 
 enum { TPB = 128, IMU_STRIDE = 17 + 45 + 225 + 1, MAX_STAGE_POSES = 512, SYRK_ROWS = 64, SYRK_LD = 14 };
 
-// accumulated SM clocks per Cholesky phase: diag, panel, trailing, backward, total, calls; then the resident kernel's load phase
-// (warps 1..7, overlapping warp 0's first diagonal block) and its calls
-__device__ long long g_chol_dbg[8];
 __device__ unsigned char c_tri_a[465];   // lower-triangle enumeration e -> (a, b), a >= b; global (not __constant__):
 __device__ unsigned char c_tri_b[465];   // the index differs per lane and would serialise on the constant cache
 
@@ -993,295 +990,6 @@ __global__ void __launch_bounds__(256) ba_allreduce_fused_kernel(P2PArgs a, BaDe
     p2p_finish_epoch(a, epoch);
 }
 
-__global__ void lm_control_pre_kernel(LmState* st) { lm_control_pre(*st); }
-
-// ------------------------------------------------------------------ K6 dense Cholesky, one CTA
-// Right-looking blocked (32) factorisation of the lower triangle of S (n x n, row-major, in L2/HBM) with
-// the right-hand side carried along as an extra row (so the forward substitution is free), then a
-// blocked backward substitution.  Result: rhs <- S^-1 rhs.
-//
-// Schedule of one 32-column step k (look-ahead of depth one, the serial part on its own warp):
-//   warp 0     : panel solve of the 32 "head" rows (= the rows of diagonal block k + 1), one row per lane;  update of diagonal block
-//                k + 1 by these rows as one 32 x 32 register-tiled product, handed to the row-per-lane layout of the factorisation
-//                through shared memory (no trip through global memory);  factorisation of block k + 1 into the OTHER (Dt, invd) buffer
-//   warps 1..7 : the INVERSE of block k of L to the block's place in S (for the backward pass);  panel solve of the remaining rows +
-//                the rhs row;  named barrier (warp 0 only arrives, once its head rows are in shared memory);  trailing update of
-//                everything but diagonal block k + 1
-// so the pivot chain of block k + 1 overlaps the panel and the trailing update of step k instead of following them.
-//
-// The schedule runs on one of two storages of S.  kResident = false: S in global memory (in practice L2), each panel copied to the
-// shared buffer P.  kResident = true (the windows, whenever plan_reduced_solver finds that the envelope fits): warps 1..7 load the
-// envelope into shared memory once (chol_resident_columns, ba_plan.h) while warp 0 factors diagonal block 0 from global memory;
-// the panel of step k is then block column k itself, the rhs a shared vector, and only x goes back to global memory.  Nothing reads
-// the factor after the solve (S is rebuilt from Hpp on every pass), so the two storages compute the same x with the same arithmetic.
-#define SA(i_, j_) S[(size_t)(i_) * (size_t)srow + (size_t)(j_) + (size_t)soff]
-struct CholGlobal {               // element (i, j) of S in global memory
-    double* S; long long srow, soff;
-    __device__ __forceinline__ double* at(int i, int j) const { return S + ((size_t)i * (size_t)srow + (size_t)j + (size_t)soff); }
-};
-struct CholResident {             // element (i, j) of block column k = j / 32 in shared memory: rows kb .. rmax[k], row stride 34
-    double* col; const int* boff;
-    __device__ __forceinline__ double* at(int i, int j) const { const int k = j >> 5; return col + boff[k] + (i - (k << 5)) * 34 + (j & 31); }
-};
-
-template <bool kResident>
-__global__ void __launch_bounds__(CHOL_T) ba_cholesky_kernel(double* __restrict__ S, double* __restrict__ rhs, int n, long long srow, long long soff,
-                                                                  double* __restrict__ invd_g, LmState* st, int run_control_pre,
-                                                                  const int* __restrict__ env_rmax, const int* __restrict__ env_cmin) {
-    if (run_control_pre) { if (threadIdx.x == 0) lm_control_pre(*st); __syncthreads(); }
-    if (st->done) return;
-    extern __shared__ __align__(16) double sm[];
-    __shared__ int fail;
-    __shared__ int boff[CHOL_RES_STEPS];
-    __shared__ long long t_load;
-    constexpr int nt = CHOL_T, nw = CHOL_T / 32;       // launched with CHOL_T threads; constants keep registers free
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    // global memory: P is the rows x 34 panel (16 B aligned rows for broadcast double2 loads), later the backward partial sums.
-    // resident: the partial sums (nw x 32), the rhs, then the block columns.
-    double* const part = sm + CHOL_HDR;
-    double* const R = kResident ? part + CHOL_T : rhs;
-    const CholGlobal G{S, srow, soff};
-    const auto W = [&] { if constexpr (kResident) return CholResident{R + ((n + 1) & ~1), boff}; else return G; }();   // chol_resident_rhs
-    if (tid == 0) fail = 0;
-    long long t_diag = 0, t_panel = 0, t_trail = 0, t0 = clock64(), tA;
-    const long long t_begin = t0;
-    // ---- diagonal block 0: warp 0, one row per lane in registers (lvb_chol.cuh), from global memory in both storages
-    if (warp == 0) {
-        const int b0 = min(32, n);
-        double a[32];
-#pragma unroll
-        for (int j = 0; j < 32; ++j) a[j] = (lane < b0 && j <= lane) ? *G.at(lane, j) : ((j == lane) ? 1.0 : 0.0);
-        const int bad = chol_diag32_pair(a, lane, sm, sm + 32 * 34);
-        if (bad && lane == 0) fail = 1;
-    } else if constexpr (kResident) {
-        // ---- load: the rhs and the envelope, all of S the solve touches (upper triangles of the diagonal blocks and columns past n
-        // as zeros); batches of 8 independent loads per thread
-        const int t1 = tid - 32, n1 = nt - 32;
-        for (int i = t1; i < n; i += n1) R[i] = rhs[i];
-        int o = 0;
-        for (int kb = 0; kb < n; kb += 32) {
-            const int cnt = (env_rmax[kb >> 5] - kb + 1) * 32;
-            if (t1 == 0) boff[kb >> 5] = o;
-            double* dst = W.col + o;
-            for (int e0 = t1; e0 < cnt; e0 += 8 * n1) {
-                double v[8];
-#pragma unroll
-                for (int u = 0; u < 8; ++u) { const int e = e0 + u * n1, r = e >> 5, c = e & 31; v[u] = (e < cnt && c <= r && kb + c < n) ? *G.at(kb + r, kb + c) : 0.0; }
-#pragma unroll
-                for (int u = 0; u < 8; ++u) { const int e = e0 + u * n1; if (e < cnt) dst[(e >> 5) * 34 + (e & 31)] = v[u]; }
-            }
-            o += cnt / 32 * 34;
-        }
-        if (t1 == 0) t_load = clock64() - t0;
-    }
-    __syncthreads();
-    tA = clock64(); t_diag += tA - t0; t0 = tA;
-    for (int kb = 0; kb < n; kb += 32) {
-        const int bs = min(32, n - kb), kn = kb + 32;
-        const int hb = max(0, min(32, n - kn));                    // rows of the next diagonal block ("head" rows of the panel)
-        double* Dt = sm + ((kb >> 5) & 1) * CHOL_DT;               // block kb of L, column-major: Dt[j * 34 + k] = L[k][j]
-        double* invd = Dt + 32 * 34;
-        double* Dn = sm + (((kb >> 5) & 1) ^ 1) * CHOL_DT;
-        // panel rows: the rows below the block inside the envelope of this block column (S is block-banded by construction) + the rhs row (last)
-        const int m = env_rmax[kb >> 5] - (kb + bs) + 1 + 1;
-        const int mh = min(hb, m - 1);                             // head rows inside the envelope
-        // panel row rr < m - 1 at P + rr * 34, the rhs row at Prhs (resident: the panel is block column k below its diagonal block)
-        double* const P = kResident ? W.at(kb + bs, kb) : part;
-        double* const Prhs = kResident ? R + kb : P + (m - 1) * 34;
-        if (warp == 0 && hb > 0) {
-            double x[32], a[32];
-#pragma unroll
-            for (int j = 0; j < 32; ++j) x[j] = (lane < mh && j < bs) ? W.at(kn + lane, kb)[j] : 0.0;
-#pragma unroll
-            for (int j = 0; j < 32; ++j) a[j] = (lane < hb && j <= lane) ? W.at(kn + lane, kn)[j] : ((j == lane) ? 1.0 : 0.0);
-            chol_panel_row(x, Dt, invd);
-#pragma unroll
-            for (int j = 0; j < 32; ++j) if (lane < mh) { P[lane * 34 + j] = x[j]; if (!kResident && j < bs) W.at(kn + lane, kb)[j] = x[j]; }
-            __syncwarp();
-            asm volatile("bar.arrive 1, %0;" :: "r"(nt) : "memory");
-            tA = clock64(); t_panel += tA - t0; t0 = tA;
-            // diagonal block kn -= (head rows)(head rows)^T: computed as a 32 x 32 tile in the 4 x 8 register micro-tile layout of the
-            // trailing update (12 LDS.128 per 64 DFMA; the row-per-lane layout would need one LDS.128 per 2 DFMA and is bound by the
-            // shared-memory return path), then passed through the free diagonal-block buffer to the row-per-lane layout of the
-            // factorisation.  Head rows outside the envelope are structurally zero and have no panel row.
-            if (mh > 0) {
-                const int ry = lane >> 2, cx = lane & 3;
-                double acc[4][8];
-#pragma unroll
-                for (int i = 0; i < 4; ++i)
-#pragma unroll
-                    for (int j = 0; j < 8; ++j) acc[i][j] = 0.0;
-                const double2* rp[4]; const double2* cp[8];
-#pragma unroll
-                for (int i = 0; i < 4; ++i) rp[i] = reinterpret_cast<const double2*>(P + (size_t)min(ry + 8 * i, mh - 1) * 34);
-#pragma unroll
-                for (int j = 0; j < 8; ++j) cp[j] = reinterpret_cast<const double2*>(P + (size_t)min(cx + 4 * j, mh - 1) * 34);
-#pragma unroll 2
-                for (int k = 0; k < 16; ++k) {
-                    double2 rv[4], cv[8];
-#pragma unroll
-                    for (int i = 0; i < 4; ++i) rv[i] = rp[i][k];
-#pragma unroll
-                    for (int j = 0; j < 8; ++j) cv[j] = cp[j][k];
-#pragma unroll
-                    for (int i = 0; i < 4; ++i)
-#pragma unroll
-                        for (int j = 0; j < 8; ++j) { acc[i][j] += rv[i].x * cv[j].x; acc[i][j] += rv[i].y * cv[j].y; }
-                }
-#pragma unroll
-                for (int i = 0; i < 4; ++i)
-#pragma unroll
-                    for (int j = 0; j < 8; ++j) Dn[(ry + 8 * i) * 34 + cx + 4 * j] = (ry + 8 * i < mh && cx + 4 * j < mh) ? acc[i][j] : 0.0;
-                __syncwarp();
-#pragma unroll
-                for (int j = 0; j < 32; ++j) a[j] -= Dn[lane * 34 + j];
-                __syncwarp();
-            }
-            const int bad = chol_diag32_pair(a, lane, Dn, Dn + 32 * 34);
-            if (bad && lane == 0) fail = 1;
-            tA = clock64(); t_diag += tA - t0; t0 = tA;
-        } else {
-            const int wid = hb > 0 ? warp - 1 : warp, nwk = hb > 0 ? nw - 1 : nw;       // the warps doing this part
-            const int t2 = wid * 32 + lane, nt2 = nwk * 32;
-            // the INVERSE of block kb of L goes to the block's place in S: the backward pass then applies a diagonal block as 32 independent
-            // FMAs per lane instead of a 32-step substitution chain.  Column c of L^-1 is the panel solve of the unit row e_c; one warp
-            // (the last one, which has the fewest panel rows) does it while the others are in the panel.
-            if (wid == nwk - 1) {
-                double e[32];
-#pragma unroll
-                for (int j = 0; j < 32; ++j) e[j] = (j == lane) ? 1.0 : 0.0;
-                chol_panel_row(e, Dt, invd);
-#pragma unroll
-                for (int j = 0; j < 32; ++j) if (j >= lane && j < bs) W.at(kb + j, kb)[lane] = e[j];
-            }
-            // ---- panel, the rows warp 0 does not take:  x L^T = a, right-looking, no divisions
-            for (int rr = mh + t2; rr < m; rr += nt2) {
-                const bool is_rhs = (rr == m - 1);
-                double* src = is_rhs ? (R + kb) : W.at(kb + bs + rr, kb);
-                double a[32];
-    #pragma unroll
-                for (int j = 0; j < 32; ++j) a[j] = (j < bs) ? src[j] : 0.0;
-                chol_panel_row(a, Dt, invd);
-    #pragma unroll
-                for (int j = 0; j < 32; ++j) { if (!kResident) P[rr * 34 + j] = a[j]; if (j < bs) src[j] = a[j]; }
-            }
-            asm volatile("bar.sync 1, %0;" :: "r"(nt) : "memory");
-            // ---- trailing update A22 -= P P^T on the lower triangle.  One warp per 32x32 tile, each lane a 4x8
-            // register micro-tile (rows ry+8i, columns cx+4j: consecutive lanes touch consecutive panel rows, so the
-            // LDS.128 operand loads are bank-conflict free and every loaded value feeds 4 or 8 DFMAs).  The head rows of
-            // tile (0, 0) -- diagonal block kn -- are warp 0's.
-            const int ntile = (m + 31) >> 5;
-            const int total = (m > 1) ? ntile * (ntile + 1) / 2 : 0;
-            for (int t = wid; t < total; t += nwk) {
-                if (t == 0 && mh >= min(32, m)) continue;
-                int ti = (int)((sqrt(8.0 * t + 1.0) - 1.0) * 0.5);
-                while ((ti + 1) * (ti + 2) / 2 <= t) ++ti;
-                while (ti * (ti + 1) / 2 > t) --ti;
-                const int tj = t - ti * (ti + 1) / 2;
-                const int row_lo = (t == 0) ? mh : 0;
-                const int ry = lane >> 2, cx = lane & 3;
-                const int r0 = ti * 32 + ry, c0 = tj * 32 + cx;
-                double acc[4][8];
-    #pragma unroll
-                for (int i = 0; i < 4; ++i)
-    #pragma unroll
-                    for (int j = 0; j < 8; ++j) acc[i][j] = 0.0;
-                // rows / columns beyond the panel read row 0 (valid memory) and are masked at the store
-                const double2* rp[4]; const double2* cp[8];
-    #pragma unroll
-                for (int i = 0; i < 4; ++i) { const int ri = min(r0 + 8 * i, m - 1); rp[i] = reinterpret_cast<const double2*>(ri == m - 1 ? Prhs : P + (size_t)ri * 34); }
-    #pragma unroll
-                for (int j = 0; j < 8; ++j) { const int ci = min(c0 + 4 * j, m - 1); cp[j] = reinterpret_cast<const double2*>(ci == m - 1 ? Prhs : P + (size_t)ci * 34); }
-    #pragma unroll 2
-                for (int k = 0; k < 16; ++k) {
-                    double2 rv[4], cv[8];
-    #pragma unroll
-                    for (int i = 0; i < 4; ++i) rv[i] = rp[i][k];
-    #pragma unroll
-                    for (int j = 0; j < 8; ++j) cv[j] = cp[j][k];
-    #pragma unroll
-                    for (int i = 0; i < 4; ++i)
-    #pragma unroll
-                        for (int j = 0; j < 8; ++j) { acc[i][j] += rv[i].x * cv[j].x; acc[i][j] += rv[i].y * cv[j].y; }
-                }
-                // read-modify-write of the tile: all loads first (one round trip), then the stores.  src / dst point at the tile's
-                // first column (tj * 32 past the panel): the tile lies in one block column of the resident storage.
-                double cur[4][8];
-                const int tc = kb + bs + tj * 32;
-    #pragma unroll
-                for (int i = 0; i < 4; ++i) {
-                    const int ip = min(r0 + 8 * i, m - 1);
-                    const double* src = (ip == m - 1) ? (R + tc) : W.at(kb + bs + ip, tc);
-    #pragma unroll
-                    for (int j = 0; j < 8; ++j) { const int jp = c0 + 4 * j; cur[i][j] = (r0 + 8 * i < m && r0 + 8 * i >= row_lo && jp < m - 1 && jp <= ip) ? src[cx + 4 * j] : 0.0; }
-                }
-    #pragma unroll
-                for (int i = 0; i < 4; ++i) {
-                    const int ip = r0 + 8 * i;
-                    if (ip >= m || ip < row_lo) continue;
-                    double* dst = (ip == m - 1) ? (R + tc) : W.at(kb + bs + ip, tc);
-    #pragma unroll
-                    for (int j = 0; j < 8; ++j) { const int jp = c0 + 4 * j; if (jp < m - 1 && jp <= ip) dst[cx + 4 * j] = cur[i][j] - acc[i][j]; }
-                }
-            }
-        }
-        __syncthreads();
-        tA = clock64(); t_trail += tA - t0; t0 = tA;
-    }
-    // ---- backward substitution  L^T x = y  (y is in rhs), left-looking per 32-column block:
-    //   x_k = D_k^-T (y_k - sum_{r below} L[r][k-block]^T x_r),  D_k^-1 stored in place of D_k by the factorisation
-    // the sum is a GEMV over the envelope rows spread over all warps (independent coalesced loads, one L2 round trip per
-    // batch), then warp 0 applies the inverse diagonal block: 32 independent FMAs per lane, no substitution chain.  x overwrites rhs.
-    const int last = ((n - 1) / 32) * 32;
-    for (int kb = last; kb >= 0; kb -= 32) {
-        const int bs = min(32, n - kb);
-        const int rend = env_rmax[kb >> 5];
-        double col[32];                               // warp 0: column `lane` of the inverse diagonal block, col[i] = Linv[kb+i][kb+lane], i >= lane
-        double t = 0.0;
-        if (warp == 0) {
-#pragma unroll
-            for (int i = 0; i < 32; ++i) col[i] = (i < bs && lane < bs && i >= lane) ? W.at(kb + i, kb)[lane] : 0.0;
-            if (lane < bs) t = R[kb + lane];
-        }
-        double acc = 0.0;
-        if (lane < bs) {
-            for (int r0 = kb + bs + warp; r0 <= rend; r0 += 16 * nw) {
-                double lv[16], xv[16];
-#pragma unroll
-                for (int u = 0; u < 16; ++u) { const int r = r0 + u * nw; const bool ok = r <= rend; lv[u] = ok ? W.at(r, kb)[lane] : 0.0; xv[u] = ok ? R[r] : 0.0; }
-#pragma unroll
-                for (int u = 0; u < 16; ++u) acc += lv[u] * xv[u];
-            }
-        }
-        part[warp * 32 + lane] = acc;
-        __syncthreads();
-        if (warp == 0) {
-            for (int w = 0; w < nw; ++w) t -= part[w * 32 + lane];
-            // x = D^-T t with the stored inverse: x_lane = sum_{j >= lane} Linv[j][lane] t_j
-            double y0 = 0.0, y1 = 0.0, y2 = 0.0, y3 = 0.0;
-#pragma unroll
-            for (int j = 0; j < 32; j += 4) {
-                y0 = fma(col[j], __shfl_sync(0xffffffffu, t, j), y0);
-                y1 = fma(col[j + 1], __shfl_sync(0xffffffffu, t, j + 1), y1);
-                y2 = fma(col[j + 2], __shfl_sync(0xffffffffu, t, j + 2), y2);
-                y3 = fma(col[j + 3], __shfl_sync(0xffffffffu, t, j + 3), y3);
-            }
-            t = (y0 + y1) + (y2 + y3);
-            if (lane < bs) R[kb + lane] = t;
-        }
-        __syncthreads();
-    }
-    if (kResident) for (int i = tid; i < n; i += nt) rhs[i] = R[i];
-    if (tid == 0 && fail) st->solve_fail = 1;
-    if (tid == 0) {
-        tA = clock64(); g_chol_dbg[0] += t_diag; g_chol_dbg[1] += t_panel; g_chol_dbg[2] += t_trail; g_chol_dbg[3] += tA - t0; g_chol_dbg[4] += tA - t_begin; g_chol_dbg[5] += 1;
-        if (kResident) { g_chol_dbg[6] += t_load; g_chol_dbg[7] += 1; }
-    }
-}
-
-#include "ba_tree.cuh"
-#include "ba_wide.cuh"
-
 // ------------------------------------------------------------------ back-substitution + candidate point
 __global__ void __launch_bounds__(TPB) ba_update_kernel(BaDev d) {
     __shared__ double s_red[TPB / 32];
@@ -1421,7 +1129,6 @@ __global__ void ba_reproj_error_kernel(BaDev d, int n, const double* __restrict_
 struct lvb_ba {
     lvb_ctx* ctx = nullptr;
     bool finalized = false;
-    DevBuf<double> chol_invd;
     double cam[22];
     bool have_cam = false;
     std::vector<double> h_poses, h_vec3, h_rho;
@@ -1432,8 +1139,7 @@ struct lvb_ba {
     int n[6] = {0, 0, 0, 0, 0, 0};      // blocks as added by the caller
     double huber[6] = {0, 0, 0, 0, 0, 0};
     BaPlan plan;                        // structure, device order, storage and solver of the last finalize (ba_plan.h)
-    DevBuf<int> chol_rmax, chol_cmin;   // envelope of S per 32-column block step
-    DevBuf<Front> fronts; DevBuf<double> front_pool;      // multifrontal tree over the banded system (ba_tree.cuh)
+    ReducedSolver solver;               // the reduced camera system's solver for plan.solver (ba_solve.h)
     // device
     DevBuf<unsigned char> upload_arena;      // one allocation for everything finalize uploads (the buffers below are views into it)
     DevBuf<double> poses, vec3, rho, c_poses, c_vec3, c_rho;
@@ -1479,10 +1185,6 @@ static int init_tables() {
     for (int i = 0; i < 30; ++i) for (int j = 0; j <= i; ++j) { a[e] = (unsigned char)i; b[e] = (unsigned char)j; ++e; }
     LVB_CUDA(cudaMemcpyToSymbol(c_tri_a, a, sizeof(a)));
     LVB_CUDA(cudaMemcpyToSymbol(c_tri_b, b, sizeof(b)));
-    LVB_CUDA(cudaFuncSetAttribute(ba_cholesky_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, MAX_CTA_SMEM));
-    LVB_CUDA(cudaFuncSetAttribute(ba_cholesky_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, MAX_CTA_SMEM));
-    LVB_CUDA(cudaFuncSetAttribute(ba_front_factor_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, MAX_CTA_SMEM));
-    LVB_CUDA(cudaFuncSetAttribute(ba_front_backward_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 64 * 1024));
     LVB_CUDA(cudaFuncSetAttribute(ba_eval_two_frame_kernel<1, 5>, cudaFuncAttributeMaxDynamicSharedMemorySize, (TPB * 31 + MAX_STAGE_POSES * 7 + 2) * 8));
     LVB_CUDA(cudaFuncSetAttribute(ba_eval_two_frame_kernel<1, 6>, cudaFuncAttributeMaxDynamicSharedMemorySize, (TPB * 31 + MAX_STAGE_POSES * 7 + 2) * 8));
     LVB_CUDA(cudaFuncSetAttribute(ba_eval_two_frame_kernel<0, 5>, cudaFuncAttributeMaxDynamicSharedMemorySize, (MAX_STAGE_POSES * 7 + 2) * 8));
@@ -1498,21 +1200,7 @@ static int init_tables() {
 }
 
 static inline int nblk(size_t n, int per) { return (int)((n + per - 1) / per); }
-static void mark(struct lvb_ba* ba, const char* name);
-#define LAUNCH_ON(ba, stream_, kernel, grid, block, smem, ...)                             \
-    do { if ((grid) > 0) { kernel<<<(grid), (block), (smem), (stream_)>>>(__VA_ARGS__); (ba)->ctx->launches++; } } while (0)
-#define LAUNCH_AS(ba, name, kernel, grid, block, smem, ...)                               \
-    do { if ((grid) > 0) { kernel<<<(grid), (block), (smem), (ba)->ctx->stream>>>(__VA_ARGS__); (ba)->ctx->launches++; mark(ba, name); } } while (0)
-#define LAUNCH(ba, kernel, grid, block, smem, ...) LAUNCH_AS(ba, #kernel, kernel, grid, block, smem, __VA_ARGS__)
-
-static void mark(lvb_ba* ba, const char* name) { lvb::timing_mark(ba->ctx->stream, name); }
 #define g_timing lvb::g_timing
-
-static int check_launch(const char* what) {
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) { set_error("kernel launch failed in %s: %s", what, cudaGetErrorString(e)); return LVB_ERR_CUDA; }
-    return LVB_OK;
-}
 
 // AoS -> SoA of one factor kind in device order: record i of the output is caller record ord[i] (or a padding copy of record
 // -1 - ord[i] with its weight column zeroed).  Compile-time strides for the visual kinds: the generic loop spends its time on the
@@ -1654,10 +1342,6 @@ int lvb_ba_set_loss(lvb_ba* ba, int kind, double a) {
     return LVB_OK;
 }
 
-// the plan-shaping A/B switches, read once per process
-static bool no_tree_switch() { static const bool on = getenv("LVB_NO_TREE") && getenv("LVB_NO_TREE")[0] == '1'; return on; }
-static bool tree_sep_band_switch() { static const bool on = getenv("LVB_TREE_SEP_BAND") && getenv("LVB_TREE_SEP_BAND")[0] == '1'; return on; }
-
 // element-wise collective over a host array of a sharded problem: through the device, like every all-reduce
 static int allreduce_host_i32(lvb_ctx* ctx, std::vector<int>& v, int (*op)(lvb_ctx*, int*, size_t)) {
     cudaStream_t s = ctx->stream;
@@ -1717,9 +1401,6 @@ int lvb_ba_finalize(lvb_ba* ba) {
     LVB_TRY(stg.put(ba->sw_lm, P.sw_lm.data(), P.sw_lm.size()));
     LVB_TRY(stg.put(ba->grp_ns, P.grp_ns.data(), P.grp_ns.size()));
     LVB_TRY(stg.put(ba->grp_off, P.grp_off.data(), P.grp_off.size()));
-    LVB_TRY(stg.put(ba->chol_rmax, P.chol_rmax.data(), P.chol_rmax.size()));
-    LVB_TRY(stg.put(ba->chol_cmin, P.chol_cmin.data(), P.chol_cmin.size()));
-    if (P.solver.tree_levels > 0) { LVB_TRY(stg.put(ba->fronts, P.solver.fronts.data(), P.solver.fronts.size())); LVB_TRY(ba->front_pool.ensure(P.solver.pool_doubles)); }
     // tensor-core Schur operands: the compaction maps and the zero-initialised split-bf16 U^T tiles
     LVB_TRY(stg.put(ba->tc_cdim, P.tc_cdim.data(), P.tc_cdim.size()));
     LVB_TRY(stg.put(ba->tc_off, P.tc_off.data(), P.tc_off.size()));
@@ -1776,7 +1457,7 @@ int lvb_ba_finalize(lvb_ba* ba) {
     PROF("planes + uploads");
 
     const size_t nH = P.nS;
-    LVB_TRY(ba->chol_invd.ensure(P.dimc + 32));
+    LVB_TRY(ba->solver.upload(ctx, P.solver, P.chol_rmax, P.dimc));
     LVB_TRY(ba->Hpp.ensure(nH)); LVB_TRY(ba->gc.ensure(P.dimc));
     LVB_TRY(ba->Hll.ensure(std::max(1, nr))); LVB_TRY(ba->gl.ensure(std::max(1, nr)));
     LVB_TRY(ba->tf_w.ensure((size_t)std::max(1, P.nd[0]) * 12));
@@ -1863,15 +1544,15 @@ static int launch_eval(lvb_ba* ba, int kind, double* r_dev, double* J_dev) {
     case 0: {
         const size_t pose_b = d.stage_poses ? (size_t)d.n_poses * 56 + 16 : 0;
         const int v = ba->ctx->eval_variant;       // LVB_EVAL_VARIANT: 0 staged/5 CTAs, 1 staged/6, 2 direct/5, 3 direct/6
-        if (v == 1) LAUNCH(ba, (ba_eval_two_frame_kernel<1, 6>), nblk(n, TPB), TPB, (size_t)(TPB * 31) * 8 + pose_b, d, r_dev, J_dev);
-        else if (v == 2) LAUNCH(ba, (ba_eval_two_frame_kernel<0, 5>), nblk(n, TPB), TPB, pose_b, d, r_dev, J_dev);
-        else if (v == 3) LAUNCH(ba, (ba_eval_two_frame_kernel<0, 6>), nblk(n, TPB), TPB, pose_b, d, r_dev, J_dev);
-        else LAUNCH(ba, (ba_eval_two_frame_kernel<1, 5>), nblk(n, TPB), TPB, (size_t)(TPB * 31) * 8 + pose_b, d, r_dev, J_dev);
+        if (v == 1) LAUNCH(ba->ctx, (ba_eval_two_frame_kernel<1, 6>), nblk(n, TPB), TPB, (size_t)(TPB * 31) * 8 + pose_b, d, r_dev, J_dev);
+        else if (v == 2) LAUNCH(ba->ctx, (ba_eval_two_frame_kernel<0, 5>), nblk(n, TPB), TPB, pose_b, d, r_dev, J_dev);
+        else if (v == 3) LAUNCH(ba->ctx, (ba_eval_two_frame_kernel<0, 6>), nblk(n, TPB), TPB, pose_b, d, r_dev, J_dev);
+        else LAUNCH(ba->ctx, (ba_eval_two_frame_kernel<1, 5>), nblk(n, TPB), TPB, (size_t)(TPB * 31) * 8 + pose_b, d, r_dev, J_dev);
         break; }
-    case 1: LAUNCH(ba, ba_eval_pose_only_kernel, nblk(n, TPB), TPB, 0, d, r_dev, J_dev); break;
-    case 2: LAUNCH(ba, ba_eval_two_camera_kernel, nblk(n, TPB), TPB, 0, d, r_dev, J_dev); break;
-    case 3: LAUNCH(ba, ba_eval_imu_kernel, nblk(n, 4), TPB, 0, d, r_dev, J_dev); break;
-    default: LAUNCH(ba, ba_eval_prior_kernel, nblk(n, 64), 64, 0, d, kind, r_dev, J_dev); break;
+    case 1: LAUNCH(ba->ctx, ba_eval_pose_only_kernel, nblk(n, TPB), TPB, 0, d, r_dev, J_dev); break;
+    case 2: LAUNCH(ba->ctx, ba_eval_two_camera_kernel, nblk(n, TPB), TPB, 0, d, r_dev, J_dev); break;
+    case 3: LAUNCH(ba->ctx, ba_eval_imu_kernel, nblk(n, 4), TPB, 0, d, r_dev, J_dev); break;
+    default: LAUNCH(ba->ctx, ba_eval_prior_kernel, nblk(n, 64), 64, 0, d, kind, r_dev, J_dev); break;
     }
     return check_launch("ba_eval");
 }
@@ -1944,14 +1625,14 @@ template <int MODE> static int launch_linearize(lvb_ba* ba) {
     lvb_ctx* ctx = ba->ctx;
     const bool one_grid = merged_linearize(ba);
     const bool fork = !one_grid && use_side_branch(ba);
-    if (one_grid) LAUNCH_AS(ba, kName[MODE][0], ba_linearize_all_kernel<MODE>, ba->ranges.b[6], TPB, std::max(ba->lin_smem, ba->imu_smem), d, ba->ranges);
+    if (one_grid) LAUNCH_AS(ba->ctx, kName[MODE][0], ba_linearize_all_kernel<MODE>, ba->ranges.b[6], TPB, std::max(ba->lin_smem, ba->imu_smem), d, ba->ranges);
     else {
     if (fork) { LVB_CUDA(cudaEventRecord(ctx->ev_fork, ctx->stream)); LVB_CUDA(cudaStreamWaitEvent(ctx->side, ctx->ev_fork, 0)); }
-    LAUNCH_AS(ba, kName[MODE][1], ba_linearize_kernel<MODE>, ba->ranges.b[3], TPB, ba->lin_smem, d, ba->ranges);
+    LAUNCH_AS(ba->ctx, kName[MODE][1], ba_linearize_kernel<MODE>, ba->ranges.b[3], TPB, ba->lin_smem, d, ba->ranges);
     if (fork) {
-        LAUNCH_ON(ba, ctx->side, ba_linearize_other_kernel<MODE>, ba->ranges.b[6] - ba->ranges.b[3], TPB, ba->imu_smem, d, ba->ranges);
+        LAUNCH_ON(ba->ctx, ctx->side, ba_linearize_other_kernel<MODE>, ba->ranges.b[6] - ba->ranges.b[3], TPB, ba->imu_smem, d, ba->ranges);
         LVB_CUDA(cudaEventRecord(ctx->ev_join, ctx->side)); LVB_CUDA(cudaStreamWaitEvent(ctx->stream, ctx->ev_join, 0));
-    } else LAUNCH_AS(ba, kName[MODE][2], ba_linearize_other_kernel<MODE>, ba->ranges.b[6] - ba->ranges.b[3], TPB, ba->imu_smem, d, ba->ranges);
+    } else LAUNCH_AS(ba->ctx, kName[MODE][2], ba_linearize_other_kernel<MODE>, ba->ranges.b[6] - ba->ranges.b[3], TPB, ba->imu_smem, d, ba->ranges);
     }
     return LVB_OK;
 }
@@ -1967,87 +1648,43 @@ static int launch_linearize_and_reduce(lvb_ba* ba, bool standalone) {
     const size_t nH = d.nS;
     LVB_TRY(launch_linearize<0>(ba));
     const bool fuse_damp = ctx->world == 1;
-    if (fuse_damp) LAUNCH(ba, ba_build_S_kernel<1>, std::min(1024, nblk(nH, 256)), 256, 0, d);
-    else LAUNCH(ba, ba_build_S_kernel<0>, std::min(1024, nblk(nH, 256)), 256, 0, d);
-    LAUNCH(ba, ba_schur_kernel, nblk(d.n_schur_warps, TPB / 32), TPB, ba->schur_smem, d, std::max(1, ba->plan.schur_cols_max));
-    if (d.tc_mode) LAUNCH(ba, ba_schur_tc_kernel, ba->n_tc_chunks / TC_CHUNKS, 128, (size_t)TC_CHUNKS * TC_CHUNK_BYTES, d, ba->n_tc_chunks);
+    if (fuse_damp) LAUNCH(ba->ctx, ba_build_S_kernel<1>, std::min(1024, nblk(nH, 256)), 256, 0, d);
+    else LAUNCH(ba->ctx, ba_build_S_kernel<0>, std::min(1024, nblk(nH, 256)), 256, 0, d);
+    LAUNCH(ba->ctx, ba_schur_kernel, nblk(d.n_schur_warps, TPB / 32), TPB, ba->schur_smem, d, std::max(1, ba->plan.schur_cols_max));
+    if (d.tc_mode) LAUNCH(ba->ctx, ba_schur_tc_kernel, ba->n_tc_chunks / TC_CHUNKS, 128, (size_t)TC_CHUNKS * TC_CHUNK_BYTES, d, ba->n_tc_chunks);
     const size_t n_arena = nH + 3 * (size_t)d.dimc + 16;
     P2PArgs pa;
     const bool fused_comm = ctx->world > 1 && comm_p2p_args(ctx, n_arena, &pa) && (size_t)(d.n_poses + d.n_vec3) <= 4096;
     if (fused_comm) {
-        LAUNCH(ba, ba_allreduce_fused_kernel, (int)std::max<size_t>(1, std::min<size_t>(XB_BLOCKS, (n_arena + 255) / 256)), 256, 0, pa, d, (int)n_arena);
+        LAUNCH(ba->ctx, ba_allreduce_fused_kernel, (int)std::max<size_t>(1, std::min<size_t>(XB_BLOCKS, (n_arena + 255) / 256)), 256, 0, pa, d, (int)n_arena);
     } else if (ctx->world > 1) {
-        LAUNCH(ba, ba_pack_scalars_kernel, 1, 1, 0, d);
+        LAUNCH(ba->ctx, ba_pack_scalars_kernel, 1, 1, 0, d);
         LVB_TRY(comm_allreduce_sum_f64(ctx, d.S, n_arena));
-        LAUNCH(ba, ba_unpack_scalars_kernel, 1, 1, 0, d);
+        LAUNCH(ba->ctx, ba_unpack_scalars_kernel, 1, 1, 0, d);
     }
     // (fusing this into the Cholesky prologue was measured: it perturbs that kernel's register allocation and is slower)
-    if (!fuse_damp && !fused_comm) LAUNCH(ba, ba_prepare_camera_kernel, nblk(d.n_poses + d.n_vec3, 128), 128, 0, d);
-    if (standalone) LAUNCH(ba, lm_control_pre_kernel, 1, 1, 0, d.st);
+    if (!fuse_damp && !fused_comm) LAUNCH(ba->ctx, ba_prepare_camera_kernel, nblk(d.n_poses + d.n_vec3, 128), 128, 0, d);
+    if (standalone) LAUNCH(ba->ctx, lm_control_pre_kernel, 1, 1, 0, d.st);
     return check_launch("linearize");
-}
-
-// rhs <- S^-1 rhs (+ the LM pre-check): multifrontal tree over the banded system, or the single-CTA envelope Cholesky
-static int launch_wide_solve(lvb_ba* ba) {
-    BaDev& d = ba->dev;
-    const int n = d.dimc;
-    static bool attr_set = false;
-    if (!attr_set) { LVB_CUDA(cudaFuncSetAttribute(ba_wide_update_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, WIDE_WARPS * 2 * 32 * 34 * 8)); attr_set = true; }
-    for (int kb = 0; kb < n; kb += 32) {
-        const int bs = std::min(32, n - kb);
-        const int m = ba->plan.chol_rmax[kb >> 5] - (kb + bs) + 2;
-        const int ntile = (m + 31) / 32, total = m > 1 ? ntile * (ntile + 1) / 2 : 0;
-        LAUNCH(ba, ba_wide_diag_kernel, 1, 32, 0, d.S, n, d.srow, d.soff, kb, ba->chol_invd.p, d.st, kb == 0 ? 1 : 0);
-        LAUNCH(ba, ba_wide_panel_kernel, nblk(m, 128), 128, 0, d.S, d.rhs, n, d.srow, d.soff, kb, ba->chol_invd.p, d.st, ba->chol_rmax.p);
-        LAUNCH(ba, ba_wide_update_kernel, nblk(total, WIDE_WARPS), WIDE_WARPS * 32, (size_t)WIDE_WARPS * 2 * 32 * 34 * 8, d.S, d.rhs, n, d.srow, d.soff, kb, d.st, ba->chol_rmax.p);
-    }
-    for (int kb = ((n - 1) / 32) * 32; kb >= 0; kb -= 32)
-        LAUNCH(ba, ba_wide_backward_kernel, 1, 256, 0, d.S, d.rhs, n, d.srow, d.soff, kb, ba->chol_invd.p, d.st, ba->chol_rmax.p);
-    return LVB_OK;
-}
-
-static int launch_reduced_solve(lvb_ba* ba) {
-    BaDev& d = ba->dev;
-    lvb_ctx* ctx = ba->ctx;
-    const SolverPlan& sp = ba->plan.solver;
-    const int band = ba->plan.band;
-    if (sp.tree_levels > 0) {
-        // multifrontal tree: leaves (all SMs) -> ... -> root, then the back-substitution root -> leaves; 2 (levels + 1) launches
-        const Front* fr = ba->fronts.p;
-        LAUNCH(ba, lm_control_pre_kernel, 1, 1, 0, d.st);
-        const int n_fronts = sp.level_first[sp.tree_levels - 1] + sp.level_count[sp.tree_levels - 1];
-        ba_front_init_kernel<<<dim3(16, n_fronts), 256, 0, ctx->stream>>>(fr, n_fronts, d.S, d.rhs, ba->front_pool.p, d.srow, d.soff, band, d.st);
-        ctx->launches++; mark(ba, "ba_front_init_kernel");
-        for (int l = 0; l < sp.tree_levels; ++l)
-            LAUNCH(ba, ba_front_factor_kernel, sp.level_count[l], CHOL_T, sp.tree_factor_smem, fr, sp.level_first[l], d.S, d.rhs, ba->front_pool.p, d.srow, d.soff, band, ba->chol_invd.p, d.st);
-        for (int l = sp.tree_levels - 1; l >= 0; --l)
-            LAUNCH(ba, ba_front_backward_kernel, sp.level_count[l], CHOL_T, sp.tree_back_smem, fr, sp.level_first[l], d.S, d.rhs, ba->front_pool.p, d.srow, d.soff, band, ba->chol_invd.p, d.st);
-    } else if (sp.wide) {
-        LVB_TRY(launch_wide_solve(ba));
-    } else if (sp.resident) {
-        LAUNCH_AS(ba, "ba_cholesky_kernel", ba_cholesky_kernel<true>, 1, CHOL_T, sp.resident_smem, d.S, d.rhs, d.dimc, d.srow, d.soff, ba->chol_invd.p, d.st, 1, ba->chol_rmax.p, ba->chol_cmin.p);
-    } else
-    LAUNCH_AS(ba, "ba_cholesky_kernel", ba_cholesky_kernel<false>, 1, CHOL_T, sp.chol_smem, d.S, d.rhs, d.dimc, d.srow, d.soff, ba->chol_invd.p, d.st, 1, ba->chol_rmax.p, ba->chol_cmin.p);
-    return LVB_OK;
 }
 
 static int launch_step(lvb_ba* ba) {
     BaDev& d = ba->dev;
     lvb_ctx* ctx = ba->ctx;
-    LVB_TRY(launch_reduced_solve(ba));
-    LAUNCH(ba, ba_update_kernel, nblk((size_t)d.n_poses + d.n_vec3 + d.n_rho, TPB), TPB, 0, d);
+    LVB_TRY(ba->solver.launch(ctx, d.S, d.rhs, d.dimc, d.srow, d.soff, ba->plan.band, d.st));
+    LAUNCH(ba->ctx, ba_update_kernel, nblk((size_t)d.n_poses + d.n_vec3 + d.n_rho, TPB), TPB, 0, d);
     LVB_TRY(launch_linearize<1>(ba));
     if (ctx->world > 1) LVB_TRY(comm_allreduce_sum_f64(ctx, &d.st->cand_cost_acc, 5));
     const bool wide = d.nS > ((size_t)1 << 20) || (size_t)d.n_poses * 7 + (size_t)d.n_vec3 * 3 + d.n_rho > ((size_t)1 << 17);
-    LAUNCH(ba, ba_post_kernel, 1, wide ? 32 : 1024, 0, d, wide ? 1 : 0);
-    if (wide) LAUNCH(ba, ba_post_wide_kernel, 4 * ba->ctx->sm_count, 256, 0, d);
+    LAUNCH(ba->ctx, ba_post_kernel, 1, wide ? 32 : 1024, 0, d, wide ? 1 : 0);
+    if (wide) LAUNCH(ba->ctx, ba_post_wide_kernel, 4 * ba->ctx->sm_count, 256, 0, d);
     return check_launch("step");
 }
 
 static int launch_clear(lvb_ba* ba) {
     BaDev& d = ba->dev;
     const size_t nH = d.nS;
-    LAUNCH(ba, ba_zero_kernel, std::min(1024, nblk(nH + d.dimc + 2 * (size_t)d.n_rho, 256)), 256, 0, d);
+    LAUNCH(ba->ctx, ba_zero_kernel, std::min(1024, nblk(nH + d.dimc + 2 * (size_t)d.n_rho, 256)), 256, 0, d);
     return check_launch("clear");
 }
 
@@ -2117,7 +1754,7 @@ int lvb_ba_solve(lvb_ba* ba, const lvb_solve_options* options, lvb_solve_summary
     cudaStream_t s = ba->ctx->stream;
     LmState h;
     memset(&h, 0, sizeof(h));
-    mark(ba, "begin");
+    lvb::timing_mark(s, "begin");
     LVB_TRY(launch_clear(ba));
     // The pass is a fixed sequence of launches whose kernels all read their control flags from the device state,
     // so it is captured once into a CUDA graph and replayed; the host looks at the state only every
@@ -2207,50 +1844,6 @@ int lvb_ba_set_schur_mode(lvb_ba* ba, int mode) {
     return LVB_OK;
 }
 
-LVB_API int lvb_debug_cholesky_clocks(long long out[8], int reset) {
-    LVB_CUDA(cudaMemcpyFromSymbol(out, g_chol_dbg, 8 * sizeof(long long)));
-    if (reset) { long long z[8] = {0}; LVB_CUDA(cudaMemcpyToSymbol(g_chol_dbg, z, sizeof(z))); }
-    return LVB_OK;
-}
-
-// Direct access to the reduced-system solver for its own parity test (tests/test_gpu_band_solver.py): solves S x = b for a
-// symmetric positive definite band matrix given as n rows of (band + 1) entries (row i: columns i - band .. i; the true half
-// bandwidth must be <= band - 31, the block-granular slack the envelope kernel needs).  use_tree = 0 forces the single-CTA kernel.
-LVB_API int lvb_debug_band_solve(lvb_ctx* ctx, int n, int band, const double* S_band, const double* b, double* x, int use_tree, int* levels_out) {
-    if (!ctx || n <= 0 || band < 31 || !S_band || !b || !x) { set_error("bad arguments"); return LVB_ERR_INVALID; }
-    LVB_CUDA(cudaSetDevice(ctx->device)); lvb::g_alloc_stream = ctx->stream;
-    LVB_TRY(init_tables());
-    lvb_ba ba;
-    ba.ctx = ctx;
-    cudaStream_t s = ctx->stream;
-    BaPlan& P = ba.plan;
-    P.dimc = n; P.band = band; P.srow = band; P.soff = band; P.nS = (size_t)n * (band + 1);
-    LVB_TRY(ba.arena.ensure(P.nS + n));
-    LVB_CUDA(cudaMemcpyAsync(ba.arena.p, S_band, P.nS * sizeof(double), cudaMemcpyHostToDevice, s));
-    LVB_CUDA(cudaMemcpyAsync(ba.arena.p + P.nS, b, (size_t)n * sizeof(double), cudaMemcpyHostToDevice, s));
-    LVB_TRY(ba.chol_invd.ensure(n + 32));
-    LVB_TRY(ba.st.ensure(1));
-    lvb_solve_options opt; lvb_default_options(&opt);
-    LmState h; lm_init(h, opt);
-    const double one = 1.0; memcpy(&h.grad_max_bits, &one, sizeof(double));        // not converged: the pre-check lets the solve run
-    LVB_CUDA(cudaMemcpyAsync(ba.st.p, &h, sizeof(h), cudaMemcpyHostToDevice, s));
-    uniform_band_envelope(n, band, P.chol_rmax, P.chol_cmin);
-    LVB_TRY(ba.chol_rmax.upload(P.chol_rmax.data(), P.chol_rmax.size(), s)); LVB_TRY(ba.chol_cmin.upload(P.chol_cmin.data(), P.chol_cmin.size(), s));
-    P.solver = plan_reduced_solver(n, band, tree_sep_band_switch() ? band : band - 31, P.chol_rmax, ctx->sm_count, !use_tree);
-    if (P.solver.tree_levels > 0) { LVB_TRY(ba.fronts.upload(P.solver.fronts.data(), P.solver.fronts.size(), s)); LVB_TRY(ba.front_pool.ensure(P.solver.pool_doubles)); }
-    if (levels_out) *levels_out = P.solver.tree_levels;
-    BaDev& d = ba.dev;
-    memset(&d, 0, sizeof(d));
-    d.dimc = n; d.srow = P.srow; d.soff = P.soff; d.nS = P.nS; d.S = ba.arena.p; d.rhs = ba.arena.p + P.nS; d.st = ba.st.p;
-    LVB_TRY(launch_reduced_solve(&ba));
-    LVB_TRY(check_launch("band solve"));
-    LVB_CUDA(cudaMemcpyAsync(x, d.rhs, (size_t)n * sizeof(double), cudaMemcpyDeviceToHost, s));
-    LVB_CUDA(cudaMemcpyAsync(&h, ba.st.p, sizeof(h), cudaMemcpyDeviceToHost, s));
-    LVB_CUDA(cudaStreamSynchronize(s));
-    if (h.solve_fail) { set_error("band solve: non-positive pivot"); return LVB_ERR_NUMERIC; }
-    return LVB_OK;
-}
-
 // The three getters share one device round trip: the first call after a solve / parameter update brings all parameter blocks back
 // (through the context's pinned staging area when it is free), the others copy from that snapshot.
 static int fetch_params(lvb_ba* ba) {
@@ -2288,7 +1881,7 @@ int lvb_ba_reprojection_errors(lvb_ba* ba, int n, const double* ob_pw, const int
     DevBuf<double> d_in, d_err; DevBuf<int> d_idx;
     cudaStream_t s = ba->ctx->stream;
     LVB_TRY(d_in.upload(ob_pw, (size_t)5 * n, s)); LVB_TRY(d_idx.upload(pose_idx, n, s)); LVB_TRY(d_err.ensure(n));
-    LAUNCH(ba, ba_reproj_error_kernel, nblk(n, 128), 128, 0, ba->dev, n, d_in.p, d_idx.p, d_err.p);
+    LAUNCH(ba->ctx, ba_reproj_error_kernel, nblk(n, 128), 128, 0, ba->dev, n, d_in.p, d_idx.p, d_err.p);
     LVB_TRY(check_launch("reproj"));
     LVB_TRY(d_err.download(err, n, s));
     LVB_CUDA(cudaStreamSynchronize(s));

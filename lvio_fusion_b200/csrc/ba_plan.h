@@ -49,6 +49,12 @@ struct Front {
     long long bd;           // offset of the border array in the pool (doubles)
 };
 
+// Shared memory of a front's partial factorisation (ba_front_factor_kernel) for panels of up to `rows` rows, in bytes: the diagonal
+// block Dt (32 x 34) and its invd (32), then the panel from FRONT_PANEL on at a row stride of 34, reserved for rows + 2 rows, then
+// 96 doubles of slack.  The slack counts in the size that decides whether a tree's fronts fit (MAX_CTA_SMEM).
+enum { FRONT_PANEL = 32 * 34 + 32 };
+inline size_t front_factor_smem(int rows) { return (size_t)(FRONT_PANEL + (rows + 2) * 34 + 96) * 8; }
+
 // How the reduced camera system is factored: the separator tree when it has levels (ba_tree.cuh), else the single-CTA kernel with
 // the whole envelope resident in shared memory when it fits, else the single-CTA kernel on S in global memory when its panel fits,
 // else the per-phase grids of ba_wide.cuh.
@@ -468,7 +474,7 @@ inline SolverPlan plan_reduced_solver(int n, int band, int sep, const std::vecto
         int rows = 0, mnb = 0, max_leaves = 1;
         while (max_leaves * 2 <= std::max(2, sm_count)) max_leaves *= 2;
         const int lv = build_front_tree(n, band, sep, max_leaves, s.fronts, s.level_first, s.level_count, s.pool_doubles, rows, mnb);
-        const size_t fs = (size_t)(32 * 33 + 32 + 128 + (rows + 2) * 34) * 8, bs = (size_t)(((mnb + 1) & ~1) + (CHOL_T / 32) * 32) * 8;
+        const size_t fs = front_factor_smem(rows), bs = (size_t)(((mnb + 1) & ~1) + (CHOL_T / 32) * 32) * 8;
         if (lv > 0 && fs <= MAX_CTA_SMEM && s.pool_doubles < ((size_t)1 << 31)) { s.tree_levels = lv; s.tree_factor_smem = fs; s.tree_back_smem = bs; }
     }
     s.resident = s.tree_levels == 0 && nstep <= CHOL_RES_STEPS && s.resident_smem <= MAX_CTA_SMEM;

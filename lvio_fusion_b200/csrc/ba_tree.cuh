@@ -18,7 +18,14 @@
 #pragma once
 #include "ba_plan.h"        // struct Front, CHOL_T; the tree itself is built there (build_front_tree)
 
-#define SG(i_, j_) S[(size_t)(i_) * (size_t)srow + (size_t)(j_) + (size_t)soff]
+// Panel row p of a front's 32-column step: the own rows r1 + p inside the band (p < nr1), then the active border rows, then the rhs
+// row.  base(p)[c] is the row's entry in own column c (c >= n: border column c - n); col(p) is the own column of its diagonal entry.
+struct FrontRows {
+    CholGlobal<double> G; double* Bd; int o0, r1, nr1, nbp, nb, n, ld;
+    __device__ __forceinline__ int border(int p) const { return (p - nr1 < nbp) ? p - nr1 : nb; }
+    __device__ __forceinline__ double* base(int p) const { return (p < nr1) ? G.at(o0 + r1 + p, o0) : Bd + (size_t)border(p) * ld; }
+    __device__ __forceinline__ int col(int p) const { return (p < nr1) ? r1 + p : n + border(p); }
+};
 
 // Every front's border array before the factorisation starts.  Leaves: zeros, the couplings with the bounding separators
 // gathered out of the band (the left one transposed: in the front the separator comes after the segment) and the right-hand
@@ -27,6 +34,7 @@
 __global__ void __launch_bounds__(256) ba_front_init_kernel(const Front* __restrict__ fr, int n_fronts, const double* __restrict__ S, const double* __restrict__ rhs,
                                                              double* __restrict__ pool, long long srow, long long soff, int band, const LmState* st) {
     if (st->done) return;
+    const CholGlobal G{S, srow, soff};
     for (int f = blockIdx.y; f < n_fronts; f += gridDim.y) {
         const Front F = fr[f];
         double* Bd = pool + F.bd;
@@ -38,8 +46,8 @@ __global__ void __launch_bounds__(256) ba_front_init_kernel(const Front* __restr
             if (c < F.m) {
                 if (q == F.nb) v = rhs[F.o0 + c];
                 else if (leaf) {
-                    if (q < F.wL) { const int gi = F.o0 + c, gj = F.bL0 + q; if (gi - gj <= band) v = SG(gi, gj); }
-                    else { const int gi = F.bR0 + (q - F.wL), gj = F.o0 + c; if (gi - gj <= band) v = SG(gi, gj); }
+                    if (q < F.wL) { const int gi = F.o0 + c, gj = F.bL0 + q; if (gi - gj <= band) v = *G.at(gi, gj); }
+                    else { const int gi = F.bR0 + (q - F.wL), gj = F.o0 + c; if (gi - gj <= band) v = *G.at(gi, gj); }
                 }
             }
             Bd[e] = v;
@@ -47,7 +55,7 @@ __global__ void __launch_bounds__(256) ba_front_init_kernel(const Front* __restr
     }
 }
 
-// One CTA per front of a level.  Shared memory: D (32 x 33), invd (32), Lc (2 x 64), P (panel rows x 34).
+// One CTA per front of a level.  Shared memory (front_factor_smem, ba_plan.h): Dt (32 x 34), invd (32), P (panel rows x 34).
 __global__ void __launch_bounds__(CHOL_T) ba_front_factor_kernel(const Front* __restrict__ fr, int first, double* __restrict__ S, const double* __restrict__ rhs,
                                                                   double* __restrict__ pool, long long srow, long long soff, int band,
                                                                   double* __restrict__ invd_g, LmState* st) {
@@ -55,8 +63,9 @@ __global__ void __launch_bounds__(CHOL_T) ba_front_factor_kernel(const Front* __
     extern __shared__ __align__(16) double sm[];
     double* Dt = sm;                   // 32 x 34   diagonal block of L, column-major: Dt[j * 34 + k] = L[k][j] (lvb_chol.cuh)
     double* invd = sm + 32 * 34;       // 32        reciprocals of diag(L) of the current block
-    double* P = invd + 32;             // rows x 34 panel (16 B aligned rows for broadcast double2 loads)
+    double* P = sm + FRONT_PANEL;      // rows x 34 panel (16 B aligned rows for broadcast double2 loads)
     __shared__ int fail;
+    const CholGlobal G{S, srow, soff};
     const Front F = fr[first + blockIdx.x];
     const int n = F.m, nb = F.nb, ld = F.ld;
     double* Bd = pool + F.bd;
@@ -73,14 +82,12 @@ __global__ void __launch_bounds__(CHOL_T) ba_front_factor_kernel(const Front* __
             const int nr1 = max(0, min(n - 1, kb + band) - r1 + 1);
             const int nbp = F.wL + ((r1 > F.actR) ? F.wR : 0);
             const int m = nr1 + nbp + 1;
-            // row_base(p)[c] = entry of panel row p in own column c (c >= n: border column c - n); col_of(p) = its own column index
-#define ROW_BASE(p_) (((p_) < nr1) ? (&SG(F.o0 + r1 + (p_), F.o0)) : (Bd + (size_t)((((p_) - nr1) < nbp) ? ((p_) - nr1) : nb) * ld))
-#define COL_OF(p_) (((p_) < nr1) ? (r1 + (p_)) : (n + ((((p_) - nr1) < nbp) ? ((p_) - nr1) : nb)))
+            const FrontRows rows{G, Bd, F.o0, r1, nr1, nbp, nb, n, ld};
             // the diagonal block factored during the previous step's look-ahead goes to its place in S (all threads, row by row)
-            for (int e = tid; e < 32 * 32; e += nt) { const int k = e >> 5, j = e & 31; if (j <= k && k < bs) SG(F.o0 + kb + k, F.o0 + kb + j) = Dt[j * 34 + k]; }
+            for (int e = tid; e < 32 * 32; e += nt) { const int k = e >> 5, j = e & 31; if (j <= k && k < bs) *G.at(F.o0 + kb + k, F.o0 + kb + j) = Dt[j * 34 + k]; }
             if (tid < bs) invd_g[F.o0 + kb + tid] = invd[tid];
             for (int rr = tid; rr < m; rr += nt) {
-                double* src = ROW_BASE(rr) + kb;
+                double* src = rows.base(rr) + kb;
                 double a[32];
 #pragma unroll
                 for (int j = 0; j < 32; ++j) a[j] = (j < bs) ? src[j] : 0.0;
@@ -93,42 +100,25 @@ __global__ void __launch_bounds__(CHOL_T) ba_front_factor_kernel(const Front* __
             const int ntile = (m + 31) >> 5;
             const int total = ntile * (ntile + 1) / 2;
             for (int t = (warp == 0) ? 0 : warp; t < total; t += (warp == 0) ? total : (nw - 1)) {
-                int ti = (int)((sqrt(8.0 * t + 1.0) - 1.0) * 0.5);
-                while ((ti + 1) * (ti + 2) / 2 <= t) ++ti;
-                while (ti * (ti + 1) / 2 > t) --ti;
-                const int tj = t - ti * (ti + 1) / 2;
+                int ti, tj;
+                chol_tile_index(t, ti, tj);
                 const int ry = lane >> 2, cx = lane & 3;
                 const int r0 = ti * 32 + ry, c0 = tj * 32 + cx;
-                double acc[4][8];
-#pragma unroll
-                for (int i = 0; i < 4; ++i)
-#pragma unroll
-                    for (int j = 0; j < 8; ++j) acc[i][j] = 0.0;
+                double acc[4][8] = {};
                 const double2* rp[4]; const double2* cp[8];
 #pragma unroll
                 for (int i = 0; i < 4; ++i) rp[i] = reinterpret_cast<const double2*>(P + (size_t)min(r0 + 8 * i, m - 1) * 34);
 #pragma unroll
                 for (int j = 0; j < 8; ++j) cp[j] = reinterpret_cast<const double2*>(P + (size_t)min(c0 + 4 * j, m - 1) * 34);
-#pragma unroll 2
-                for (int k = 0; k < 16; ++k) {
-                    double2 rv[4], cv[8];
-#pragma unroll
-                    for (int i = 0; i < 4; ++i) rv[i] = rp[i][k];
-#pragma unroll
-                    for (int j = 0; j < 8; ++j) cv[j] = cp[j][k];
-#pragma unroll
-                    for (int i = 0; i < 4; ++i)
-#pragma unroll
-                        for (int j = 0; j < 8; ++j) { acc[i][j] += rv[i].x * cv[j].x; acc[i][j] += rv[i].y * cv[j].y; }
-                }
+                chol_tile_product(acc, rp, cp);
                 int colx[8];
 #pragma unroll
-                for (int j = 0; j < 8; ++j) { const int jp = min(c0 + 4 * j, m - 1); colx[j] = COL_OF(jp); }
+                for (int j = 0; j < 8; ++j) { const int jp = min(c0 + 4 * j, m - 1); colx[j] = rows.col(jp); }
                 double cur[4][8];
 #pragma unroll
                 for (int i = 0; i < 4; ++i) {
                     const int ip = min(r0 + 8 * i, m - 1);
-                    const double* src = ROW_BASE(ip);
+                    const double* src = rows.base(ip);
 #pragma unroll
                     for (int j = 0; j < 8; ++j) { const int jp = c0 + 4 * j; cur[i][j] = (r0 + 8 * i < m && jp < m - 1 && jp <= ip) ? src[colx[j]] : 0.0; }
                 }
@@ -136,13 +126,11 @@ __global__ void __launch_bounds__(CHOL_T) ba_front_factor_kernel(const Front* __
                 for (int i = 0; i < 4; ++i) {
                     const int ip = r0 + 8 * i;
                     if (ip >= m) continue;
-                    double* dst = ROW_BASE(ip);
+                    double* dst = rows.base(ip);
 #pragma unroll
                     for (int j = 0; j < 8; ++j) { const int jp = c0 + 4 * j; if (jp < m - 1 && jp <= ip) dst[colx[j]] = cur[i][j] - acc[i][j]; }
                 }
             }
-#undef ROW_BASE
-#undef COL_OF
         }
         const int kn = kb + 32, bn = min(32, n - kn);
         // ---- diagonal block kn: warp 0 holds one row per lane in registers and factors it with shuffles (4 groups of 8 columns)
@@ -151,7 +139,7 @@ __global__ void __launch_bounds__(CHOL_T) ba_front_factor_kernel(const Front* __
             if (warp == 0) {
                 double a[32];
 #pragma unroll
-                for (int j = 0; j < 32; ++j) a[j] = (lane < bn && j <= lane) ? SG(F.o0 + kn + lane, F.o0 + kn + j) : ((j == lane) ? 1.0 : 0.0);
+                for (int j = 0; j < 32; ++j) a[j] = (lane < bn && j <= lane) ? *G.at(F.o0 + kn + lane, F.o0 + kn + j) : ((j == lane) ? 1.0 : 0.0);
                 const int bad = chol_diag32_pair(a, lane, Dt, invd);
                 if (bad && lane == 0) fail = 1;
             }
@@ -184,7 +172,7 @@ __global__ void __launch_bounds__(CHOL_T) ba_front_factor_kernel(const Front* __
                 if (r == nb) { atomicAdd(&Bp[(size_t)pnb * pld + (c_own ? c_idx : pn + c_idx)], u[k]); continue; }
                 bool r_own; int r_idx;
                 if (F.side == 0) { r_own = r >= F.wL; r_idx = r_own ? r - F.wL : r; } else { r_own = r < F.wL; r_idx = r_own ? r : Pf.wL + (r - F.wL); }
-                if (r_own && c_own) atomicAdd(&SG(Pf.o0 + r_idx, Pf.o0 + c_idx), u[k]);          // r_idx >= c_idx: the maps are monotone
+                if (r_own && c_own) atomicAdd(G.at(Pf.o0 + r_idx, Pf.o0 + c_idx), u[k]);          // r_idx >= c_idx: the maps are monotone
                 else if (r_own) atomicAdd(&Bp[(size_t)c_idx * pld + r_idx], u[k]);                 // A(own, left border): stored transposed
                 else if (c_own) atomicAdd(&Bp[(size_t)r_idx * pld + c_idx], u[k]);                 // A(right border, own)
                 else atomicAdd(&Bp[(size_t)r_idx * pld + pn + c_idx], u[k]);                       // border x border
@@ -200,6 +188,7 @@ __global__ void __launch_bounds__(CHOL_T) ba_front_backward_kernel(const Front* 
                                                                     const double* __restrict__ invd_g, const LmState* st) {
     if (st->done) return;
     extern __shared__ __align__(16) double sm[];
+    const CholGlobal G{S, srow, soff};
     const Front F = fr[first + blockIdx.x];
     const int n = F.m, nb = F.nb, ld = F.ld;
     const double* Bd = pool + F.bd;
@@ -217,7 +206,7 @@ __global__ void __launch_bounds__(CHOL_T) ba_front_backward_kernel(const Front* 
         double t = 0.0, my_inv = 1.0;
         if (warp == 0) {
 #pragma unroll
-            for (int i = 0; i < 32; ++i) col[i] = (i < bs && lane < bs && i >= lane) ? SG(F.o0 + kb + i, F.o0 + kb + lane) : 0.0;
+            for (int i = 0; i < 32; ++i) col[i] = (i < bs && lane < bs && i >= lane) ? *G.at(F.o0 + kb + i, F.o0 + kb + lane) : 0.0;
             if (lane < bs) { t = Bd[(size_t)nb * ld + kb + lane]; my_inv = invd_g[F.o0 + kb + lane]; }
         }
         double acc = 0.0;
@@ -225,7 +214,7 @@ __global__ void __launch_bounds__(CHOL_T) ba_front_backward_kernel(const Front* 
             for (int r0 = kb + bs + warp; r0 <= rend; r0 += 16 * nw) {
                 double lv[16], xv[16];
 #pragma unroll
-                for (int u = 0; u < 16; ++u) { const int r = r0 + u * nw; const bool ok = r <= rend; lv[u] = ok ? SG(F.o0 + r, F.o0 + kb + lane) : 0.0; xv[u] = ok ? x[F.o0 + r] : 0.0; }
+                for (int u = 0; u < 16; ++u) { const int r = r0 + u * nw; const bool ok = r <= rend; lv[u] = ok ? *G.at(F.o0 + r, F.o0 + kb + lane) : 0.0; xv[u] = ok ? x[F.o0 + r] : 0.0; }
 #pragma unroll
                 for (int u = 0; u < 16; ++u) acc += lv[u] * xv[u];
             }
@@ -241,15 +230,9 @@ __global__ void __launch_bounds__(CHOL_T) ba_front_backward_kernel(const Front* 
         __syncthreads();
         if (warp == 0) {
             for (int w = 0; w < nw; ++w) t -= part[w * 32 + lane];
-#pragma unroll
-            for (int j = 31; j >= 0; --j) {
-                const double xj = __shfl_sync(0xffffffffu, t * my_inv, j);
-                if (lane == j) t = xj;
-                else if (lane < j) t -= col[j] * xj;
-            }
+            t = chol_back_block(t, my_inv, col, lane);
             if (lane < bs) x[F.o0 + kb + lane] = t;
         }
         __syncthreads();
     }
 }
-#undef SG

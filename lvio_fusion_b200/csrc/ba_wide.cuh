@@ -17,14 +17,15 @@ __global__ void __launch_bounds__(32) ba_wide_diag_kernel(double* __restrict__ S
     if (st->done) return;
     __shared__ __align__(16) double Dt[32 * 34];
     __shared__ double invd[32];
+    const CholGlobal G{S, srow, soff};
     const int lane = threadIdx.x, bs = min(32, n - kb);
     double a[32];
 #pragma unroll
-    for (int j = 0; j < 32; ++j) a[j] = (lane < bs && j <= lane) ? SA(kb + lane, kb + j) : ((j == lane) ? 1.0 : 0.0);
+    for (int j = 0; j < 32; ++j) a[j] = (lane < bs && j <= lane) ? *G.at(kb + lane, kb + j) : ((j == lane) ? 1.0 : 0.0);
     const int bad = chol_diag32_pair(a, lane, Dt, invd);
     if (bad && lane == 0) st->solve_fail = 1;
 #pragma unroll
-    for (int j = 0; j < 32; ++j) if (lane < bs && j <= lane) SA(kb + lane, kb + j) = Dt[j * 34 + lane];
+    for (int j = 0; j < 32; ++j) if (lane < bs && j <= lane) *G.at(kb + lane, kb + j) = Dt[j * 34 + lane];
     if (lane < bs) invd_g[kb + lane] = invd[lane];
 }
 
@@ -34,14 +35,15 @@ __global__ void __launch_bounds__(128) ba_wide_panel_kernel(double* __restrict__
     if (st->done) return;
     __shared__ __align__(16) double Dt[32 * 34];
     __shared__ double invd[32];
+    const CholGlobal G{S, srow, soff};
     const int bs = min(32, n - kb);
-    for (int e = threadIdx.x; e < 32 * 32; e += blockDim.x) { const int k = e >> 5, j = e & 31; Dt[j * 34 + k] = (j <= k && k < bs) ? SA(kb + k, kb + j) : ((j == k) ? 1.0 : 0.0); }
+    for (int e = threadIdx.x; e < 32 * 32; e += blockDim.x) { const int k = e >> 5, j = e & 31; Dt[j * 34 + k] = (j <= k && k < bs) ? *G.at(kb + k, kb + j) : ((j == k) ? 1.0 : 0.0); }
     if (threadIdx.x < 32) invd[threadIdx.x] = threadIdx.x < bs ? invd_g[kb + threadIdx.x] : 1.0;
     __syncthreads();
     const int m = env_rmax[kb >> 5] - (kb + bs) + 1 + 1;
     const int rr = blockIdx.x * blockDim.x + threadIdx.x;
     if (rr >= m) return;
-    double* src = (rr == m - 1) ? (rhs + kb) : &SA(kb + bs + rr, kb);
+    double* src = (rr == m - 1) ? (rhs + kb) : G.at(kb + bs + rr, kb);
     double a[32];
 #pragma unroll
     for (int j = 0; j < 32; ++j) a[j] = (j < bs) ? src[j] : 0.0;
@@ -55,6 +57,7 @@ __global__ void __launch_bounds__(WIDE_WARPS * 32) ba_wide_update_kernel(double*
                                                                          const LmState* st, const int* __restrict__ env_rmax) {
     if (st->done) return;
     extern __shared__ __align__(16) double wsm[];
+    const CholGlobal G{S, srow, soff};
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const int bs = min(32, n - kb);
     const int m = env_rmax[kb >> 5] - (kb + bs) + 1 + 1;
@@ -62,10 +65,8 @@ __global__ void __launch_bounds__(WIDE_WARPS * 32) ba_wide_update_kernel(double*
     const int total = (m > 1) ? ntile * (ntile + 1) / 2 : 0;
     const int t = blockIdx.x * WIDE_WARPS + warp;
     if (t >= total) return;
-    int ti = (int)((sqrt(8.0 * t + 1.0) - 1.0) * 0.5);
-    while ((ti + 1) * (ti + 2) / 2 <= t) ++ti;
-    while (ti * (ti + 1) / 2 > t) --ti;
-    const int tj = t - ti * (ti + 1) / 2;
+    int ti, tj;
+    chol_tile_index(t, ti, tj);
     // the two operand strips (rows of tile row ti, rows of tile row tj) of the panel: 2 x 32 rows x 32 columns, from S / rhs
     double* Pr = wsm + (size_t)warp * 2 * 32 * 34;
     double* Pc = Pr + 32 * 34;
@@ -73,40 +74,25 @@ __global__ void __launch_bounds__(WIDE_WARPS * 32) ba_wide_update_kernel(double*
         const int ir = ti * 32 + r, ic = tj * 32 + r;
         double vr = 0.0, vc = 0.0;
         if (lane < bs) {
-            if (ir < m) vr = (ir == m - 1) ? rhs[kb + lane] : SA(kb + bs + ir, kb + lane);
-            if (ic < m) vc = (ic == m - 1) ? rhs[kb + lane] : SA(kb + bs + ic, kb + lane);
+            if (ir < m) vr = (ir == m - 1) ? rhs[kb + lane] : *G.at(kb + bs + ir, kb + lane);
+            if (ic < m) vc = (ic == m - 1) ? rhs[kb + lane] : *G.at(kb + bs + ic, kb + lane);
         }
         Pr[r * 34 + lane] = vr; Pc[r * 34 + lane] = vc;
     }
     __syncwarp();
     const int ry = lane >> 2, cx = lane & 3;
-    double acc[4][8];
-#pragma unroll
-    for (int i = 0; i < 4; ++i)
-#pragma unroll
-        for (int j = 0; j < 8; ++j) acc[i][j] = 0.0;
+    double acc[4][8] = {};
     const double2* rp[4]; const double2* cp[8];
 #pragma unroll
     for (int i = 0; i < 4; ++i) rp[i] = reinterpret_cast<const double2*>(Pr + (ry + 8 * i) * 34);
 #pragma unroll
     for (int j = 0; j < 8; ++j) cp[j] = reinterpret_cast<const double2*>(Pc + (cx + 4 * j) * 34);
-#pragma unroll 2
-    for (int k = 0; k < 16; ++k) {
-        double2 rv[4], cv[8];
-#pragma unroll
-        for (int i = 0; i < 4; ++i) rv[i] = rp[i][k];
-#pragma unroll
-        for (int j = 0; j < 8; ++j) cv[j] = cp[j][k];
-#pragma unroll
-        for (int i = 0; i < 4; ++i)
-#pragma unroll
-            for (int j = 0; j < 8; ++j) { acc[i][j] += rv[i].x * cv[j].x; acc[i][j] += rv[i].y * cv[j].y; }
-    }
+    chol_tile_product(acc, rp, cp);
 #pragma unroll
     for (int i = 0; i < 4; ++i) {
         const int ip = ti * 32 + ry + 8 * i;
         if (ip >= m) continue;
-        double* dst = (ip == m - 1) ? (rhs + kb + bs) : &SA(kb + bs + ip, kb + bs);
+        double* dst = (ip == m - 1) ? (rhs + kb + bs) : G.at(kb + bs + ip, kb + bs);
 #pragma unroll
         for (int j = 0; j < 8; ++j) { const int jp = tj * 32 + cx + 4 * j; if (jp < m - 1 && jp <= ip) dst[jp] -= acc[i][j]; }
     }
@@ -117,24 +103,20 @@ __global__ void __launch_bounds__(256) ba_wide_backward_kernel(const double* __r
                                                                const double* __restrict__ invd_g, const LmState* st, const int* __restrict__ env_rmax) {
     if (st->done) return;
     __shared__ double part[8 * 32];
+    const CholGlobal G{S, srow, soff};
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nw = blockDim.x >> 5;
     const int bs = min(32, n - kb), rend = env_rmax[kb >> 5];
     double acc = 0.0;
-    if (lane < bs) for (int r = kb + bs + warp; r <= rend; r += nw) acc += SA(r, kb + lane) * rhs[r];
+    if (lane < bs) for (int r = kb + bs + warp; r <= rend; r += nw) acc += *G.at(r, kb + lane) * rhs[r];
     part[warp * 32 + lane] = acc;
     __syncthreads();
     if (warp != 0) return;
     double col[32];
 #pragma unroll
-    for (int i = 0; i < 32; ++i) col[i] = (i < bs && lane < bs && i >= lane) ? SA(kb + i, kb + lane) : 0.0;
+    for (int i = 0; i < 32; ++i) col[i] = (i < bs && lane < bs && i >= lane) ? *G.at(kb + i, kb + lane) : 0.0;
     double t = lane < bs ? rhs[kb + lane] : 0.0;
     const double my_inv = lane < bs ? invd_g[kb + lane] : 1.0;
     for (int w = 0; w < nw; ++w) t -= part[w * 32 + lane];
-#pragma unroll
-    for (int j = 31; j >= 0; --j) {
-        const double xj = __shfl_sync(0xffffffffu, t * my_inv, j);     // lane j's t is final here
-        if (lane == j) t = xj;
-        else if (lane < j) t -= col[j] * xj;
-    }
+    t = chol_back_block(t, my_inv, col, lane);
     if (lane < bs) rhs[kb + lane] = t;
 }

@@ -1,91 +1,29 @@
-// lvb_chol.cuh -- the two latency-critical pieces of the blocked Cholesky kernels (ba_cholesky_kernel, ba_front_factor_kernel):
-// the 32 x 32 diagonal-block factorisation by one warp and the per-row panel solve.
+// lvb_chol.cuh -- the pieces the blocked (32-column, right-looking) Cholesky kernels of the reduced camera system share
+// (ba_cholesky_kernel, the separator tree's ba_front_* and the wide solver's ba_wide_* kernels, all in ba_solve.cu): the element
+// accessors of S, the 32 x 32 diagonal-block factorisation by one warp, the per-row panel solve, the register micro-tile of the
+// trailing update and the 32-step back-substitution of one block.
 //
 // Shared-memory operand: Dt[j * 34 + k] = L[k][j] (the block's factor, column-major with a 16-byte aligned stride), invd[j] = 1 / L[j][j].
 #pragma once
 
-// 1 / sqrt(x) for a positive normal x without the library routine's special-case branch: a single warp is an in-order machine, and
-// that branch (plus the call behind it) fences the scheduler, so nothing independent could be interleaved into the pivot chain's
-// latency.  MUFU.RSQ64H seed (rsqrt.approx.ftz.f64, ~2^-20) + two coupled Newton (Goldschmidt) steps: 2^-40, then below 2^-52.
-__device__ __forceinline__ double rsqrt_pos(double x) {
-    double y;
-    asm("rsqrt.approx.ftz.f64 %0, %1;" : "=d"(y) : "d"(x));
-    double g = x * y, h = 0.5 * y;
-    double r = fma(-g, h, 0.5);
-    g = fma(g, r, g); h = fma(h, r, h);
-    r = fma(-g, h, 0.5);
-    h = fma(h, r, h);
-    return h + h;
-}
+// Element (i, j), i >= j, of S in global memory: lower triangle, row-major at i * srow + j + soff (dense: srow = n, soff = 0;
+// banded of half bandwidth B: srow = soff = B).  T = const double for the kernels that only read S.
+template <class T> struct CholGlobal {
+    T* S; long long srow, soff;
+    __device__ __forceinline__ T* at(int i, int j) const { return S + ((size_t)i * (size_t)srow + (size_t)j + (size_t)soff); }
+};
+template <class T> CholGlobal(T*, long long, long long) -> CholGlobal<T>;
 
-// One warp, lane = row of the block, a[r] = entry (lane, c0 + r) of the block (lower triangle valid).
-// The 32 columns go in 4 groups of 8.  Inside a group a finished column is applied at once only to the group's own columns: its
-// entries L[c0 + r][j] come from the owning lanes by shuffle (no shared-memory round trip, no warp barrier in the chain); the
-// columns right of the group receive the group's rank-8 update in one sweep afterwards, operands broadcast from Dt as LDS.128.
-// Per column the dependent chain is mul -> shuffle -> FMA -> shuffle -> rsqrt (~110 cycles); everything else is independent work
-// the scheduler can place into its shadow because the loop body is branch-free.  Entries above the diagonal are don't-care and are
-// updated without per-lane predicates (garbage stays garbage, nothing valid ever reads it), and nothing is stored to global memory
-// here -- the caller copies the finished block (Dt, invd) to its place with all threads at the start of the next panel phase.
-__device__ __forceinline__ int chol_diag32(double (&a)[32], const int lane, double* __restrict__ Dt, double* __restrict__ invd) {
-    int bad = 0;
-    double d0 = __shfl_sync(0xffffffffu, a[0], 0);
-    if (!(d0 > 0.0)) { bad = 1; d0 = 1.0; }
-    double inv = rsqrt_pos(d0);
-#pragma unroll 1
-    for (int c0 = 0; c0 < 32; c0 += 8) {
-        const int rel = lane - c0;                    // register index of this lane's diagonal entry
-#pragma unroll
-        for (int jj = 0; jj < 8; ++jj) {
-            const int j = c0 + jj;
-            a[jj] *= inv;                             // l_ij for lanes >= j (lane j: sqrt(d_jj)); don't-care above the diagonal
-            Dt[j * 34 + lane] = a[jj];
-            if (rel == jj) invd[j] = inv;
-#pragma unroll
-            for (int r = jj + 1; r < 8; ++r) {        // r = jj + 1 first: it completes the next pivot
-                const double v = __shfl_sync(0xffffffffu, a[jj], c0 + r);
-                a[r] -= a[jj] * v;
-                if (r == jj + 1) {
-                    double dn = __shfl_sync(0xffffffffu, a[jj + 1], j + 1);
-                    if (!(dn > 0.0)) { bad = 1; dn = 1.0; }
-                    inv = rsqrt_pos(dn);
-                }
-            }
-        }
-        if (c0 < 24) {
-            __syncwarp();                             // the group's columns are in Dt
-            // rank-8 update of the columns right of the group: a[r] -= sum_k L[lane][c0 + k] * L[c0 + r][c0 + k].  Register 8 (the next
-            // pivot's column) first, so that its shuffle + rsqrt overlap the rest of the sweep.
-#pragma unroll
-            for (int k = 0; k < 8; ++k) {
-                const double2 v = *reinterpret_cast<const double2*>(Dt + (c0 + k) * 34 + c0 + 8);
-                a[8] -= a[k] * v.x; a[9] -= a[k] * v.y;
-            }
-            double dn = __shfl_sync(0xffffffffu, a[8], c0 + 8);
-            if (!(dn > 0.0)) { bad = 1; dn = 1.0; }
-            inv = rsqrt_pos(dn);
-#pragma unroll
-            for (int r = 10; r < 32; r += 2) {
-                if (c0 + r < 32) {                    // warp-uniform
-#pragma unroll
-                    for (int k = 0; k < 8; ++k) {
-                        const double2 v = *reinterpret_cast<const double2*>(Dt + (c0 + k) * 34 + c0 + r);
-                        a[r] -= a[k] * v.x; a[r + 1] -= a[k] * v.y;
-                    }
-                }
-            }
-        }
-#pragma unroll
-        for (int r = 0; r < 24; ++r) a[r] = a[r + 8];
-#pragma unroll
-        for (int r = 24; r < 32; ++r) a[r] = 0.0;
-    }
-    __syncwarp();
-    return bad;
-}
+// Element (i, j) of block column k = j / 32 in shared memory: rows kb .. rmax[k], row stride 34, block column k at col + boff[k]
+// (chol_resident_columns, ba_plan.h).
+struct CholResident {
+    double* col; const int* boff;
+    __device__ __forceinline__ double* at(int i, int j) const { const int k = j >> 5; return col + boff[k] + (i - (k << 5)) * 34 + (j & 31); }
+};
 
 // 1 / sqrt(x), seed + ONE third-order step  y (1 + e/2 + 3 e^2/8),  e = 1 - x y^2: the seed is good to ~2^-20 (tools/lat_probe.cu prints
 // the measured worst case), the truncation term 5/16 e^3 is then below 2^-58, and the dependent chain is MUFU + 4 FP64 operations
-// instead of MUFU + 6.
+// instead of MUFU + 6 for two Goldschmidt steps (tools/diag_probe.cu compares both).
 __device__ __forceinline__ double rsqrt_pos3(double x) {
     double y;
     asm("rsqrt.approx.ftz.f64 %0, %1;" : "=d"(y) : "d"(x));
@@ -95,10 +33,15 @@ __device__ __forceinline__ double rsqrt_pos3(double x) {
     return fma(ye, p, y);
 }
 
-// Same contract as chol_diag32, two columns per pivot step.  The 2 x 2 pivot block [[p, q], [q, c]] is factored in closed form:
+// One warp, lane = row of the block, a[r] = entry (lane, r) of the block (lower triangle valid; rows past the block's end are
+// identity rows, whose unit pivots leave the valid rows alone); returns 1 on a non-positive pivot.  Two columns per pivot step:
+// the 2 x 2 pivot block [[p, q], [q, c]] is factored in closed form:
 // L11 = sqrt(p), L21 = q / L11, L22 = sqrt(det / p) with det = p c - q^2, so the two reciprocal square roots 1 / sqrt(p) and 1 / sqrt(det)
 // are independent and run side by side -- one MUFU + refinement latency per TWO columns -- and the broadcast / update round trip
-// (shuffle -> FMA -> shuffle) is also paid once per pair.
+// (shuffle -> FMA -> shuffle) is also paid once per pair.  The 32 columns go in 4 groups of 8: a finished pair is applied at once only
+// to the group's own columns, by shuffle; the columns right of the group receive the group's rank-8 update in one sweep afterwards,
+// operands broadcast from Dt as LDS.128.  Entries above the diagonal are don't-care and are updated without per-lane predicates, and
+// nothing is stored to global memory here -- the caller copies the finished block (Dt, invd) to its place.
 __device__ __forceinline__ int chol_diag32_pair(double (&a)[32], const int lane, double* __restrict__ Dt, double* __restrict__ invd) {
     int bad = 0;
 #pragma unroll 1
@@ -163,4 +106,43 @@ __device__ __forceinline__ void chol_panel_row(double (&a)[32], const double* __
             }
         }
     }
+}
+
+// Tile t of the lower triangle of a grid of 32 x 32 tiles, row by row: t -> (ti, tj), tj <= ti.
+__device__ __forceinline__ void chol_tile_index(const int t, int& ti, int& tj) {
+    ti = (int)((sqrt(8.0 * t + 1.0) - 1.0) * 0.5);
+    while ((ti + 1) * (ti + 2) / 2 <= t) ++ti;
+    while (ti * (ti + 1) / 2 > t) --ti;
+    tj = t - ti * (ti + 1) / 2;
+}
+
+// One lane's 4 x 8 register micro-tile of a 32 x 32 tile of P P^T: acc[i][j] += (row rp[i]) . (row cp[j]) over 32 columns, rows read
+// as double2.  The callers give lane the rows ry + 8 i and the columns cx + 4 j (ry = lane / 4, cx = lane % 4): consecutive lanes
+// touch consecutive panel rows, so the LDS.128 operand loads are bank-conflict free and every loaded value feeds 4 or 8 DFMAs.
+// The callers zero acc before they set up rp and cp: zeroing it here instead makes the compiler schedule ba_front_factor_kernel
+// differently.
+__device__ __forceinline__ void chol_tile_product(double (&acc)[4][8], const double2* const (&rp)[4], const double2* const (&cp)[8]) {
+#pragma unroll 2
+    for (int k = 0; k < 16; ++k) {
+        double2 rv[4], cv[8];
+#pragma unroll
+        for (int i = 0; i < 4; ++i) rv[i] = rp[i][k];
+#pragma unroll
+        for (int j = 0; j < 8; ++j) cv[j] = cp[j][k];
+#pragma unroll
+        for (int i = 0; i < 4; ++i)
+#pragma unroll
+            for (int j = 0; j < 8; ++j) { acc[i][j] += rv[i].x * cv[j].x; acc[i][j] += rv[i].y * cv[j].y; }
+    }
+}
+
+// L^T x = t for one diagonal block, one warp: lane i holds t_i, 1 / L[i][i] and col[j] = L[j][i] (j >= i, zero elsewhere); returns x_i.
+__device__ __forceinline__ double chol_back_block(double t, const double my_inv, const double (&col)[32], const int lane) {
+#pragma unroll
+    for (int j = 31; j >= 0; --j) {
+        const double xj = __shfl_sync(0xffffffffu, t * my_inv, j);     // lane j's t is final here
+        if (lane == j) t = xj;
+        else if (lane < j) t -= col[j] * xj;
+    }
+    return t;
 }

@@ -69,6 +69,20 @@ int lidar_segment_ground_device(lvb_ctx* ctx, const float4* in, int n, double th
 int comm_check(lvb_ctx* ctx);                                          // LVB_ERR_COMM when an in-kernel exchange timed out
 int comm_max_seconds(lvb_ctx* ctx, double* seconds);                   // collective: max over the ranks (no-op when world == 1)
 
+// Kernel launches on a context's stream (LAUNCH_ON: on another stream, unnamed): an empty grid launches nothing, every launch is
+// counted in ctx->launches and, with per-kernel timing on, marked with its name.
+#define LAUNCH_ON(ctx, stream_, kernel, grid, block, smem, ...)                            \
+    do { if ((grid) > 0) { kernel<<<(grid), (block), (smem), (stream_)>>>(__VA_ARGS__); (ctx)->launches++; } } while (0)
+#define LAUNCH_AS(ctx, name, kernel, grid, block, smem, ...)                              \
+    do { if ((grid) > 0) { kernel<<<(grid), (block), (smem), (ctx)->stream>>>(__VA_ARGS__); (ctx)->launches++; lvb::timing_mark((ctx)->stream, name); } } while (0)
+#define LAUNCH(ctx, kernel, grid, block, smem, ...) LAUNCH_AS(ctx, #kernel, kernel, grid, block, smem, __VA_ARGS__)
+
+inline int check_launch(const char* what) {
+    cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) { set_error("kernel launch failed in %s: %s", what, cudaGetErrorString(e)); return LVB_ERR_CUDA; }
+    return LVB_OK;
+}
+
 // Minimal owning device buffer on the stream-ordered allocator: a problem object allocates ~40 arrays, and
 // cudaMalloc (a device-wide synchronising call, ~0.1 ms each) would dominate the end-to-end time of a solve that
 // itself takes a couple of milliseconds.  lvb_ctx_create raises the pool's release threshold so freed blocks are
