@@ -244,6 +244,29 @@ LVB_API int lvb_icp_scan_to_map(lvb_icp* icp, int mode, const void* scan, int n,
                         const double frame_pose[7], const double map_pose[7], double rpyxyz[6],
                         double weight, double prior_weight, double huber_a, double dist_thr,
                         const lvb_solve_options* options, lvb_solve_summary* summary);
+/* Mapping::Optimize for one keyframe (mapping.cpp:147-185) against the map frame lvb_icp_map_build made on each handle:
+ *   rpyxyz = se32rpyxyz(map_pose^-1 * pose)                                        (computed once, from the incoming pose)
+ *   ground: ScanToMapWithGround + Solve, pose = map_pose * rpyxyz2se3(rpyxyz)
+ *   surf:   ScanToMapWithSegmented + Solve from that rpyxyz, queries transformed by the pose the ground solve produced; pose again
+ *   ToWorld: each robot-frame cloud, transformed by pose.cast<float>(), is stored under `key` in its handle, replacing what `key`
+ *            held; lvb_icp_map_append(NULL) on a handle afterwards refers to this call's cloud.
+ * All on the device with one host synchronisation, at the end.  Index [0] of weight / huber_a / dist_thr / summary is the ground
+ * registration, [1] the surf one, with the meaning lvb_icp_scan_to_map gives them; prior_weight < 0 omits both priors.
+ * A NULL handle skips that registration and its ToWorld (mapping.cpp:155,167 skip a registration whose map cloud is empty); its
+ * summary is zero with termination_type = -1.  ToWorld still stores that keyframe's cloud in the reference (mapping.cpp:215-216):
+ * the caller does it with lvb_icp_map_evict(key) + lvb_icp_map_append(key, cloud, returned pose) on that side's handle
+ * (lvio_b200/association.h, OptimizeKeyframe, does).  Both handles belong to one context.  total_time_in_seconds is the whole call's.
+ * LVB_ERR_STATE when a handle has no map; LVB_ERR_INVALID when options.max_solver_time_in_seconds is set (< 1e8: Mapping::Optimize
+ * sets no limit, and the call decides nothing on the host); LVB_ERR_UNSUPPORTED on a context with world_size > 1 (sharded
+ * registration: lvb_icp_scan_to_map).  Errors are reported before any state changes. */
+typedef struct lvb_map_optimize_params {
+    double weight[2], prior_weight, huber_a[2], dist_thr[2];   /* association.cpp:270-384 */
+    lvb_solve_options options;                                 /* mapping.cpp:159-162: DENSE_QR, max_num_iterations = 4 */
+} lvb_map_optimize_params;
+LVB_API int lvb_icp_map_optimize_keyframe(lvb_icp* ground, lvb_icp* surf, const double map_pose[7], long long key,
+                                          const void* ground_pts, int n_ground, const void* surf_pts, int n_surf, int stride_bytes,
+                                          const lvb_map_optimize_params* p, double pose[7] /* in: frame->pose, out: optimised */,
+                                          double rpyxyz[6] /* out */, lvb_solve_summary summary[2]);
 
 /* ---- lidar feature pipeline, the producer of the scan-to-map inputs (SURVEY 8(f).2).
  * Stands behind FeatureAssociation::Process (association.cpp:88-268: Preprocess, AdjustDistortion, CalculateSmoothness,

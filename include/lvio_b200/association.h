@@ -85,11 +85,63 @@ public:
     bool BuildMapFrame(const long long* keys, int n_keys, double ground_ransac_threshold) {
         Handles& h = handles_of_thread()[this];
         if (!ensure_handles(h)) return false;
-        h.resident = lvb_icp_map_build(h.ground, keys, n_keys, cell_of(resolution_ * resolution_ * 100), ground_ransac_threshold, nullptr) == LVB_OK &&
-                     lvb_icp_map_build(h.surf, keys, n_keys, cell_of(resolution_ * resolution_ * 25), -1.0, nullptr) == LVB_OK;
+        // each side is built on its own: OptimizeKeyframe registers whichever side has a map frame cloud (mapping.cpp:155,167)
+        h.ground_map = lvb_icp_map_build(h.ground, keys, n_keys, cell_of(resolution_ * resolution_ * 100), ground_ransac_threshold, nullptr) == LVB_OK;
+        h.surf_map = lvb_icp_map_build(h.surf, keys, n_keys, cell_of(resolution_ * resolution_ * 25), -1.0, nullptr) == LVB_OK;
+        h.resident = h.ground_map && h.surf_map;
         return h.resident;
     }
-    void UsePerCallMap() { handles_of_thread()[this].resident = false; }
+    void UsePerCallMap() { Handles& h = handles_of_thread()[this]; h.resident = h.ground_map = h.surf_map = false; }
+
+    // What ScanToMapWithGround / ScanToMapWithSegmented put into their problems for `frame` (association.cpp:270-384: weights, the
+    // PoseErrorRPZ / YXY prior unless relocating, TrivialLoss / HuberLoss(0.1), the two gates) and the options of the two Solve
+    // calls of Mapping::Optimize (mapping.cpp:159-162, 171-174), as lvb_icp_map_optimize_keyframe takes them.
+    template <class FramePtr>
+    lvb_map_optimize_params MapOptimizeParams(FramePtr frame, bool relocate = false) const {
+        lvb_map_optimize_params p;
+        p.weight[0] = frame->weights.lidar_ground; p.weight[1] = frame->weights.lidar_surf;
+        p.prior_weight = relocate ? -1.0 : (double)frame->features_left.size() * frame->weights.visual;
+        p.huber_a[0] = 0.0; p.huber_a[1] = 0.1;
+        p.dist_thr[0] = resolution_ * resolution_ * 100; p.dist_thr[1] = resolution_ * resolution_ * 25;
+        lvb_default_options(&p.options);
+        p.options.linear_solver_type = 2;            // DENSE_QR
+        p.options.max_num_iterations = 4;
+        return p;
+    }
+    // The body of Mapping::Optimize's loop after BuildMapFrame (mapping.cpp:152-185 without PoseGraph::ForwardUpdate): the
+    // registrations against the map frame BuildMapFrame just made, frame->pose updated in place, then ToWorld of the keyframe's two
+    // robot-frame clouds under `key` -- one device call, one host synchronisation.  As in the reference, a side whose map frame
+    // cloud could not be built (BuildMapFrame with no keys: the first lidar keyframe, mapping.cpp:118-119; an empty merged cloud,
+    // :155,167) is not registered, and ToWorld stores both clouds whatever ran (:185).  summary: 2 entries (ground, surf) or NULL;
+    // a registration that did not run has termination_type = -1.  false: a library call failed (lvb_last_error()).
+    template <class FramePtr>
+    bool OptimizeKeyframe(FramePtr frame, const double* map_pose7, long long key, lvb_solve_summary* summary = nullptr) {
+        Handles& h = handles_of_thread()[this];
+        if (!ensure_handles(h)) return false;
+        const auto& g = frame->feature_lidar->points_ground;
+        const auto& s = frame->feature_lidar->points_surf;
+        const int stride = (int)sizeof(assoc_detail::cloud_data(g, 0)[0]);
+        lvb_icp* reg_g = h.ground_map ? h.ground : nullptr;
+        lvb_icp* reg_s = h.surf_map ? h.surf : nullptr;
+        lvb_solve_summary sums[2];
+        lvb_solve_summary* out = summary ? summary : sums;
+        if (reg_g || reg_s) {
+            const lvb_map_optimize_params p = MapOptimizeParams(frame);
+            double rpyxyz[6];
+            if (lvb_icp_map_optimize_keyframe(reg_g, reg_s, map_pose7, key, assoc_detail::cloud_data(g, 0), (int)g.size(),
+                                              assoc_detail::cloud_data(s, 0), (int)s.size(), stride, &p, frame->pose.data(), rpyxyz, out) != LVB_OK)
+                return false;
+        } else {
+            for (int m = 0; m < 2; ++m) { std::memset(&out[m], 0, sizeof(out[m])); out[m].termination_type = -1; }
+        }
+        // ToWorld of a side that was not registered: the call above stores only the clouds of the handles it was given
+        const double* pose = frame->pose.data();
+        if (!reg_g && !(lvb_icp_map_evict(h.ground, key) == LVB_OK &&
+                        lvb_icp_map_append(h.ground, key, assoc_detail::cloud_data(g, 0), (int)g.size(), stride, pose) == LVB_OK)) return false;
+        if (!reg_s && !(lvb_icp_map_evict(h.surf, key) == LVB_OK &&
+                        lvb_icp_map_append(h.surf, key, assoc_detail::cloud_data(s, 0), (int)s.size(), stride, pose) == LVB_OK)) return false;
+        return true;
+    }
 
 private:
     static float cell_of(double thr) { return std::nextafter((float)std::sqrt(thr), 1e30f) * 1.0001f; }
@@ -100,8 +152,11 @@ private:
         if (!rt.ensure()) { delete loss; return false; }
         if (!icp && lvb_icp_create(rt.ctx, &icp) != LVB_OK) { delete loss; return false; }
         const int stride = (int)sizeof(assoc_detail::cloud_data(scan, 0)[0]);
-        if (!handles_of_thread()[this].resident &&
-            lvb_icp_set_map(icp, assoc_detail::cloud_data(map, 0), (int)map.size(), stride, cell_of(thr)) != LVB_OK) { delete loss; return false; }
+        Handles& h = handles_of_thread()[this];
+        if (!h.resident) {
+            (mode == 0 ? h.ground_map : h.surf_map) = false;          // the per-call map replaces this side's map frame
+            if (lvb_icp_set_map(icp, assoc_detail::cloud_data(map, 0), (int)map.size(), stride, cell_of(thr)) != LVB_OK) { delete loss; return false; }
+        }
         if (mode == 0) { problem.AddParameterBlock(para + 1, 1); problem.AddParameterBlock(para + 2, 1); problem.AddParameterBlock(para + 5, 1); }
         else { problem.AddParameterBlock(para + 0, 1); problem.AddParameterBlock(para + 3, 1); problem.AddParameterBlock(para + 4, 1); }
         double* x0 = mode == 0 ? para + 1 : para + 0; double* x1 = mode == 0 ? para + 2 : para + 3; double* x2 = mode == 0 ? para + 5 : para + 4;
@@ -120,7 +175,8 @@ private:
     // lvb_icp handles (voxel hash + scratch on one context's stream) are single-threaded and the context is per host thread
     // (ceres_shim.h): Mapping::Optimize and Relocator::RelocateByPoints reach the same object from two threads without a lock
     // (mapping.cpp:155-177, relocator.cpp:188-206), so every thread gets its own pair.
-    struct Handles { lvb_icp* ground = nullptr; lvb_icp* surf = nullptr; bool resident = false; };
+    // resident: both map frames built (ScanToMapWith* use them); ground_map / surf_map: that side's map frame is the last BuildMapFrame's
+    struct Handles { lvb_icp* ground = nullptr; lvb_icp* surf = nullptr; bool resident = false, ground_map = false, surf_map = false; };
     static bool ensure_handles(Handles& h) {
         lvb::Runtime& rt = lvb::Runtime::get();
         if (!rt.ensure()) return false;

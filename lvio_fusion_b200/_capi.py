@@ -65,6 +65,17 @@ class LidarConfig(C.Structure):
     ]
 
 
+class MapOptimizeParams(C.Structure):
+    """lvb_map_optimize_params (include/lvio_b200.h): [0] ground registration, [1] surf registration."""
+    _fields_ = [
+        ("weight", C.c_double * 2),
+        ("prior_weight", C.c_double),
+        ("huber_a", C.c_double * 2),
+        ("dist_thr", C.c_double * 2),
+        ("options", SolveOptions),
+    ]
+
+
 VP = C.c_void_p
 _SIGS = {
     "version": (C.c_int, []),
@@ -121,6 +132,8 @@ _LVB_ONLY = {
     "icp_map_evict": (C.c_int, [VP, C.c_longlong]),
     "icp_map_build": (C.c_int, [VP, C.POINTER(C.c_longlong), C.c_int, C.c_float, C.c_double, c_int_p]),
     "icp_map_download": (C.c_int, [VP, c_float_p, C.c_int, c_int_p]),
+    "icp_map_optimize_keyframe": (C.c_int, [VP, VP, c_double_p, C.c_longlong, VP, C.c_int, VP, C.c_int, C.c_int,
+                                            C.POINTER(MapOptimizeParams), c_double_p, c_double_p, C.POINTER(SolveSummary)]),
     "debug_timing": (C.c_int, [C.c_int]),
     "debug_cholesky_clocks": (C.c_int, [C.POINTER(C.c_longlong), C.c_int]),
     "debug_timing_report": (C.c_int, [C.c_char_p, C.c_int]),

@@ -343,6 +343,43 @@ class FeatureAssociation:
         return e, s
 
 
+def optimize_keyframe(ground, surf, key, map_pose, pose, ground_points, surf_points, weight, prior_weight, huber_a, dist_thr,
+                      options=None, **kw):
+    """Mapping::Optimize for one keyframe (mapping.cpp:147-185) in one device call (CUDA library only): both registrations against the
+    map frames that map_build made on `ground` / `surf` (FeatureAssociation handles of one context; None skips that registration),
+    the pose hand-off between them, and ToWorld of the two robot-frame clouds under `key`.  weight, huber_a and dist_thr are
+    (ground, surf) pairs as ScanToMapWithGround / ScanToMapWithSegmented derive them.  Returns (pose, rpyxyz, (ground summary,
+    surf summary)); a skipped registration's summary has termination_type -1.  Keyword arguments set solver options, on top of
+    `options` when it is given."""
+    if ground is None and surf is None:
+        raise ValueError("optimize_keyframe: at least one of ground / surf is needed")
+    api = (ground or surf).api
+    pts, n, strides = [None, None], [0, 0], set()
+    for m, (fa, cloud) in enumerate(((ground, ground_points), (surf, surf_points))):
+        if fa is not None:
+            pts[m], n[m], stride = FeatureAssociation._cloud(cloud)
+            strides.add(stride)
+    if len(strides) != 1:
+        raise ValueError("optimize_keyframe: the ground and surf clouds must have the same record stride, got %s" % sorted(strides))
+    prm = _capi.MapOptimizeParams()
+    for k in range(2):
+        prm.weight[k], prm.huber_a[k], prm.dist_thr[k] = float(weight[k]), float(huber_a[k]), float(dist_thr[k])
+    prm.prior_weight = float(prior_weight)
+    if options is None:
+        options = default_options(api, max_num_iterations=4, linear_solver_type=DENSE_QR)
+    prm.options = options                # a copy: kw below does not touch the caller's structure
+    for k, v in kw.items():
+        setattr(prm.options, k, v)
+    mp = _f64(map_pose).reshape(7)
+    p = _f64(pose).reshape(7).copy()
+    e = np.zeros(6)
+    s = (SolveSummary * 2)()
+    vp = [None if a is None else a.ctypes.data_as(C.c_void_p) for a in pts]
+    api.check(api.icp_map_optimize_keyframe(ground.h if ground else None, surf.h if surf else None, _dp(mp), int(key), vp[0], n[0], vp[1], n[1],
+                                            strides.pop(), C.byref(prm), _dp(p), _dp(e), s), "icp_map_optimize_keyframe")
+    return p, e, (s[0], s[1])
+
+
 def _fp(a):
     return None if a is None else a.ctypes.data_as(_capi.c_float_p)
 

@@ -1242,22 +1242,8 @@ struct Stager {
         static const bool off = getenv("LVB_NO_STAGING") && getenv("LVB_NO_STAGING")[0] == '1';      // A/B switch
         if (off) staged = false;
     }
-    int begin() {
-        if (!staged) return LVB_OK;
-        if (!ctx->stage_ev) LVB_CUDA(cudaEventCreateWithFlags(&ctx->stage_ev, cudaEventDisableTiming));
-        if (ctx->stage_busy) { LVB_CUDA(cudaEventSynchronize(ctx->stage_ev)); ctx->stage_busy = false; }      // the previous problem's copy has read it
-        return LVB_OK;
-    }
-    int grow(size_t need) {
-        if (need <= ctx->stage_cap) return LVB_OK;
-        size_t cap = std::max<size_t>(std::max<size_t>(2 * ctx->stage_cap, need), (size_t)4 << 20);
-        unsigned char* q = nullptr;
-        LVB_CUDA(cudaHostAlloc((void**)&q, cap, cudaHostAllocDefault));
-        if (used) memcpy(q, ctx->stage_h, used);
-        if (ctx->stage_h) cudaFreeHost(ctx->stage_h);
-        ctx->stage_h = q; ctx->stage_cap = cap;
-        return LVB_OK;
-    }
+    int begin() { return staged ? lvb::stage_wait(ctx) : LVB_OK; }      // the previous problem's copy has read it
+    int grow(size_t need) { return lvb::stage_grow(ctx, need, used); }
     // memory for `count` elements of dst, to be filled by the caller before the next reserve / put; finish() after filling
     template <class T> int reserve(DevBuf<T>& dst, size_t count, T** out) {
         const size_t c = std::max<size_t>(count, 1), bytes = c * sizeof(T);
@@ -1293,8 +1279,7 @@ struct Stager {
         arena.release();
         LVB_TRY(arena.ensure(std::max<size_t>(used, 256)));
         LVB_CUDA(cudaMemcpyAsync(arena.p, ctx->stage_h, used, cudaMemcpyHostToDevice, s));
-        LVB_CUDA(cudaEventRecord(ctx->stage_ev, s));
-        ctx->stage_busy = true;
+        LVB_TRY(lvb::stage_mark_busy(ctx, s));
         for (const Item& it : items) it.bind(it.buf, arena.p, it.off, it.count);
         return LVB_OK;
     }

@@ -26,6 +26,27 @@ int cuda_fail(cudaError_t e, const char* what, const char* file, int line) {
     return LVB_ERR_CUDA;
 }
 
+int stage_wait(lvb_ctx* ctx) {
+    if (!ctx->stage_ev) LVB_CUDA(cudaEventCreateWithFlags(&ctx->stage_ev, cudaEventDisableTiming));
+    if (ctx->stage_busy) { LVB_CUDA(cudaEventSynchronize(ctx->stage_ev)); ctx->stage_busy = false; }
+    return LVB_OK;
+}
+int stage_grow(lvb_ctx* ctx, size_t need, size_t keep) {
+    if (need <= ctx->stage_cap) return LVB_OK;
+    const size_t cap = std::max<size_t>(std::max<size_t>(2 * ctx->stage_cap, need), (size_t)4 << 20);
+    unsigned char* q = nullptr;
+    LVB_CUDA(cudaHostAlloc((void**)&q, cap, cudaHostAllocDefault));
+    if (keep) memcpy(q, ctx->stage_h, keep);
+    if (ctx->stage_h) cudaFreeHost(ctx->stage_h);
+    ctx->stage_h = q; ctx->stage_cap = cap;
+    return LVB_OK;
+}
+int stage_mark_busy(lvb_ctx* ctx, cudaStream_t s) {
+    LVB_CUDA(cudaEventRecord(ctx->stage_ev, s));
+    ctx->stage_busy = true;
+    return LVB_OK;
+}
+
 bool g_timing = false;
 static std::vector<std::pair<const char*, cudaEvent_t>> g_marks;
 void timing_mark(cudaStream_t s, const char* name) {

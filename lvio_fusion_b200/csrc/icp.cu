@@ -15,6 +15,7 @@
 #include <math.h>
 #include <algorithm>
 #include <chrono>
+#include <memory>
 #include <stdlib.h>
 #include <string.h>
 #include <vector>
@@ -211,10 +212,10 @@ __device__ __forceinline__ Best3 knn3_query(const IcpDev& d, float3 q) {
 // every ring): 0.57 ms -- the lanes prune with their own looser bounds and scan more voxels than the chain they shorten; runs only for
 // the face rows of the outer rings (r >= 2): 0.57 ms.  The kernel takes ~0.47 - 0.50 ms whether a rank holds 120 k, 60 k or 30 k of
 // the queries (round-2 runs at 1 / 2 / 4 GPUs): its duration is set by its slowest warps, not by the query count.
-__global__ void icp_query_key_kernel(IcpDev d, int shift, int cgx, int cgy, int cgz, int* __restrict__ key, int* __restrict__ counts) {
+__device__ __forceinline__ void query_key(const IcpDev& d, const float* tf, int shift, int cgx, int cgy, int cgz, int* __restrict__ key, int* __restrict__ counts) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= d.K) return;
-    const float3 q = transform_f32(d.tf, load_xyz(d.scan, i, d.stride));
+    const float3 q = transform_f32(tf, load_xyz(d.scan, i, d.stride));
     const Grid& g = d.g;
     const int ix = clampi(cell_coord(q.x, g.minx, g.inv_cell), 0, g.gx - 1) >> shift;
     const int iy = clampi(cell_coord(q.y, g.miny, g.inv_cell), 0, g.gy - 1) >> shift;
@@ -222,6 +223,15 @@ __global__ void icp_query_key_kernel(IcpDev d, int shift, int cgx, int cgy, int 
     const int c = ix + cgx * (iy + cgy * iz);
     key[i] = c;
     atomicAdd(&counts[c], 1);
+}
+__global__ void icp_query_key_kernel(IcpDev d, int shift, int cgx, int cgy, int cgz, int* __restrict__ key, int* __restrict__ counts) {
+    query_key(d, d.tf, shift, cgx, cgy, cgz, key, counts);
+}
+// the same with the query transform read from device memory (float[7], written by an earlier kernel: lvb_icp_map_optimize_keyframe)
+__global__ void icp_query_key_dev_tf_kernel(IcpDev d, const float* __restrict__ tf7, int shift, int cgx, int cgy, int cgz, int* __restrict__ key, int* __restrict__ counts) {
+    float tf[7];
+    for (int k = 0; k < 7; ++k) tf[k] = tf7[k];
+    query_key(d, tf, shift, cgx, cgy, cgz, key, counts);
 }
 __global__ void icp_query_scatter_kernel(int n, const int* __restrict__ key, const int* __restrict__ start, int* __restrict__ fill, int* __restrict__ order) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -240,11 +250,11 @@ __global__ void __launch_bounds__(ITPB) icp_knn_kernel(IcpDev d, int* __restrict
 }
 
 // K8: transform + 3-NN + gate (association.cpp:296-300) + plane constants (lidar_error.hpp:13-18)
-__global__ void __launch_bounds__(ITPB) icp_associate_kernel(IcpDev d) {
+__device__ __forceinline__ void associate_query(const IcpDev& d, const float* tf) {
     const int t = blockIdx.x * ITPB + threadIdx.x;
     if (t >= d.K) return;
     const int i = d.order ? d.order[t] : t;
-    const float3 q = transform_f32(d.tf, load_xyz(d.scan, i, d.stride));
+    const float3 q = transform_f32(tf, load_xyz(d.scan, i, d.stride));
     const Best3 b = knn3_query(d, q);
     int ok = 1;
     for (int j = 0; j < 3; ++j) if (!(b.i[j] >= 0 && b.i[j] < d.P && (double)b.d[j] < d.thr)) ok = 0;
@@ -254,6 +264,13 @@ __global__ void __launch_bounds__(ITPB) icp_associate_kernel(IcpDev d) {
     const V3 n = plane_normal(v3(a.x, a.y, a.z), v3(bb.x, bb.y, bb.z), v3(c.x, c.y, c.z));
     d.pa[i] = a.x; d.pa[d.K + i] = a.y; d.pa[2 * d.K + i] = a.z;
     d.nrm[i] = n.x; d.nrm[d.K + i] = n.y; d.nrm[2 * (size_t)d.K + i] = n.z;
+}
+__global__ void __launch_bounds__(ITPB) icp_associate_kernel(IcpDev d) { associate_query(d, d.tf); }
+// the same with the query transform read from device memory (see icp_query_key_dev_tf_kernel)
+__global__ void __launch_bounds__(ITPB) icp_associate_dev_tf_kernel(IcpDev d, const float* __restrict__ tf7) {
+    float tf[7];
+    for (int k = 0; k < 7; ++k) tf[k] = tf7[k];
+    associate_query(d, tf);
 }
 
 __device__ __forceinline__ void icp_substitute(const IcpState& s, const double* x, double* e) {
@@ -384,6 +401,110 @@ __global__ void icp_post_kernel(IcpState* st) {
     }
 }
 
+// ---- Mapping::Optimize for one keyframe on the device (lvb_icp_map_optimize_keyframe): the pose arithmetic between the two
+// registrations.  FP64 on one thread; every product and sum is rounded on its own (__dmul_rn / __dadd_rn / __dsub_rn: no FMA
+// contraction), in the operation order of the host formulas cited at each function.  Poses are [qx qy qz qw tx ty tz].
+struct KfBlock {             // the call's device state, read back with one copy at its end
+    IcpState st[2];          // [0] ground (mode 0), [1] surf (mode 1)
+    double map_pose[7];      // map_frame->pose                                   (uploaded)
+    double pose[7];          // frame->pose: the incoming one, then after each registration
+    double rpyxyz[6];
+    float tf[8];             // pose.cast<float>(): the query transform of the next association, then of ToWorld
+};
+struct KfSeed {              // what ScanToMapWith* put in each problem (association.cpp:270-384) and the solver options
+    lvb_solve_options o;
+    double weight[2], huber_a[2], prior_w;
+};
+__constant__ int c_free[2][3] = {{1, 2, 5}, {0, 3, 4}};     // rpyxyz entries a registration solves for: pitch roll z / yaw x y
+
+__device__ __forceinline__ double dm(double a, double b) { return __dmul_rn(a, b); }
+__device__ __forceinline__ double da(double a, double b) { return __dadd_rn(a, b); }
+__device__ __forceinline__ double ds(double a, double b) { return __dsub_rn(a, b); }
+
+// Sophus::SO3 construction from a quaternion (so3.hpp): coeffs /= norm(), squared norm summed x, y, z, w
+__device__ void kf_normalize(double* q) {
+    const double n = __dsqrt_rn(da(da(da(dm(q[0], q[0]), dm(q[1], q[1])), dm(q[2], q[2])), dm(q[3], q[3])));
+    for (int k = 0; k < 4; ++k) q[k] = __ddiv_rn(q[k], n);
+}
+// SO3 * point = Eigen QuaternionBase::_transformVector: uv = 2 (q.vec x p); p + w uv + q.vec x uv
+__device__ void kf_rotate(const double* q, const double* p, double* out) {
+    double uv[3] = {ds(dm(q[1], p[2]), dm(q[2], p[1])), ds(dm(q[2], p[0]), dm(q[0], p[2])), ds(dm(q[0], p[1]), dm(q[1], p[0]))};
+    for (int k = 0; k < 3; ++k) uv[k] = da(uv[k], uv[k]);
+    const double c[3] = {ds(dm(q[1], uv[2]), dm(q[2], uv[1])), ds(dm(q[2], uv[0]), dm(q[0], uv[2])), ds(dm(q[0], uv[1]), dm(q[1], uv[0]))};
+    for (int k = 0; k < 3; ++k) out[k] = da(da(p[k], dm(q[3], uv[k])), c[k]);
+}
+// SE3 * SE3 (Sophus se3.hpp): q = qa qb (Eigen's quaternion product), renormalised by 2 / (1 + |q|^2) when |q|^2 != 1 (so3.hpp
+// SO3Base::operator*); t = ta + qa tb
+__device__ void kf_se3_mul(const double* a, const double* b, double* c) {
+    const double aw = a[3], ax = a[0], ay = a[1], az = a[2], bw = b[3], bx = b[0], by = b[1], bz = b[2];
+    double q[4];
+    q[3] = ds(ds(ds(dm(aw, bw), dm(ax, bx)), dm(ay, by)), dm(az, bz));
+    q[0] = ds(da(da(dm(aw, bx), dm(ax, bw)), dm(ay, bz)), dm(az, by));
+    q[1] = ds(da(da(dm(aw, by), dm(ay, bw)), dm(az, bx)), dm(ax, bz));
+    q[2] = ds(da(da(dm(aw, bz), dm(az, bw)), dm(ax, by)), dm(ay, bx));
+    const double n2 = da(da(da(dm(q[0], q[0]), dm(q[1], q[1])), dm(q[2], q[2])), dm(q[3], q[3]));
+    if (n2 != 1.0) { const double s = __ddiv_rn(2.0, da(1.0, n2)); for (int k = 0; k < 4; ++k) q[k] = dm(q[k], s); }
+    double t[3];
+    kf_rotate(a, b + 4, t);
+    for (int k = 0; k < 4; ++k) c[k] = q[k];
+    for (int k = 0; k < 3; ++k) c[4 + k] = da(a[4 + k], t[k]);
+}
+// SE3::inverse (se3.hpp): R^-1 = SO3(conjugate), t^-1 = R^-1 (-t)
+__device__ void kf_se3_inv(const double* a, double* c) {
+    c[0] = -a[0]; c[1] = -a[1]; c[2] = -a[2]; c[3] = a[3];
+    kf_normalize(c);
+    const double mt[3] = {-a[4], -a[5], -a[6]};
+    kf_rotate(c, mt, c + 4);
+}
+// se32rpyxyz (utility.cpp:27-33): ceres::EigenQuaternionToRPY (ceres/base.hpp:95-108), then the translation
+__device__ void kf_se32rpyxyz(const double* T, double* e) {
+    const double q0 = T[3], q1 = T[0], q2 = T[1], q3 = T[2];
+    e[0] = atan2(dm(2.0, da(dm(q1, q2), dm(q0, q3))), ds(1.0, dm(2.0, da(dm(q2, q2), dm(q3, q3)))));
+    e[1] = asin(dm(2.0, ds(dm(q0, q2), dm(q1, q3))));
+    e[2] = atan2(dm(2.0, da(dm(q2, q3), dm(q0, q1))), ds(1.0, dm(2.0, da(dm(q1, q1), dm(q2, q2)))));
+    e[3] = T[4]; e[4] = T[5]; e[5] = T[6];
+}
+// rpyxyz2se3 (utility.cpp:35-40): ceres::RPYToEigenQuaternion (ceres/base.hpp:110-132), SE3d(Quaterniond(q), t) normalises q
+__device__ void kf_rpyxyz2se3(const double* e, double* T) {
+    const double z = __ddiv_rn(e[0], 2.0), y = __ddiv_rn(e[1], 2.0), x = __ddiv_rn(e[2], 2.0);
+    const double cz = cos(z), sz = sin(z), cy = cos(y), sy = sin(y), cx = cos(x), sx = sin(x);
+    T[3] = da(dm(dm(cz, cy), cx), dm(dm(sz, sy), sx));
+    T[0] = ds(dm(dm(cz, cy), sx), dm(dm(sz, sy), cx));
+    T[1] = da(dm(dm(cz, sy), cx), dm(dm(sz, cy), sx));
+    T[2] = ds(dm(dm(sz, cy), cx), dm(dm(cz, sy), sx));
+    kf_normalize(T);
+    T[4] = e[3]; T[5] = e[4]; T[6] = e[5];
+}
+
+// One step of mapping.cpp:147-185 on one thread.
+//   from < 0  : rpyxyz = se32rpyxyz(map_pose^-1 * pose)                                   (mapping.cpp:154)
+//   from = m  : registration m is solved: its free scalars go back into rpyxyz, pose = map_pose * rpyxyz2se3(rpyxyz)  (:165, :177)
+//   then      : tf = pose.cast<float>() (association.cpp:287, mapping.cpp:195), and with seed = m the IcpState of registration m
+//               is set up from rpyxyz as lvb_icp_scan_to_map's init_state does on the host
+__global__ void icp_kf_pose_kernel(KfBlock* b, int from, int seed, KfSeed p) {
+    if (from < 0) {
+        double inv[7], rel[7];
+        kf_se3_inv(b->map_pose, inv);
+        kf_se3_mul(inv, b->pose, rel);
+        kf_se32rpyxyz(rel, b->rpyxyz);
+    } else {
+        for (int k = 0; k < 3; ++k) b->rpyxyz[c_free[from][k]] = b->st[from].x[k];
+        double rel[7];
+        kf_rpyxyz2se3(b->rpyxyz, rel);
+        kf_se3_mul(b->map_pose, rel, b->pose);
+    }
+    for (int k = 0; k < 7; ++k) b->tf[k] = __double2float_rn(b->pose[k]);
+    if (seed < 0) return;
+    IcpState& s = b->st[seed];
+    memset(&s, 0, sizeof(s));
+    lm_init(s.lm, p.o);
+    s.mode = seed;
+    for (int k = 0; k < 7; ++k) s.Twc1[k] = b->map_pose[k];
+    for (int k = 0; k < 6; ++k) s.rpyxyz[k] = b->rpyxyz[k];
+    for (int k = 0; k < 3; ++k) { s.x[k] = b->rpyxyz[c_free[seed][k]]; s.cand[k] = s.x[k]; s.prior_target[k] = s.x[k]; }
+    s.prior_w = p.prior_w; s.huber_a = p.huber_a[seed]; s.weight = p.weight[seed];
+}
+
 }  // namespace
 
 // ====================================================================================== host side
@@ -408,6 +529,10 @@ struct lvb_icp {
     std::vector<Segment> segments;
     DevBuf<float4> merged, merged2;
     int scan_n = 0, scan_stride = 0;          // the scan of the last upload_scan (reusable by lvb_icp_map_append)
+    const unsigned char* scan_dev = nullptr;  // where that scan lies: scan_raw, or this handle's part of kf_arena
+    // lvb_icp_map_optimize_keyframe's upload: [KfBlock | ground scan | surf scan] in one allocation, held by both handles of the call
+    // so that either one's scan stays valid for lvb_icp_map_append(NULL) until that handle uploads another scan
+    std::shared_ptr<DevBuf<unsigned char>> kf_arena;
     ~lvb_icp() { for (auto& sg : segments) delete sg.pts; }
 };
 
@@ -421,20 +546,18 @@ static int icheck(const char* what) {
     return LVB_OK;
 }
 
-static int upload_scan(lvb_icp* h, const void* scan, int n, int stride, const double* frame_pose, float max_d2, double thr, IcpDev& d) {
-    if (!h->have_map) { set_error("set_map first"); return LVB_ERR_STATE; }
-    if (n < 0 || stride < 12 || (stride & 3) || (n && !scan)) { set_error("bad scan arguments"); return LVB_ERR_INVALID; }
+// The association buffers and the visiting order of the n queries at d_scan (device, stride bytes each).  The query transform is
+// d.tf (set by the caller), or, when tf_dev is given, the float[7] at tf_dev in device memory.
+static int bind_scan(lvb_icp* h, const unsigned char* d_scan, int n, int stride, const float* tf_dev, float max_d2, double thr, IcpDev& d) {
     cudaStream_t s = h->ctx->stream;
-    LVB_TRY(h->scan_raw.upload((const unsigned char*)scan, (size_t)n * stride, s));
-    h->scan_n = n; h->scan_stride = stride;
+    h->scan_n = n; h->scan_stride = stride; h->scan_dev = d_scan;
     LVB_TRY(h->accepted.ensure(std::max(1, n)));
     LVB_TRY(h->pa.ensure((size_t)std::max(1, n) * 3));
     LVB_TRY(h->nrm.ensure((size_t)std::max(1, n) * 3));
     LVB_TRY(h->st.ensure(1));
     d.map = h->map_sorted.p; d.cell_start = h->cell_start.p; d.g = h->grid; d.P = h->P;
     d.coarse = h->coarse.p; d.cbx = h->cbx; d.cby = h->cby; d.cbz = h->cbz;
-    d.scan = h->scan_raw.p; d.K = n; d.stride = stride;
-    for (int i = 0; i < 7; ++i) d.tf[i] = (float)frame_pose[i];
+    d.scan = d_scan; d.K = n; d.stride = stride;
     d.max_d2 = max_d2; d.thr = thr;
     d.accepted = h->accepted.p; d.pa = h->pa.p; d.nrm = h->nrm.p; d.st = h->st.p;
     d.rank = h->ctx->rank; d.world = h->ctx->world;
@@ -455,7 +578,8 @@ static int upload_scan(lvb_icp* h, const void* scan, int n, int stride, const do
         LVB_TRY(h->q_start.ensure((size_t)nc + 1)); LVB_TRY(h->q_sums.ensure(nb)); LVB_TRY(h->q_total.ensure(1));
         LVB_CUDA(cudaMemsetAsync(h->q_counts.p, 0, (size_t)nc * sizeof(int), s));
         LVB_CUDA(cudaMemsetAsync(h->q_fill.p, 0, (size_t)nc * sizeof(int), s));
-        ILAUNCH(h, icp_query_key_kernel, (n + 255) / 256, 256, d, shift, cgx, cgy, cgz, h->q_key.p, h->q_counts.p);
+        if (tf_dev) ILAUNCH(h, icp_query_key_dev_tf_kernel, (n + 255) / 256, 256, d, tf_dev, shift, cgx, cgy, cgz, h->q_key.p, h->q_counts.p);
+        else ILAUNCH(h, icp_query_key_kernel, (n + 255) / 256, 256, d, shift, cgx, cgy, cgz, h->q_key.p, h->q_counts.p);
         ILAUNCH(h, scan_block_kernel, nb, 1024, h->q_counts.p, h->q_start.p, nc, h->q_sums.p);
         ILAUNCH(h, scan_sums_kernel, 1, 1024, h->q_sums.p, nb, h->q_total.p);
         ILAUNCH(h, scan_add_kernel, nb, 1024, h->q_start.p, nc, h->q_sums.p, h->q_start.p + nc, h->q_total.p);
@@ -463,6 +587,15 @@ static int upload_scan(lvb_icp* h, const void* scan, int n, int stride, const do
         d.order = h->q_order.p;
     }
     return LVB_OK;
+}
+
+static int upload_scan(lvb_icp* h, const void* scan, int n, int stride, const double* frame_pose, float max_d2, double thr, IcpDev& d) {
+    if (!h->have_map) { set_error("set_map first"); return LVB_ERR_STATE; }
+    if (n < 0 || stride < 12 || (stride & 3) || (n && !scan)) { set_error("bad scan arguments"); return LVB_ERR_INVALID; }
+    LVB_TRY(h->scan_raw.upload((const unsigned char*)scan, (size_t)n * stride, h->ctx->stream));
+    h->kf_arena.reset();
+    for (int i = 0; i < 7; ++i) d.tf[i] = (float)frame_pose[i];
+    return bind_scan(h, h->scan_raw.p, n, stride, nullptr, max_d2, thr, d);
 }
 
 extern "C" {
@@ -551,7 +684,7 @@ int lvb_icp_map_append(lvb_icp* h, long long key, const void* robot_points, int 
         src = up.p;
     } else {      // the scan the last scan_to_map / knn3 / eval call uploaded: Mapping::Optimize followed by ToWorld of the same frame
         if (h->scan_n <= 0) { set_error("lvb_icp_map_append: no scan on the device"); return LVB_ERR_STATE; }
-        n = h->scan_n; stride = h->scan_stride; src = h->scan_raw.p;
+        n = h->scan_n; stride = h->scan_stride; src = h->scan_dev;
     }
     for (auto& sg : h->segments) if (sg.key == key) { set_error("lvb_icp_map_append: key %lld exists", key); return LVB_ERR_INVALID; }
     lvb_icp::Segment sg; sg.key = key; sg.n = n; sg.pts = new DevBuf<float4>();
@@ -671,6 +804,15 @@ static int init_state(lvb_icp* h, int mode, const double* map_pose, const double
     return LVB_OK;
 }
 
+static void fill_summary(const IcpState& hs, double prior_weight, double seconds, lvb_solve_summary* summary) {
+    const int nb = hs.lm.n_accepted + (prior_weight >= 0 ? 1 : 0);
+    summary->initial_cost = hs.lm.initial_cost; summary->final_cost = hs.lm.x_cost;
+    summary->num_iterations = hs.lm.iter; summary->num_successful_steps = hs.lm.num_successful;
+    summary->termination_type = hs.lm.termination; summary->num_residual_blocks = nb; summary->num_residual_blocks_reduced = nb;
+    summary->final_radius = hs.lm.radius;
+    summary->total_time_in_seconds = seconds;
+}
+
 int lvb_icp_eval(lvb_icp* h, int mode, const void* scan, int n, int stride, const double frame_pose[7], const double map_pose[7],
                  const double rpyxyz[6], double weight, double dist_thr, uint8_t* accepted, double* r, double* J) {
     if (mode < 0 || mode > 1) { set_error("bad mode"); return LVB_ERR_INVALID; }
@@ -731,13 +873,112 @@ int lvb_icp_scan_to_map(lvb_icp* h, int mode, const void* scan, int n, int strid
     }
     const int fr[2][3] = {{1, 2, 5}, {0, 3, 4}};
     for (int k = 0; k < 3; ++k) rpyxyz[fr[mode][k]] = hs.x[k];
+    if (summary) fill_summary(hs, prior_weight, std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count(), summary);
+    return LVB_OK;
+}
+
+// Mapping::Optimize for one keyframe (mapping.cpp:147-185, after BuildMapFrame): se32rpyxyz, ScanToMapWithGround + Solve, the pose
+// hand-off, ScanToMapWithSegmented + Solve, ToWorld.  Every step is enqueued on the context's stream without a host decision in
+// between: the LM passes run max_num_iterations + 1 times unconditionally (the kernels return at once after the solver stopped), the
+// pose kernels write the query transform the next association reads, and the host synchronises once, at the end, to read the two
+// solver states and the pose back in one copy.
+int lvb_icp_map_optimize_keyframe(lvb_icp* ground, lvb_icp* surf, const double map_pose[7], long long key,
+                                  const void* ground_pts, int n_ground, const void* surf_pts, int n_surf, int stride,
+                                  const lvb_map_optimize_params* p, double pose[7], double rpyxyz[6], lvb_solve_summary summary[2]) {
+    lvb_icp* hs[2] = {ground, surf};
+    const void* pts[2] = {ground_pts, surf_pts};
+    const int ns[2] = {n_ground, n_surf};
+    if ((!ground && !surf) || ground == surf || !map_pose || !p || !pose || !rpyxyz) { set_error("null argument"); return LVB_ERR_INVALID; }
+    lvb_icp* h0 = ground ? ground : surf;
+    lvb_ctx* ctx = h0->ctx;
+    if (ground && surf && ground->ctx != surf->ctx) { set_error("lvb_icp_map_optimize_keyframe: the two handles belong to different contexts"); return LVB_ERR_INVALID; }
+    if (ctx->world > 1) { set_error("lvb_icp_map_optimize_keyframe: sharded contexts register through lvb_icp_scan_to_map"); return LVB_ERR_UNSUPPORTED; }
+    const lvb_solve_options& opt = p->options;
+    if (opt.max_solver_time_in_seconds < 1e8) { set_error("lvb_icp_map_optimize_keyframe: no time limit (Mapping::Optimize sets none)"); return LVB_ERR_INVALID; }
+    if (opt.max_num_iterations < 0 || stride < 12 || (stride & 3)) { set_error("bad arguments"); return LVB_ERR_INVALID; }
+    for (int m = 0; m < 2; ++m) {
+        lvb_icp* h = hs[m];
+        if (!h) continue;
+        if (!h->have_map) { set_error("lvb_icp_map_optimize_keyframe: build the map frame first"); return LVB_ERR_STATE; }
+        if (ns[m] < 0 || (ns[m] && !pts[m])) { set_error("bad scan arguments"); return LVB_ERR_INVALID; }
+        if ((double)h->cell_size * h->cell_size * (1.0 + 1e-6) < p->dist_thr[m]) {
+            set_error("dist_thr %.6g exceeds the map's cell_size^2 %.6g", p->dist_thr[m], (double)h->cell_size * h->cell_size); return LVB_ERR_INVALID; }
+    }
+    LVB_CUDA(cudaSetDevice(ctx->device)); lvb::g_alloc_stream = ctx->stream;
+    const auto t0 = std::chrono::steady_clock::now();
+    cudaStream_t s = ctx->stream;
+    lvb::timing_mark(s, "begin");
+    // one upload: [KfBlock | ground scan | surf scan], assembled in the pinned staging area
+    size_t off[2], bytes[2], total = (sizeof(KfBlock) + 255) & ~(size_t)255;
+    for (int m = 0; m < 2; ++m) {
+        bytes[m] = hs[m] ? (size_t)ns[m] * stride : 0;
+        off[m] = total; total = (total + bytes[m] + 255) & ~(size_t)255;
+    }
+    LVB_TRY(lvb::stage_wait(ctx));
+    LVB_TRY(lvb::stage_grow(ctx, total, 0));
+    KfBlock* hb = reinterpret_cast<KfBlock*>(ctx->stage_h);
+    memset(hb, 0, sizeof(KfBlock));
+    memcpy(hb->map_pose, map_pose, sizeof(hb->map_pose)); memcpy(hb->pose, pose, sizeof(hb->pose));
+    for (int m = 0; m < 2; ++m) if (bytes[m]) memcpy(ctx->stage_h + off[m], pts[m], bytes[m]);
+    auto arena = std::make_shared<DevBuf<unsigned char>>();
+    LVB_TRY(arena->ensure(total));
+    LVB_CUDA(cudaMemcpyAsync(arena->p, ctx->stage_h, total, cudaMemcpyHostToDevice, s));
+    LVB_TRY(lvb::stage_mark_busy(ctx, s));
+    KfBlock* blk = reinterpret_cast<KfBlock*>(arena->p);
+
+    KfSeed seed;
+    seed.o = opt; seed.prior_w = p->prior_weight;
+    for (int m = 0; m < 2; ++m) { seed.weight[m] = p->weight[m]; seed.huber_a[m] = p->huber_a[m]; }
+    const int first = ground ? 0 : 1;
+    ILAUNCH(h0, icp_kf_pose_kernel, 1, 1, blk, -1, first, seed);                   // rpyxyz from the incoming pose (mapping.cpp:154)
+    for (int m = first; m < 2 && hs[m]; ++m) {
+        lvb_icp* h = hs[m];
+        IcpDev d;
+        LVB_TRY(bind_scan(h, arena->p + off[m], ns[m], stride, blk->tf, h->cell_size * h->cell_size, p->dist_thr[m], d));
+        h->kf_arena = arena;
+        d.st = &blk->st[m];
+        ILAUNCH(h, icp_associate_dev_tf_kernel, inblk(ns[m], ITPB), ITPB, d, blk->tf);
+        const int lin_blocks = std::max(1, std::min(inblk(ns[m], ITPB), 4 * ctx->sm_count));
+        for (int pass = 0; pass <= opt.max_num_iterations; ++pass) {
+            ILAUNCH(h, icp_linearize_kernel<0>, lin_blocks, ITPB, d);
+            ILAUNCH(h, icp_solve_kernel, 1, 1, d.st);
+            ILAUNCH(h, icp_linearize_kernel<1>, lin_blocks, ITPB, d);
+            ILAUNCH(h, icp_post_kernel, 1, 1, d.st);
+        }
+        // pose = map_pose * rpyxyz2se3(rpyxyz) (:165, :177); after the ground solve it also seeds the surf registration
+        ILAUNCH(h, icp_kf_pose_kernel, 1, 1, blk, m, m == 0 && surf ? 1 : -1, seed);
+    }
+    // ToWorld (mapping.cpp:205-220): the robot-frame clouds, transformed by pose.cast<float>(), replace whatever `key` held
+    lvb_icp::Segment fresh[2];
+    for (int m = 0; m < 2; ++m) {
+        fresh[m].pts = nullptr;
+        if (!hs[m]) continue;
+        fresh[m].key = key; fresh[m].n = ns[m]; fresh[m].pts = new DevBuf<float4>();
+        int rc = fresh[m].pts->ensure(std::max(1, ns[m]));
+        if (rc != LVB_OK) { delete fresh[0].pts; delete fresh[1].pts; return rc; }
+        ILAUNCH(hs[m], icp_to_world_kernel, inblk(ns[m], 256), 256, arena->p + off[m], fresh[m].pts->p, ns[m], stride, blk->tf);
+    }
+    int rc = icheck("map_optimize_keyframe");
+    if (rc != LVB_OK) { delete fresh[0].pts; delete fresh[1].pts; return rc; }
+    for (int m = 0; m < 2; ++m) {
+        if (!hs[m]) continue;
+        auto& segs = hs[m]->segments;
+        bool replaced = false;
+        for (auto& sg : segs) if (sg.key == key) { delete sg.pts; sg = fresh[m]; replaced = true; }
+        if (!replaced) segs.push_back(fresh[m]);
+    }
+    // the one read-back: both solver states, rpyxyz and the pose
+    LVB_CUDA(cudaMemcpyAsync(ctx->stage_h, blk, sizeof(KfBlock), cudaMemcpyDeviceToHost, s));
+    LVB_CUDA(cudaStreamSynchronize(s));
+    ctx->stage_busy = false;
+    const double el = std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
+    memcpy(pose, hb->pose, sizeof(hb->pose)); memcpy(rpyxyz, hb->rpyxyz, sizeof(hb->rpyxyz));
     if (summary) {
-        const int nb = hs.lm.n_accepted + (prior_weight >= 0 ? 1 : 0);
-        summary->initial_cost = hs.lm.initial_cost; summary->final_cost = hs.lm.x_cost;
-        summary->num_iterations = hs.lm.iter; summary->num_successful_steps = hs.lm.num_successful;
-        summary->termination_type = hs.lm.termination; summary->num_residual_blocks = nb; summary->num_residual_blocks_reduced = nb;
-        summary->final_radius = hs.lm.radius;
-        summary->total_time_in_seconds = std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
+        for (int m = 0; m < 2; ++m) {
+            if (hs[m]) { fill_summary(hb->st[m], p->prior_weight, el, &summary[m]); continue; }
+            memset(&summary[m], 0, sizeof(summary[m]));
+            summary[m].termination_type = -1;          // registration skipped (mapping.cpp:155,167: empty map cloud)
+        }
     }
     return LVB_OK;
 }

@@ -66,6 +66,13 @@ int comm_allreduce_max_i32(lvb_ctx* ctx, int* buf, size_t count);
 extern bool g_timing;
 void timing_mark(cudaStream_t s, const char* name);
 int lidar_segment_ground_device(lvb_ctx* ctx, const float4* in, int n, double thr, float4* out, int* n_out);   // lidar.cu
+// The context's pinned staging area (lvb_ctx::stage_h), used by ba.cu (Stager) and icp.cu (lvb_icp_map_optimize_keyframe):
+//   stage_wait        wait until the last copy that read it has run (then it may be written)
+//   stage_grow        at least `need` bytes, the first `keep` bytes carried over (grows to max(2 x capacity, need, 4 MB))
+//   stage_mark_busy   a copy reading it has just been enqueued on `s`
+int stage_wait(lvb_ctx* ctx);
+int stage_grow(lvb_ctx* ctx, size_t need, size_t keep);
+int stage_mark_busy(lvb_ctx* ctx, cudaStream_t s);
 int comm_check(lvb_ctx* ctx);                                          // LVB_ERR_COMM when an in-kernel exchange timed out
 int comm_max_seconds(lvb_ctx* ctx, double* seconds);                   // collective: max over the ranks (no-op when world == 1)
 

@@ -445,6 +445,21 @@ def relative_rpyxyz(map_pose, frame_pose):
     return np.array([yaw, pitch, roll, t[0], t[1], t[2]])
 
 
+def rpyxyz2se3(e):
+    """rpyxyz2se3 (utility.cpp:35-40): RPYToEigenQuaternion (ceres/base.hpp:110-132), normalised as Sophus stores it."""
+    cz, sz = np.cos(e[0] / 2), np.sin(e[0] / 2)
+    cy, sy = np.cos(e[1] / 2), np.sin(e[1] / 2)
+    cx, sx = np.cos(e[2] / 2), np.sin(e[2] / 2)
+    q = np.array([cz * cy * sx - sz * sy * cx, cz * sy * cx + sz * cy * sx, sz * cy * cx - cz * sy * sx, cz * cy * cx + sz * sy * sx])
+    return np.concatenate([q / np.linalg.norm(q), e[3:6]])
+
+
+def se3_mul(a, b):
+    """Sophus SE3 product a * b of two poses [qx qy qz qw tx ty tz]."""
+    q = quat_mul(a[:4], b[:4])
+    return np.concatenate([q / np.linalg.norm(q), se3_apply(a, b[4:])])
+
+
 def make_lidar_scan(seed=SEED, num_scans=64, horizon_scan=1800, ang_res_y=0.427, ang_bottom=24.9, sensor_height=1.73,
                     sigma=0.01, dropout=0.02, n_boxes=14):
     """One revolution of a KITTI-like 64-beam spinning lidar (kitti.yaml:35-42) in the sensor frame (z up).
