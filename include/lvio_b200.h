@@ -109,6 +109,7 @@ LVB_API int lvb_ctx_create(int device, void* cuda_stream, lvb_ctx** out);
 LVB_API void lvb_ctx_destroy(lvb_ctx* ctx);
 LVB_API const char* lvb_last_error(void);            /* thread-local text of the last failure */
 LVB_API long long lvb_launch_count(lvb_ctx* ctx);    /* kernels launched through this context so far */
+LVB_API long long lvb_sync_count(lvb_ctx* ctx);      /* host synchronisations the library has made on this context's stream so far */
 LVB_API int lvb_ctx_synchronize(lvb_ctx* ctx);
 
 /* Multi-GPU (SURVEY 8e): one process per GPU; the id is produced on rank 0 and shipped to
@@ -267,6 +268,30 @@ LVB_API int lvb_icp_map_optimize_keyframe(lvb_icp* ground, lvb_icp* surf, const 
                                           const void* ground_pts, int n_ground, const void* surf_pts, int n_surf, int stride_bytes,
                                           const lvb_map_optimize_params* p, double pose[7] /* in: frame->pose, out: optimised */,
                                           double rpyxyz[6] /* out */, lvb_solve_summary summary[2]);
+/* Mapping::BuildMapFrame + the body of Mapping::Optimize's loop for one keyframe (mapping.cpp:114-137, 147-185): the two
+ * lvb_icp_map_build calls and lvb_icp_map_optimize_keyframe in one call, with one host synchronisation.
+ *   keys / n_keys  the map frame's keyframes in merge order, as for lvb_icp_map_build, resident on both handles; `key` may not be one
+ *                  of them.  n_keys == 0 is the first lidar keyframe (BuildMapFrame returns early, :118-119): nothing is registered
+ *                  and both clouds are stored at the incoming pose.
+ *   cell_size[2], ground_threshold  what the two lvb_icp_map_build calls take: SegmentGround (plane RANSAC, ground_threshold > 0) on
+ *                  the merged cloud of handle `ground`, none on `surf`.
+ *   Both handles are required: ToWorld stores both clouds under `key` (:185), replacing what `key` held.  A side is not registered
+ *   -- its summary is zero with termination_type = -1 -- when its merged cloud is empty (:155,167) or SegmentGround keeps no point;
+ *   its cloud is still stored, with the pose the other registration produced, and its previous map frame stays.  The registrations,
+ *   weights, gates and pose hand-off are lvb_icp_map_optimize_keyframe's.  rpyxyz = se32rpyxyz(map_pose^-1 * pose) of the incoming
+ *   pose, then updated by each registration that ran.  n_map_points (may be NULL): each map frame's size (0 = not built).
+ * Afterwards each handle is in the state lvb_icp_map_build + lvb_icp_map_optimize_keyframe leave it in (knn3, scan_to_map,
+ * map_download, map_append(NULL) work on it).  The map frame's voxel grid is decided on the device; the host sizes its buffers from
+ * the bounding boxes of the resident clouds, recorded when this call stores a cloud.  A resident cloud stored by another entry point
+ * has none: the first call that merges it computes it, at the cost of one more host synchronisation, and keeps it.
+ * Errors as lvb_icp_map_optimize_keyframe, plus LVB_ERR_INVALID for an unknown key or `key` among `keys`.  Failures found on the
+ * device -- a map frame with no finite bounding box (LVB_ERR_INVALID), a grid above 2^26 voxels at the coarsest ring
+ * (LVB_ERR_UNSUPPORTED) -- are reported after the synchronisation and leave every resident cloud and map frame as they were. */
+LVB_API int lvb_icp_map_build_optimize_keyframe(lvb_icp* ground, lvb_icp* surf, const long long* keys, int n_keys,
+                                                const float cell_size[2], double ground_threshold, const double map_pose[7], long long key,
+                                                const void* ground_pts, int n_ground, const void* surf_pts, int n_surf, int stride_bytes,
+                                                const lvb_map_optimize_params* p, double pose[7] /* in: frame->pose, out: optimised */,
+                                                double rpyxyz[6] /* out */, lvb_solve_summary summary[2], int n_map_points[2]);
 
 /* ---- lidar feature pipeline, the producer of the scan-to-map inputs (SURVEY 8(f).2).
  * Stands behind FeatureAssociation::Process (association.cpp:88-268: Preprocess, AdjustDistortion, CalculateSmoothness,

@@ -143,6 +143,35 @@ public:
         return true;
     }
 
+    // Mapping::BuildMapFrame + the same body of Mapping::Optimize's loop (mapping.cpp:114-185 without PoseGraph::ForwardUpdate) in ONE
+    // device call with one host synchronisation (lvb_icp_map_build_optimize_keyframe): the map frame of `keys` (in merge order; none
+    // for the first lidar keyframe, :118-119) is merged, SegmentGround'ed (ground_ransac_threshold > 0) and hashed with the cell sizes
+    // BuildMapFrame uses, each side with a non-empty map frame is registered, frame->pose is updated in place and both robot-frame
+    // clouds are stored under `key`.  Afterwards the map frames it built are the resident ones, as after BuildMapFrame.
+    // summary: 2 entries (ground, surf) or NULL; a side that was not registered has termination_type = -1.  false: the call failed
+    // (lvb_last_error()).
+    template <class FramePtr>
+    bool OptimizeKeyframe(FramePtr frame, const long long* keys, int n_keys, const double* map_pose7, long long key,
+                          double ground_ransac_threshold, lvb_solve_summary* summary = nullptr) {
+        Handles& h = handles_of_thread()[this];
+        if (!ensure_handles(h)) return false;
+        const auto& g = frame->feature_lidar->points_ground;
+        const auto& s = frame->feature_lidar->points_surf;
+        const int stride = (int)sizeof(assoc_detail::cloud_data(g, 0)[0]);
+        const lvb_map_optimize_params p = MapOptimizeParams(frame);
+        const float cells[2] = {cell_of(resolution_ * resolution_ * 100), cell_of(resolution_ * resolution_ * 25)};
+        lvb_solve_summary sums[2];
+        double rpyxyz[6];
+        int n_map[2];
+        if (lvb_icp_map_build_optimize_keyframe(h.ground, h.surf, keys, n_keys, cells, ground_ransac_threshold, map_pose7, key,
+                                                assoc_detail::cloud_data(g, 0), (int)g.size(), assoc_detail::cloud_data(s, 0), (int)s.size(), stride,
+                                                &p, frame->pose.data(), rpyxyz, summary ? summary : sums, n_map) != LVB_OK)
+            return false;
+        h.ground_map = n_map[0] > 0; h.surf_map = n_map[1] > 0;
+        h.resident = h.ground_map && h.surf_map;
+        return true;
+    }
+
 private:
     static float cell_of(double thr) { return std::nextafter((float)std::sqrt(thr), 1e30f) * 1.0001f; }
     template <class FramePtr, class Cloud, class Problem>

@@ -134,6 +134,10 @@ _LVB_ONLY = {
     "icp_map_download": (C.c_int, [VP, c_float_p, C.c_int, c_int_p]),
     "icp_map_optimize_keyframe": (C.c_int, [VP, VP, c_double_p, C.c_longlong, VP, C.c_int, VP, C.c_int, C.c_int,
                                             C.POINTER(MapOptimizeParams), c_double_p, c_double_p, C.POINTER(SolveSummary)]),
+    "icp_map_build_optimize_keyframe": (C.c_int, [VP, VP, C.POINTER(C.c_longlong), C.c_int, c_float_p, C.c_double, c_double_p, C.c_longlong,
+                                                  VP, C.c_int, VP, C.c_int, C.c_int, C.POINTER(MapOptimizeParams), c_double_p, c_double_p,
+                                                  C.POINTER(SolveSummary), c_int_p]),
+    "sync_count": (C.c_longlong, [VP]),
     "debug_timing": (C.c_int, [C.c_int]),
     "debug_cholesky_clocks": (C.c_int, [C.POINTER(C.c_longlong), C.c_int]),
     "debug_timing_report": (C.c_int, [C.c_char_p, C.c_int]),

@@ -59,6 +59,10 @@ class Context:
     def launch_count(self):
         return int(self.api.launch_count(self.h))
 
+    def sync_count(self):
+        """Host synchronisations the CUDA library has made on this context's stream so far."""
+        return int(self.api.sync_count(self.h))
+
     def synchronize(self):
         self.api.check(self.api.ctx_synchronize(self.h), "ctx_synchronize")
 
@@ -343,16 +347,10 @@ class FeatureAssociation:
         return e, s
 
 
-def optimize_keyframe(ground, surf, key, map_pose, pose, ground_points, surf_points, weight, prior_weight, huber_a, dist_thr,
-                      options=None, **kw):
-    """Mapping::Optimize for one keyframe (mapping.cpp:147-185) in one device call (CUDA library only): both registrations against the
-    map frames that map_build made on `ground` / `surf` (FeatureAssociation handles of one context; None skips that registration),
-    the pose hand-off between them, and ToWorld of the two robot-frame clouds under `key`.  weight, huber_a and dist_thr are
-    (ground, surf) pairs as ScanToMapWithGround / ScanToMapWithSegmented derive them.  Returns (pose, rpyxyz, (ground summary,
-    surf summary)); a skipped registration's summary has termination_type -1.  Keyword arguments set solver options, on top of
-    `options` when it is given."""
+def _keyframe_args(fn, ground, surf, ground_points, surf_points, weight, prior_weight, huber_a, dist_thr, options, kw):
+    """The clouds, their common stride and the lvb_map_optimize_params of optimize_keyframe / build_and_optimize_keyframe."""
     if ground is None and surf is None:
-        raise ValueError("optimize_keyframe: at least one of ground / surf is needed")
+        raise ValueError("%s: at least one of ground / surf is needed" % fn)
     api = (ground or surf).api
     pts, n, strides = [None, None], [0, 0], set()
     for m, (fa, cloud) in enumerate(((ground, ground_points), (surf, surf_points))):
@@ -360,7 +358,7 @@ def optimize_keyframe(ground, surf, key, map_pose, pose, ground_points, surf_poi
             pts[m], n[m], stride = FeatureAssociation._cloud(cloud)
             strides.add(stride)
     if len(strides) != 1:
-        raise ValueError("optimize_keyframe: the ground and surf clouds must have the same record stride, got %s" % sorted(strides))
+        raise ValueError("%s: the ground and surf clouds must have the same record stride, got %s" % (fn, sorted(strides)))
     prm = _capi.MapOptimizeParams()
     for k in range(2):
         prm.weight[k], prm.huber_a[k], prm.dist_thr[k] = float(weight[k]), float(huber_a[k]), float(dist_thr[k])
@@ -370,14 +368,51 @@ def optimize_keyframe(ground, surf, key, map_pose, pose, ground_points, surf_poi
     prm.options = options                # a copy: kw below does not touch the caller's structure
     for k, v in kw.items():
         setattr(prm.options, k, v)
+    vp = [None if a is None else a.ctypes.data_as(C.c_void_p) for a in pts]
+    return api, pts, vp, n, strides.pop(), prm
+
+
+def optimize_keyframe(ground, surf, key, map_pose, pose, ground_points, surf_points, weight, prior_weight, huber_a, dist_thr,
+                      options=None, **kw):
+    """Mapping::Optimize for one keyframe (mapping.cpp:147-185) in one device call (CUDA library only): both registrations against the
+    map frames that map_build made on `ground` / `surf` (FeatureAssociation handles of one context; None skips that registration),
+    the pose hand-off between them, and ToWorld of the two robot-frame clouds under `key`.  weight, huber_a and dist_thr are
+    (ground, surf) pairs as ScanToMapWithGround / ScanToMapWithSegmented derive them.  Returns (pose, rpyxyz, (ground summary,
+    surf summary)); a skipped registration's summary has termination_type -1.  Keyword arguments set solver options, on top of
+    `options` when it is given."""
+    api, pts, vp, n, stride, prm = _keyframe_args("optimize_keyframe", ground, surf, ground_points, surf_points, weight, prior_weight,
+                                                  huber_a, dist_thr, options, kw)
     mp = _f64(map_pose).reshape(7)
     p = _f64(pose).reshape(7).copy()
     e = np.zeros(6)
     s = (SolveSummary * 2)()
-    vp = [None if a is None else a.ctypes.data_as(C.c_void_p) for a in pts]
     api.check(api.icp_map_optimize_keyframe(ground.h if ground else None, surf.h if surf else None, _dp(mp), int(key), vp[0], n[0], vp[1], n[1],
-                                            strides.pop(), C.byref(prm), _dp(p), _dp(e), s), "icp_map_optimize_keyframe")
+                                            stride, C.byref(prm), _dp(p), _dp(e), s), "icp_map_optimize_keyframe")
     return p, e, (s[0], s[1])
+
+
+def build_and_optimize_keyframe(ground, surf, keys, cell_sizes, ground_threshold, key, map_pose, pose, ground_points, surf_points,
+                                weight, prior_weight, huber_a, dist_thr, options=None, **kw):
+    """Mapping::BuildMapFrame + Mapping::Optimize for one keyframe (mapping.cpp:114-137, 147-185) in one device call with one host
+    synchronisation (CUDA library only): map_build of `keys` on both handles (cell_sizes = (ground, surf); SegmentGround on the
+    ground side when ground_threshold > 0), then optimize_keyframe.  Both handles are required; an empty `keys` is the first lidar
+    keyframe (nothing registered, both clouds stored at `pose`).  A side whose map frame comes out empty is not registered
+    (termination_type -1).  Returns (pose, rpyxyz, (ground summary, surf summary), (ground map points, surf map points))."""
+    if ground is None or surf is None:
+        raise ValueError("build_and_optimize_keyframe: both the ground and the surf handle are needed")
+    api, pts, vp, n, stride, prm = _keyframe_args("build_and_optimize_keyframe", ground, surf, ground_points, surf_points, weight,
+                                                  prior_weight, huber_a, dist_thr, options, kw)
+    k = (C.c_longlong * max(1, len(keys)))(*[int(x) for x in keys])
+    cs = np.asarray(cell_sizes, dtype=np.float32).reshape(2).copy()
+    mp = _f64(map_pose).reshape(7)
+    p = _f64(pose).reshape(7).copy()
+    e = np.zeros(6)
+    s = (SolveSummary * 2)()
+    nm = np.zeros(2, dtype=np.int32)
+    api.check(api.icp_map_build_optimize_keyframe(ground.h, surf.h, k, len(keys), cs.ctypes.data_as(_capi.c_float_p), float(ground_threshold),
+                                                  _dp(mp), int(key), vp[0], n[0], vp[1], n[1], stride, C.byref(prm), _dp(p), _dp(e), s,
+                                                  nm.ctypes.data_as(_capi.c_int_p)), "icp_map_build_optimize_keyframe")
+    return p, e, (s[0], s[1]), (int(nm[0]), int(nm[1]))
 
 
 def _fp(a):

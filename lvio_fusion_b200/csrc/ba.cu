@@ -1334,7 +1334,7 @@ static int allreduce_host_i32(lvb_ctx* ctx, std::vector<int>& v, int (*op)(lvb_c
     LVB_TRY(tmp.upload(v.data(), v.size(), s));
     LVB_TRY(op(ctx, tmp.p, v.size()));
     LVB_CUDA(cudaMemcpyAsync(v.data(), tmp.p, v.size() * sizeof(int), cudaMemcpyDeviceToHost, s));
-    LVB_CUDA(cudaStreamSynchronize(s));
+    LVB_TRY(lvb::host_sync(ctx, s));
     return LVB_OK;
 }
 
@@ -1507,7 +1507,7 @@ int lvb_ba_update_params(lvb_ba* ba, const double* P, const double* V, const dou
     if (P) { ba->h_poses.assign(P, P + ba->h_poses.size()); LVB_TRY(ba->poses.upload(P, ba->h_poses.size(), s)); }
     if (V) { ba->h_vec3.assign(V, V + ba->h_vec3.size()); LVB_TRY(ba->vec3.upload(V, ba->h_vec3.size(), s)); }
     if (R) { ba->h_rho.assign(R, R + ba->h_rho.size()); LVB_TRY(ba->rho.upload(R, ba->h_rho.size(), s)); }
-    LVB_CUDA(cudaStreamSynchronize(s));
+    LVB_TRY(lvb::host_sync(ba->ctx, s));
     return LVB_OK;
 }
 
@@ -1515,7 +1515,7 @@ static int check_imu_status(lvb_ba* ba) {
     if (ba->imu_checked || ba->plan.nd[3] == 0) { ba->imu_checked = true; return LVB_OK; }
     std::vector<int> status(ba->plan.nd[3]);
     LVB_TRY(ba->imu_status.download(status.data(), status.size(), ba->ctx->stream));
-    LVB_CUDA(cudaStreamSynchronize(ba->ctx->stream));
+    LVB_TRY(lvb::host_sync(ba->ctx, ba->ctx->stream));
     for (size_t f = 0; f < status.size(); ++f) if (status[f]) { set_error("ImuError %d: covariance is singular or not finite (code %d)", (int)f, status[f]); return LVB_ERR_NUMERIC; }
     ba->imu_checked = true;
     return LVB_OK;
@@ -1564,14 +1564,14 @@ int lvb_ba_eval(lvb_ba* ba, int kind, double* r, double* J) {
     if (identity) {
         if (r) LVB_TRY(ba->eval_r.download(r, nd * rd, s));
         if (J) LVB_TRY(ba->eval_J.download(J, nd * jd, s));
-        LVB_CUDA(cudaStreamSynchronize(s));
+        LVB_TRY(lvb::host_sync(ba->ctx, s));
         return LVB_OK;
     }
     // the device layout is sorted / padded: hand the rows back in the caller's block order
     std::vector<double> hr(r ? nd * rd : 0), hJ(J ? nd * jd : 0);
     if (r) LVB_TRY(ba->eval_r.download(hr.data(), nd * rd, s));
     if (J) LVB_TRY(ba->eval_J.download(hJ.data(), nd * jd, s));
-    LVB_CUDA(cudaStreamSynchronize(s));
+    LVB_TRY(lvb::host_sync(ba->ctx, s));
     for (size_t i = 0; i < nd; ++i) {
         if (ord[i] < 0) continue;
         if (r) memcpy(r + (size_t)ord[i] * rd, hr.data() + i * rd, rd * sizeof(double));
@@ -1714,7 +1714,7 @@ int lvb_ba_reduced_system(lvb_ba* ba, double radius, double* S, double* b, doubl
     LVB_CUDA(cudaMemcpyAsync(hS.data(), ba->dev.S, hS.size() * sizeof(double), cudaMemcpyDeviceToHost, s));
     if (b) LVB_CUDA(cudaMemcpyAsync(b, ba->dev.rhs, n * sizeof(double), cudaMemcpyDeviceToHost, s));
     LVB_CUDA(cudaMemcpyAsync(&h, ba->st.p, sizeof(h), cudaMemcpyDeviceToHost, s));
-    LVB_CUDA(cudaStreamSynchronize(s));
+    LVB_TRY(lvb::host_sync(ba->ctx, s));
     // hand the system back in the caller-visible order (all poses, then all vec3 blocks)
     const std::vector<int>& cn = ba->plan.canon;
     if (S) for (int i = 0; i < n; ++i) for (int j = 0; j < n; ++j) S[(size_t)cn[i] * n + cn[j]] = (j <= i) ? at(i, j) : at(j, i);
@@ -1804,7 +1804,7 @@ int lvb_ba_solve(lvb_ba* ba, const lvb_solve_options* options, lvb_solve_summary
         }
         pass += chunk;
         LVB_CUDA(cudaMemcpyAsync(&h, ba->st.p, sizeof(h), cudaMemcpyDeviceToHost, s));
-        LVB_CUDA(cudaStreamSynchronize(s));
+        LVB_TRY(lvb::host_sync(ba->ctx, s));
         LVB_TRY(comm_check(ba->ctx));
         PROF("launch + wait");
         if (h.done) break;             // identical on every rank: the state is a function of bitwise-identical all-reduced sums
@@ -1842,7 +1842,7 @@ static int fetch_params(lvb_ba* ba) {
     double* dst = pinned ? reinterpret_cast<double*>(c->stage_h) : ba->r_params.data();
     cudaStream_t s = c->stream;
     LVB_TRY(ba->poses.download(dst, n0, s)); LVB_TRY(ba->vec3.download(dst + n0, n1, s)); LVB_TRY(ba->rho.download(dst + n0 + n1, n2, s));
-    LVB_CUDA(cudaStreamSynchronize(s));
+    LVB_TRY(lvb::host_sync(c, s));
     if (pinned) { memcpy(ba->r_params.data(), dst, total); c->stage_busy = false; }
     ba->host_fresh = true;
     return LVB_OK;
@@ -1869,7 +1869,7 @@ int lvb_ba_reprojection_errors(lvb_ba* ba, int n, const double* ob_pw, const int
     LAUNCH(ba->ctx, ba_reproj_error_kernel, nblk(n, 128), 128, 0, ba->dev, n, d_in.p, d_idx.p, d_err.p);
     LVB_TRY(check_launch("reproj"));
     LVB_TRY(d_err.download(err, n, s));
-    LVB_CUDA(cudaStreamSynchronize(s));
+    LVB_TRY(lvb::host_sync(ba->ctx, s));
     return LVB_OK;
 }
 

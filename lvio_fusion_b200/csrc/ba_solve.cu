@@ -361,7 +361,7 @@ LVB_API int lvb_debug_band_solve(lvb_ctx* ctx, int n, int band, const double* S_
     LVB_TRY(check_launch("band solve"));
     LVB_CUDA(cudaMemcpyAsync(x, Sb.p + nS, (size_t)n * sizeof(double), cudaMemcpyDeviceToHost, s));
     LVB_CUDA(cudaMemcpyAsync(&h, st.p, sizeof(h), cudaMemcpyDeviceToHost, s));
-    LVB_CUDA(cudaStreamSynchronize(s));
+    LVB_TRY(lvb::host_sync(ctx, s));
     if (h.solve_fail) { set_error("band solve: non-positive pivot"); return LVB_ERR_NUMERIC; }
     return LVB_OK;
 }

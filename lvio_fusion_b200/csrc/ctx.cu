@@ -28,7 +28,12 @@ int cuda_fail(cudaError_t e, const char* what, const char* file, int line) {
 
 int stage_wait(lvb_ctx* ctx) {
     if (!ctx->stage_ev) LVB_CUDA(cudaEventCreateWithFlags(&ctx->stage_ev, cudaEventDisableTiming));
-    if (ctx->stage_busy) { LVB_CUDA(cudaEventSynchronize(ctx->stage_ev)); ctx->stage_busy = false; }
+    if (ctx->stage_busy) { LVB_CUDA(cudaEventSynchronize(ctx->stage_ev)); ctx->syncs++; ctx->stage_busy = false; }
+    return LVB_OK;
+}
+int host_sync(lvb_ctx* ctx, cudaStream_t s) {
+    LVB_CUDA(cudaStreamSynchronize(s));
+    ctx->syncs++;
     return LVB_OK;
 }
 int stage_grow(lvb_ctx* ctx, size_t need, size_t keep) {
@@ -125,7 +130,7 @@ static int p2p_setup(lvb_ctx* ctx) {
         const int rc = g_nccl.all_gather(d_all + hb * ctx->rank, d_all, hb, /*ncclChar*/ 0, ctx->comm, ctx->stream);
         if (rc != 0) { cudaFree(d_all); return nccl_fail(rc, "ncclAllGather"); }
     }
-    LVB_CUDA(cudaStreamSynchronize(ctx->stream));
+    LVB_TRY(host_sync(ctx, ctx->stream));
     std::vector<cudaIpcMemHandle_t> all(ctx->world);
     LVB_CUDA(cudaMemcpy(all.data(), d_all, hb * ctx->world, cudaMemcpyDeviceToHost));
     if (ok) {
@@ -139,7 +144,7 @@ static int p2p_setup(lvb_ctx* ctx) {
     LVB_CUDA(cudaMemcpy(d_ok, &ok, sizeof(int), cudaMemcpyHostToDevice));
     const int rc = g_nccl.all_reduce(d_ok, d_ok, 1, /*ncclInt32*/ 2, /*ncclMin*/ 3, ctx->comm, ctx->stream);
     if (rc != 0) { cudaFree(d_all); return nccl_fail(rc, "ncclAllReduce(p2p ok)"); }
-    LVB_CUDA(cudaStreamSynchronize(ctx->stream));
+    LVB_TRY(host_sync(ctx, ctx->stream));
     LVB_CUDA(cudaMemcpy(&ok, d_ok, sizeof(int), cudaMemcpyDeviceToHost));
     cudaFree(d_all);
     ctx->p2p_ok = ok != 0;
@@ -184,7 +189,7 @@ int comm_check(lvb_ctx* ctx) {
     if (ctx->world <= 1 || !ctx->p2p_ok || !ctx->xbuf) return LVB_OK;
     unsigned int word = 0;
     LVB_CUDA(cudaMemcpyAsync(&word, ctx->xbuf + XB_FLAGS + 8, sizeof(word), cudaMemcpyDeviceToHost, ctx->stream));
-    LVB_CUDA(cudaStreamSynchronize(ctx->stream));
+    LVB_TRY(host_sync(ctx, ctx->stream));
     if (word) {
         set_error("peer-memory all-reduce on rank %d timed out after %.1f s waiting for rank %u: the ranks issued different collective sequences "
                   "or a peer is gone; this communicator is unusable", ctx->rank, ctx->p2p_timeout_ns * 1e-9, word - 1u);
@@ -201,7 +206,7 @@ int comm_max_seconds(lvb_ctx* ctx, double* seconds) {
     LVB_CUDA(cudaMemcpyAsync(ctx->scratch_i32, &us, sizeof(int), cudaMemcpyHostToDevice, ctx->stream));
     LVB_TRY(comm_allreduce_max_i32(ctx, ctx->scratch_i32, 1));
     LVB_CUDA(cudaMemcpyAsync(&us, ctx->scratch_i32, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
-    LVB_CUDA(cudaStreamSynchronize(ctx->stream));
+    LVB_TRY(host_sync(ctx, ctx->stream));
     *seconds = us * 1e-6;
     return LVB_OK;
 }
@@ -296,10 +301,11 @@ void lvb_ctx_destroy(lvb_ctx* ctx) {
 }
 
 long long lvb_launch_count(lvb_ctx* ctx) { return ctx ? ctx->launches : 0; }
+long long lvb_sync_count(lvb_ctx* ctx) { return ctx ? ctx->syncs : 0; }
 
 int lvb_ctx_synchronize(lvb_ctx* ctx) {
     if (!ctx) return LVB_ERR_INVALID;
-    LVB_CUDA(cudaStreamSynchronize(ctx->stream));
+    LVB_TRY(host_sync(ctx, ctx->stream));
     return LVB_OK;
 }
 

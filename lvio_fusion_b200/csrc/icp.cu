@@ -66,30 +66,48 @@ struct IcpDev {
     int cbx, cby, cbz;           // its dimensions
 };
 
+// A map frame whose grid is decided on the device (lvb_icp_map_build_optimize_keyframe): what build_hash and bind_scan decide on the
+// host for the other entry points, written by icp_map_grid_kernel and read by the *_map kernels below.
+struct MapDesc {
+    Grid g;
+    int P;                       // map points (the surf merge: uploaded; the ground merge: SegmentGround's inlier count)
+    int ncell, cbx, cby, cbz, ncb;          // gx * gy * gz; coarse-block grid and its size
+    int shift, cgx, cgy, cgz, nc;           // query visiting order (bind_scan): key granularity and its grid
+    int err;                     // 0, 1: no finite bounding box, 2: more than MAX_CELLS voxels at ring 1
+    int bbox[6];                 // the cloud's bounding box (ordered ints, icp_bbox_kernel's layout), uploaded with its seed values
+};
+
 __device__ __forceinline__ float3 load_xyz(const unsigned char* base, int i, int stride) {
     const float* f = reinterpret_cast<const float*>(base + (size_t)i * stride);
     return make_float3(f[0], f[1], f[2]);
 }
 
-__global__ void icp_bbox_kernel(const unsigned char* pts, int n, int stride, int* bbox /*6: min xyz, max xyz (ordered ints)*/) {
+// warp min / max of the per-thread boxes, merged into bbox[6] (min xyz, max xyz as ordered ints) by one lane per warp
+__device__ __forceinline__ void bbox_merge(float* mn, float* mx, int* bbox) {
+    for (int a = 0; a < 3; ++a) {
+        for (int o = 16; o > 0; o >>= 1) { mn[a] = fminf(mn[a], __shfl_xor_sync(0xffffffffu, mn[a], o)); mx[a] = fmaxf(mx[a], __shfl_xor_sync(0xffffffffu, mx[a], o)); }
+        if ((threadIdx.x & 31) == 0) { atomicMin(&bbox[a], f2ord(mn[a])); atomicMax(&bbox[3 + a], f2ord(mx[a])); }
+    }
+}
+__device__ __forceinline__ void bbox_points(const unsigned char* pts, int n, int stride, int* bbox) {
     float mn[3] = {FLT_MAX, FLT_MAX, FLT_MAX}, mx[3] = {-FLT_MAX, -FLT_MAX, -FLT_MAX};
     for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
         const float3 p = load_xyz(pts, i, stride);
         mn[0] = fminf(mn[0], p.x); mn[1] = fminf(mn[1], p.y); mn[2] = fminf(mn[2], p.z);
         mx[0] = fmaxf(mx[0], p.x); mx[1] = fmaxf(mx[1], p.y); mx[2] = fmaxf(mx[2], p.z);
     }
-    for (int a = 0; a < 3; ++a) {
-        for (int o = 16; o > 0; o >>= 1) { mn[a] = fminf(mn[a], __shfl_xor_sync(0xffffffffu, mn[a], o)); mx[a] = fmaxf(mx[a], __shfl_xor_sync(0xffffffffu, mx[a], o)); }
-        if ((threadIdx.x & 31) == 0) { atomicMin(&bbox[a], f2ord(mn[a])); atomicMax(&bbox[3 + a], f2ord(mx[a])); }
-    }
+    bbox_merge(mn, mx, bbox);
 }
+__global__ void icp_bbox_kernel(const unsigned char* pts, int n, int stride, int* bbox /*6: min xyz, max xyz (ordered ints)*/) {
+    bbox_points(pts, n, stride, bbox);
+}
+// the same over the map frame of a MapDesc (its point count is known on the device only)
+__global__ void icp_bbox_map_kernel(const unsigned char* pts, int stride, MapDesc* m) { bbox_points(pts, m->P, stride, m->bbox); }
 
 __device__ __forceinline__ int cell_coord(float v, float mn, float inv_cell) { return (int)floorf((v - mn) * inv_cell); }
 __device__ __forceinline__ int clampi(int v, int lo, int hi) { return v < lo ? lo : (v > hi ? hi : v); }
 
-__global__ void icp_count_kernel(const unsigned char* pts, int n, int stride, Grid g, int* cell_of, int* counts, int* coarse, int cbx, int cby) {
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
+__device__ __forceinline__ void count_point(const unsigned char* pts, int i, int stride, const Grid& g, int* cell_of, int* counts, int* coarse, int cbx, int cby) {
     const float3 p = load_xyz(pts, i, stride);
     const int ix = clampi(cell_coord(p.x, g.minx, g.inv_cell), 0, g.gx - 1);
     const int iy = clampi(cell_coord(p.y, g.miny, g.inv_cell), 0, g.gy - 1);
@@ -99,14 +117,50 @@ __global__ void icp_count_kernel(const unsigned char* pts, int n, int stride, Gr
     atomicAdd(&counts[c], 1);
     coarse[(ix >> 2) + cbx * ((iy >> 2) + cby * (iz >> 2))] = 1;       // benign race: every writer stores 1
 }
-
-__global__ void icp_scatter_kernel(const unsigned char* pts, int n, int stride, const int* cell_of, const int* cell_start, int* fill, float4* sorted) {
+__global__ void icp_count_kernel(const unsigned char* pts, int n, int stride, Grid g, int* cell_of, int* counts, int* coarse, int cbx, int cby) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
+    count_point(pts, i, stride, g, cell_of, counts, coarse, cbx, cby);
+}
+__global__ void icp_count_map_kernel(const unsigned char* pts, int stride, const MapDesc* m, int* cell_of, int* counts, int* coarse) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= m->P) return;
+    count_point(pts, i, stride, m->g, cell_of, counts, coarse, m->cbx, m->cby);
+}
+
+__device__ __forceinline__ void scatter_point(const unsigned char* pts, int i, int stride, const int* cell_of, const int* cell_start, int* fill, float4* sorted) {
     const float3 p = load_xyz(pts, i, stride);
     const int c = cell_of[i];
     const int pos = cell_start[c] + atomicAdd(&fill[c], 1);
     sorted[pos] = make_float4(p.x, p.y, p.z, __int_as_float(i));
+}
+__global__ void icp_scatter_kernel(const unsigned char* pts, int n, int stride, const int* cell_of, const int* cell_start, int* fill, float4* sorted) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    scatter_point(pts, i, stride, cell_of, cell_start, fill, sorted);
+}
+__global__ void icp_scatter_map_kernel(const unsigned char* pts, int stride, const MapDesc* m, const int* cell_of, const int* cell_start, int* fill, float4* sorted) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= m->P) return;
+    scatter_point(pts, i, stride, cell_of, cell_start, fill, sorted);
+}
+
+// zero a[0..*n) (and b[0..*n) unless null): counters sized on the host by an upper bound, used up to the size the device decided
+__global__ void icp_zero_map_kernel(int* a, int* b, const int* n) {
+    const int cnt = *n;
+    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < cnt; i += gridDim.x * blockDim.x) { a[i] = 0; if (b) b[i] = 0; }
+}
+// the exclusive scan of lvb_cloud.cuh over the first *n entries (blocks launched for an upper bound of *n)
+__global__ void scan_block_map_kernel(const int* in, int* out, const int* n, int* block_sums) {
+    const int cnt = *n;
+    if ((int)blockIdx.x * 1024 >= cnt) return;
+    scan_block(in, out, cnt, block_sums);
+}
+__global__ void scan_sums_map_kernel(int* block_sums, const int* n, int* total_out) { scan_sums(block_sums, (*n + 1023) / 1024, total_out); }
+__global__ void scan_add_map_kernel(int* out, const int* n, const int* block_sums, const int* total) {
+    const int cnt = *n;
+    if ((int)blockIdx.x * 1024 >= cnt) return;
+    scan_add(out, cnt, block_sums, out + cnt, total);
 }
 
 // Mapping::MergeScan (mapping.cpp:193-203): world cloud = float32 SE3 transform of the robot-frame cloud; the other
@@ -124,14 +178,29 @@ __global__ void icp_transform_cloud_kernel(const unsigned char* __restrict__ in,
 }
 
 // Mapping::ToWorld (mapping.cpp:205-220) into the resident store: records of any stride -> packed (x, y, z, intensity) in the world frame
-__global__ void icp_to_world_kernel(const unsigned char* __restrict__ in, float4* __restrict__ out, int n, int stride, const float* __restrict__ tf7) {
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
+__device__ __forceinline__ float3 to_world_point(const unsigned char* __restrict__ in, float4* __restrict__ out, int i, int stride, const float* __restrict__ tf7) {
     float tf[7];
     for (int k = 0; k < 7; ++k) tf[k] = tf7[k];
     const float* src = reinterpret_cast<const float*>(in + (size_t)i * stride);
     const float3 q = transform_f32(tf, make_float3(src[0], src[1], src[2]));
     out[i] = make_float4(q.x, q.y, q.z, stride >= 16 ? src[3] : 0.0f);
+    return q;
+}
+__global__ void icp_to_world_kernel(const unsigned char* __restrict__ in, float4* __restrict__ out, int n, int stride, const float* __restrict__ tf7) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    to_world_point(in, out, i, stride, tf7);
+}
+// the same, and the bounding box of the stored cloud into bbox[6] (icp_bbox_kernel's min / max: equal to what it finds on `out`)
+__global__ void icp_to_world_bbox_kernel(const unsigned char* __restrict__ in, float4* __restrict__ out, int n, int stride, const float* __restrict__ tf7, int* bbox) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    float mn[3] = {FLT_MAX, FLT_MAX, FLT_MAX}, mx[3] = {-FLT_MAX, -FLT_MAX, -FLT_MAX};
+    if (i < n) {
+        const float3 q = to_world_point(in, out, i, stride, tf7);
+        mn[0] = fminf(mn[0], q.x); mn[1] = fminf(mn[1], q.y); mn[2] = fminf(mn[2], q.z);
+        mx[0] = fmaxf(mx[0], q.x); mx[1] = fmaxf(mx[1], q.y); mx[2] = fmaxf(mx[2], q.z);
+    }
+    bbox_merge(mn, mx, bbox);
 }
 
 struct Best3 { float d[3]; int i[3]; int p[3]; };   // d2, original index, position in the sorted array
@@ -233,6 +302,13 @@ __global__ void icp_query_key_dev_tf_kernel(IcpDev d, const float* __restrict__ 
     for (int k = 0; k < 7; ++k) tf[k] = tf7[k];
     query_key(d, tf, shift, cgx, cgy, cgz, key, counts);
 }
+// ... and with the map grid and the key granularity of a MapDesc
+__global__ void icp_query_key_map_kernel(IcpDev d, const float* __restrict__ tf7, const MapDesc* __restrict__ m, int* __restrict__ key, int* __restrict__ counts) {
+    float tf[7];
+    for (int k = 0; k < 7; ++k) tf[k] = tf7[k];
+    d.g = m->g;
+    query_key(d, tf, m->shift, m->cgx, m->cgy, m->cgz, key, counts);
+}
 __global__ void icp_query_scatter_kernel(int n, const int* __restrict__ key, const int* __restrict__ start, int* __restrict__ fill, int* __restrict__ order) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
@@ -271,6 +347,63 @@ __global__ void __launch_bounds__(ITPB) icp_associate_dev_tf_kernel(IcpDev d, co
     float tf[7];
     for (int k = 0; k < 7; ++k) tf[k] = tf7[k];
     associate_query(d, tf);
+}
+// ... and with the map frame of a MapDesc; an empty one (SegmentGround kept no point) accepts no query
+__global__ void __launch_bounds__(ITPB) icp_associate_map_kernel(IcpDev d, const float* __restrict__ tf7, const MapDesc* __restrict__ m) {
+    if (m->P == 0) {
+        const int t = blockIdx.x * ITPB + threadIdx.x;
+        if (t < d.K) d.accepted[t] = 0;
+        return;
+    }
+    float tf[7];
+    for (int k = 0; k < 7; ++k) tf[k] = tf7[k];
+    d.g = m->g; d.P = m->P; d.cbx = m->cbx; d.cby = m->cby; d.cbz = m->cbz;
+    associate_query(d, tf);
+}
+
+// build_hash's grid and bind_scan's key granularity on one thread, from the bounding box in m->bbox: the same float / double
+// operations in the same order, each rounded on its own (no contraction), so the voxels, the neighbours and the query visiting
+// order are those of the step-by-step path.  An empty or failed map frame gets a one-voxel grid and P = 0, which every *_map kernel
+// treats as "nothing to do".
+__global__ void icp_map_grid_kernel(MapDesc* m, float cell_size, int forced_shift) {
+    Grid g;
+    int P = m->P, err = 0;
+    double dx = 1, dy = 1, dz = 1;
+    g.ring = 1;
+    if (P > 0) {
+        g.minx = ord2f(m->bbox[0]); g.miny = ord2f(m->bbox[1]); g.minz = ord2f(m->bbox[2]);
+        const float mx = ord2f(m->bbox[3]), my = ord2f(m->bbox[4]), mz = ord2f(m->bbox[5]);
+        const float wx = __fsub_rn(mx, g.minx), wy = __fsub_rn(my, g.miny), wz = __fsub_rn(mz, g.minz);
+        if (!(mx >= g.minx) || !(my >= g.miny) || !(mz >= g.minz) || !isfinite(wx) || !isfinite(wy) || !isfinite(wz)) err = 1;
+        else {
+            int ring = 4;
+            for (;; ring >>= 1) {
+                g.cell = __fdiv_rn(__fmul_rn(cell_size, 1.0001f), (float)ring); g.inv_cell = __fdiv_rn(1.0f, g.cell);
+                dx = __dadd_rn(floor(__dmul_rn((double)wx, (double)g.inv_cell)), 1.0);
+                dy = __dadd_rn(floor(__dmul_rn((double)wy, (double)g.inv_cell)), 1.0);
+                dz = __dadd_rn(floor(__dmul_rn((double)wz, (double)g.inv_cell)), 1.0);
+                if (__dmul_rn(__dmul_rn(dx, dy), dz) <= (double)MAX_CELLS || ring == 1) break;
+            }
+            if (__dmul_rn(__dmul_rn(dx, dy), dz) > (double)MAX_CELLS) err = 2;
+            g.ring = ring;
+        }
+    }
+    if (P <= 0 || err) {
+        P = 0; dx = dy = dz = 1;
+        g.minx = g.miny = g.minz = 0.0f; g.cell = g.inv_cell = 1.0f; g.ring = 1;
+    }
+    g.gx = (int)dx; g.gy = (int)dy; g.gz = (int)dz;
+    m->g = g; m->P = P; m->err = err;
+    m->ncell = g.gx * g.gy * g.gz;
+    m->cbx = (g.gx + 3) >> 2; m->cby = (g.gy + 3) >> 2; m->cbz = (g.gz + 3) >> 2;
+    m->ncb = m->cbx * m->cby * m->cbz;
+    int shift = 1;
+    while (forced_shift < 0 && __dmul_rn(__dmul_rn((double)((g.gx >> shift) + 1), (double)((g.gy >> shift) + 1)), (double)((g.gz >> shift) + 1)) > 8.0e6) ++shift;
+    if (forced_shift >= 0) shift = forced_shift;
+    const int rnd = (1 << shift) - 1;
+    m->shift = shift;
+    m->cgx = (g.gx + rnd) >> shift; m->cgy = (g.gy + rnd) >> shift; m->cgz = (g.gz + rnd) >> shift;
+    m->nc = m->cgx * m->cgy * m->cgz;
 }
 
 __device__ __forceinline__ void icp_substitute(const IcpState& s, const double* x, double* e) {
@@ -481,7 +614,7 @@ __device__ void kf_rpyxyz2se3(const double* e, double* T) {
 //   from = m  : registration m is solved: its free scalars go back into rpyxyz, pose = map_pose * rpyxyz2se3(rpyxyz)  (:165, :177)
 //   then      : tf = pose.cast<float>() (association.cpp:287, mapping.cpp:195), and with seed = m the IcpState of registration m
 //               is set up from rpyxyz as lvb_icp_scan_to_map's init_state does on the host
-__global__ void icp_kf_pose_kernel(KfBlock* b, int from, int seed, KfSeed p) {
+__device__ __forceinline__ void kf_pose_update(KfBlock* b, int from) {
     if (from < 0) {
         double inv[7], rel[7];
         kf_se3_inv(b->map_pose, inv);
@@ -493,8 +626,8 @@ __global__ void icp_kf_pose_kernel(KfBlock* b, int from, int seed, KfSeed p) {
         kf_rpyxyz2se3(b->rpyxyz, rel);
         kf_se3_mul(b->map_pose, rel, b->pose);
     }
-    for (int k = 0; k < 7; ++k) b->tf[k] = __double2float_rn(b->pose[k]);
-    if (seed < 0) return;
+}
+__device__ __forceinline__ void kf_seed(KfBlock* b, int seed, const KfSeed& p) {
     IcpState& s = b->st[seed];
     memset(&s, 0, sizeof(s));
     lm_init(s.lm, p.o);
@@ -503,6 +636,22 @@ __global__ void icp_kf_pose_kernel(KfBlock* b, int from, int seed, KfSeed p) {
     for (int k = 0; k < 6; ++k) s.rpyxyz[k] = b->rpyxyz[k];
     for (int k = 0; k < 3; ++k) { s.x[k] = b->rpyxyz[c_free[seed][k]]; s.cand[k] = s.x[k]; s.prior_target[k] = s.x[k]; }
     s.prior_w = p.prior_w; s.huber_a = p.huber_a[seed]; s.weight = p.weight[seed];
+}
+__global__ void icp_kf_pose_kernel(KfBlock* b, int from, int seed, KfSeed p) {
+    kf_pose_update(b, from);
+    for (int k = 0; k < 7; ++k) b->tf[k] = __double2float_rn(b->pose[k]);
+    if (seed < 0) return;
+    kf_seed(b, seed, p);
+}
+// The same when the map frames were built in the same call (lvb_icp_map_build_optimize_keyframe): a registration whose map frame is
+// empty (maps[m].P == 0: SegmentGround kept no point) is not solved -- its LM passes return at once -- and leaves rpyxyz and the pose
+// as they were, as BuildMapFrame's failure on that side does in the step-by-step path.
+__global__ void icp_kf_pose_map_kernel(KfBlock* b, int from, int seed, KfSeed p, const MapDesc* maps) {
+    if (from < 0 || maps[from].P > 0) kf_pose_update(b, from);
+    for (int k = 0; k < 7; ++k) b->tf[k] = __double2float_rn(b->pose[k]);
+    if (seed < 0) return;
+    kf_seed(b, seed, p);
+    if (maps[seed].P == 0) b->st[seed].lm.done = 1;
 }
 
 }  // namespace
@@ -525,9 +674,14 @@ struct lvb_icp {
     DevBuf<IcpState> st;
     DevBuf<int> q_key, q_counts, q_start, q_fill, q_sums, q_total, q_order;
     // device-resident world clouds per keyframe (Mapping::pointclouds_surf / _ground, mapping.cpp:208-219) and the merged map frame
-    struct Segment { long long key; DevBuf<float4>* pts; int n; };
+    // lo / hi: the cloud's bounding box (icp_bbox_kernel's), recorded by lvb_icp_map_build_optimize_keyframe for the clouds it stores
+    // and computed by it once for the others (has_bbox false)
+    struct Segment { long long key; DevBuf<float4>* pts; int n; bool has_bbox = false; float lo[3], hi[3]; };
     std::vector<Segment> segments;
     DevBuf<float4> merged, merged2;
+    // lvb_icp_map_build_optimize_keyframe builds the map frame here and swaps it in only when the device found no failure
+    DevBuf<float4> nx_sorted;
+    DevBuf<int> nx_cell_start, nx_coarse;
     int scan_n = 0, scan_stride = 0;          // the scan of the last upload_scan (reusable by lvb_icp_map_append)
     const unsigned char* scan_dev = nullptr;  // where that scan lies: scan_raw, or this handle's part of kf_arena
     // lvb_icp_map_optimize_keyframe's upload: [KfBlock | ground scan | surf scan] in one allocation, held by both handles of the call
@@ -546,28 +700,39 @@ static int icheck(const char* what) {
     return LVB_OK;
 }
 
-// The association buffers and the visiting order of the n queries at d_scan (device, stride bytes each).  The query transform is
-// d.tf (set by the caller), or, when tf_dev is given, the float[7] at tf_dev in device memory.
-static int bind_scan(lvb_icp* h, const unsigned char* d_scan, int n, int stride, const float* tf_dev, float max_d2, double thr, IcpDev& d) {
-    cudaStream_t s = h->ctx->stream;
+// key granularity of the query visiting order: blocks of 2 x 2 x 2 voxels (measured on configs[2], association kernel: 4 x 4 x 4
+// blocks 0.51 ms, 2 x 2 x 2 0.44 ms, single voxels 0.50 ms plus a slower sort) -- coarser only when the grid would need more than
+// 8 M counters; env LVB_ICP_SORT_SHIFT forces one (A/B)
+static int sort_shift_forced() {
+    static const int forced = getenv("LVB_ICP_SORT_SHIFT") ? atoi(getenv("LVB_ICP_SORT_SHIFT")) : -1;
+    return forced;
+}
+
+// the association buffers of the n queries at d_scan and everything of d but the map grid
+static int bind_buffers(lvb_icp* h, const unsigned char* d_scan, int n, int stride, float max_d2, double thr, IcpDev& d) {
     h->scan_n = n; h->scan_stride = stride; h->scan_dev = d_scan;
     LVB_TRY(h->accepted.ensure(std::max(1, n)));
     LVB_TRY(h->pa.ensure((size_t)std::max(1, n) * 3));
     LVB_TRY(h->nrm.ensure((size_t)std::max(1, n) * 3));
     LVB_TRY(h->st.ensure(1));
-    d.map = h->map_sorted.p; d.cell_start = h->cell_start.p; d.g = h->grid; d.P = h->P;
-    d.coarse = h->coarse.p; d.cbx = h->cbx; d.cby = h->cby; d.cbz = h->cbz;
     d.scan = d_scan; d.K = n; d.stride = stride;
     d.max_d2 = max_d2; d.thr = thr;
     d.accepted = h->accepted.p; d.pa = h->pa.p; d.nrm = h->nrm.p; d.st = h->st.p;
     d.rank = h->ctx->rank; d.world = h->ctx->world;
     d.order = nullptr;
+    return LVB_OK;
+}
+
+// The association buffers and the visiting order of the n queries at d_scan (device, stride bytes each).  The query transform is
+// d.tf (set by the caller), or, when tf_dev is given, the float[7] at tf_dev in device memory.
+static int bind_scan(lvb_icp* h, const unsigned char* d_scan, int n, int stride, const float* tf_dev, float max_d2, double thr, IcpDev& d) {
+    cudaStream_t s = h->ctx->stream;
+    LVB_TRY(bind_buffers(h, d_scan, n, stride, max_d2, thr, d));
+    d.map = h->map_sorted.p; d.cell_start = h->cell_start.p; d.g = h->grid; d.P = h->P;
+    d.coarse = h->coarse.p; d.cbx = h->cbx; d.cby = h->cby; d.cbz = h->cbz;
     if (n >= 4096) {       // spatial visiting order: counting sort of the queries by coarse voxel block
         const Grid& g = h->grid;
-        // key granularity: blocks of 2 x 2 x 2 voxels (measured on configs[2], association kernel: 4 x 4 x 4 blocks 0.51 ms, 2 x 2 x 2
-        // 0.44 ms, single voxels 0.50 ms plus a slower sort) -- coarser only when the grid would need more than 8 M counters;
-        // env LVB_ICP_SORT_SHIFT forces one (A/B)
-        static const int forced = getenv("LVB_ICP_SORT_SHIFT") ? atoi(getenv("LVB_ICP_SORT_SHIFT")) : -1;
+        const int forced = sort_shift_forced();
         int shift = 1;
         while (forced < 0 && (double)((g.gx >> shift) + 1) * ((g.gy >> shift) + 1) * ((g.gz >> shift) + 1) > 8.0e6) ++shift;
         if (forced >= 0) shift = forced;
@@ -598,6 +763,9 @@ static int upload_scan(lvb_icp* h, const void* scan, int n, int stride, const do
     return bind_scan(h, h->scan_raw.p, n, stride, nullptr, max_d2, thr, d);
 }
 
+// exchange two buffers' ownership (DevBuf has no move operations)
+template <class T> static void swap_buf(DevBuf<T>& a, DevBuf<T>& b) { std::swap(a.p, b.p); std::swap(a.n, b.n); std::swap(a.s, b.s); std::swap(a.view, b.view); }
+
 extern "C" {
 
 int lvb_icp_create(lvb_ctx* ctx, lvb_icp** out) {
@@ -622,7 +790,7 @@ static int build_hash(lvb_icp* h, const unsigned char* d_points, int n, int stri
     LVB_TRY(icheck("bbox"));
     int hb[6];
     LVB_TRY(h->bbox.download(hb, 6, s));
-    LVB_CUDA(cudaStreamSynchronize(s));
+    LVB_TRY(host_sync(h->ctx, s));
     Grid g;
     // The voxel edge is (radius * 1.0001) / ring: the hair of slack guarantees that float rounding of the voxel
     // coordinate never separates two points closer than the radius by more than `ring` voxels.  ring = 4 unless the
@@ -657,7 +825,7 @@ static int build_hash(lvb_icp* h, const unsigned char* d_points, int n, int stri
     ILAUNCH(h, scan_add_kernel, nb, 1024, h->cell_start.p, ncell, h->block_sums.p, h->cell_start.p + ncell, h->total.p);
     ILAUNCH(h, icp_scatter_kernel, inblk(n, 256), 256, d_points, n, stride, h->cell_of.p, h->cell_start.p, h->fill.p, h->map_sorted.p);
     LVB_TRY(icheck("set_map"));
-    LVB_CUDA(cudaStreamSynchronize(s));
+    LVB_TRY(host_sync(h->ctx, s));
     h->grid = g; h->P = n; h->cell_size = cell_size; h->have_map = true;
     return LVB_OK;
 }
@@ -696,7 +864,7 @@ int lvb_icp_map_append(lvb_icp* h, long long key, const void* robot_points, int 
     ILAUNCH(h, icp_to_world_kernel, inblk(n, 256), 256, src, sg.pts->p, n, stride, d_tf.p);
     rc = icheck("map_append");
     if (rc != LVB_OK) { delete sg.pts; return rc; }
-    LVB_CUDA(cudaStreamSynchronize(s));
+    LVB_TRY(host_sync(h->ctx, s));
     h->segments.push_back(sg);
     return LVB_OK;
 }
@@ -752,7 +920,7 @@ int lvb_icp_map_download(lvb_icp* h, float* xyzi, int capacity, int* n_out) {
     // hand the cloud back in its original (merge) order: map_sorted carries the original index in .w
     std::vector<float4> tmp(h->P);
     LVB_CUDA(cudaMemcpyAsync(tmp.data(), h->map_sorted.p, (size_t)h->P * sizeof(float4), cudaMemcpyDeviceToHost, h->ctx->stream));
-    LVB_CUDA(cudaStreamSynchronize(h->ctx->stream));
+    LVB_TRY(host_sync(h->ctx, h->ctx->stream));
     for (int j = 0; j < h->P; ++j) { int i; memcpy(&i, &tmp[j].w, 4); if (i < 0 || i >= h->P) { set_error("corrupt index"); return LVB_ERR_NUMERIC; } xyzi[4 * (size_t)i] = tmp[j].x; xyzi[4 * (size_t)i + 1] = tmp[j].y; xyzi[4 * (size_t)i + 2] = tmp[j].z; xyzi[4 * (size_t)i + 3] = 0.0f; }
     return LVB_OK;
 }
@@ -768,7 +936,7 @@ int lvb_icp_transform_cloud(lvb_icp* h, const void* points, int n, int stride, c
     ILAUNCH(h, icp_transform_cloud_kernel, inblk(n, 256), 256, d_in.p, d_out.p, n, stride, d_tf.p);
     LVB_TRY(icheck("transform_cloud"));
     LVB_TRY(d_out.download((unsigned char*)out, (size_t)n * stride, s));
-    LVB_CUDA(cudaStreamSynchronize(s));
+    LVB_TRY(host_sync(h->ctx, s));
     return LVB_OK;
 }
 
@@ -783,7 +951,7 @@ int lvb_icp_knn3(lvb_icp* h, const void* scan, int n, int stride, const double f
     LVB_TRY(icheck("knn3"));
     LVB_TRY(h->knn_idx.download(idx, (size_t)n * 3, h->ctx->stream));
     LVB_TRY(h->knn_d2.download(d2, (size_t)n * 3, h->ctx->stream));
-    LVB_CUDA(cudaStreamSynchronize(h->ctx->stream));
+    LVB_TRY(host_sync(h->ctx, h->ctx->stream));
     return LVB_OK;
 }
 
@@ -800,7 +968,7 @@ static int init_state(lvb_icp* h, int mode, const double* map_pose, const double
     for (int k = 0; k < 3; ++k) { hs.x[k] = rpyxyz[fr[mode][k]]; hs.cand[k] = hs.x[k]; hs.prior_target[k] = hs.x[k]; }
     hs.prior_w = prior_w; hs.huber_a = huber_a; hs.weight = weight;
     LVB_CUDA(cudaMemcpyAsync(h->st.p, &hs, sizeof(hs), cudaMemcpyHostToDevice, h->ctx->stream));
-    LVB_CUDA(cudaStreamSynchronize(h->ctx->stream));
+    LVB_TRY(host_sync(h->ctx, h->ctx->stream));
     return LVB_OK;
 }
 
@@ -829,7 +997,7 @@ int lvb_icp_eval(lvb_icp* h, int mode, const void* scan, int n, int stride, cons
     if (accepted) LVB_TRY(h->accepted.download(accepted, n, s));
     if (r) LVB_TRY(h->eval_r.download(r, n, s));
     if (J) LVB_TRY(h->eval_J.download(J, (size_t)n * 3, s));
-    LVB_CUDA(cudaStreamSynchronize(s));
+    LVB_TRY(host_sync(h->ctx, s));
     return LVB_OK;
 }
 
@@ -862,7 +1030,7 @@ int lvb_icp_scan_to_map(lvb_icp* h, int mode, const void* scan, int n, int strid
         ILAUNCH(h, icp_post_kernel, 1, 1, d.st);
         LVB_TRY(icheck("icp iteration"));
         LVB_CUDA(cudaMemcpyAsync(&hs, h->st.p, sizeof(hs), cudaMemcpyDeviceToHost, s));
-        LVB_CUDA(cudaStreamSynchronize(s));
+        LVB_TRY(host_sync(h->ctx, s));
         LVB_TRY(comm_check(ctx));
         if (hs.lm.done) break;
         if (opt.max_solver_time_in_seconds < 1e8) {      // collective decision when the queries are sharded (see lvb_ba_solve)
@@ -969,7 +1137,7 @@ int lvb_icp_map_optimize_keyframe(lvb_icp* ground, lvb_icp* surf, const double m
     }
     // the one read-back: both solver states, rpyxyz and the pose
     LVB_CUDA(cudaMemcpyAsync(ctx->stage_h, blk, sizeof(KfBlock), cudaMemcpyDeviceToHost, s));
-    LVB_CUDA(cudaStreamSynchronize(s));
+    LVB_TRY(host_sync(ctx, s));
     ctx->stage_busy = false;
     const double el = std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
     memcpy(pose, hb->pose, sizeof(hb->pose)); memcpy(rpyxyz, hb->rpyxyz, sizeof(hb->rpyxyz));
@@ -980,6 +1148,277 @@ int lvb_icp_map_optimize_keyframe(lvb_icp* ground, lvb_icp* surf, const double m
             summary[m].termination_type = -1;          // registration skipped (mapping.cpp:155,167: empty map cloud)
         }
     }
+    return LVB_OK;
+}
+
+// ---- Mapping::BuildMapFrame + Mapping::Optimize for one keyframe in one call (lvb_icp_map_build_optimize_keyframe)
+struct BkBlock {             // the call's device state, uploaded and read back with one copy each
+    KfBlock kf;
+    MapDesc map[2];          // [0] ground, [1] surf map frame
+    int out_bbox[2][6];      // bounding boxes of the two clouds ToWorld stores
+};
+
+static void bbox_seed(int* b) {       // icp_bbox_kernel's starting values: min = FLT_MAX, max = -FLT_MAX as ordered ints
+    float big = FLT_MAX, small = -FLT_MAX; int bi, si; memcpy(&bi, &big, 4); memcpy(&si, &small, 4);
+    const int so = si >= 0 ? si : si ^ 0x7fffffff;
+    b[0] = b[1] = b[2] = bi; b[3] = b[4] = b[5] = so;
+}
+static void bbox_store(lvb_icp::Segment& sg, const int* b) {
+    for (int a = 0; a < 3; ++a) { sg.lo[a] = ord2f(b[a]); sg.hi[a] = ord2f(b[3 + a]); }
+    sg.has_bbox = true;
+}
+
+// Clouds stored by lvb_icp_map_append / lvb_icp_map_optimize_keyframe carry no bounding box: compute those of `segs` (of any handle
+// on h's context) once, all with one host synchronisation, and keep them with the segments.
+static int fill_bboxes(lvb_icp* h, const std::vector<lvb_icp::Segment*>& segs) {
+    std::vector<lvb_icp::Segment*> todo;
+    for (auto* sg : segs) if (!sg->has_bbox) todo.push_back(sg);
+    if (todo.empty()) return LVB_OK;
+    lvb_ctx* ctx = h->ctx;
+    cudaStream_t s = ctx->stream;
+    const size_t bytes = todo.size() * 6 * sizeof(int);
+    LVB_TRY(lvb::stage_wait(ctx));
+    LVB_TRY(lvb::stage_grow(ctx, bytes, 0));
+    int* hb = reinterpret_cast<int*>(ctx->stage_h);
+    for (size_t i = 0; i < todo.size(); ++i) bbox_seed(hb + 6 * i);
+    DevBuf<int> d;
+    LVB_TRY(d.ensure(todo.size() * 6));
+    LVB_CUDA(cudaMemcpyAsync(d.p, hb, bytes, cudaMemcpyHostToDevice, s));
+    for (size_t i = 0; i < todo.size(); ++i)
+        ILAUNCH(h, icp_bbox_kernel, std::min(1024, inblk(todo[i]->n, 256)), 256, reinterpret_cast<const unsigned char*>(todo[i]->pts->p), todo[i]->n, 16, d.p + 6 * i);
+    LVB_TRY(icheck("map frame bounding boxes"));
+    LVB_CUDA(cudaMemcpyAsync(hb, d.p, bytes, cudaMemcpyDeviceToHost, s));
+    LVB_TRY(host_sync(ctx, s));
+    for (size_t i = 0; i < todo.size(); ++i) bbox_store(*todo[i], hb + 6 * i);
+    return LVB_OK;
+}
+
+// Capacities of a map frame whose cloud lies inside the box lo..hi: build_hash's ring-4 grid of the box (the voxel counts per axis
+// only shrink with a smaller box or a coarser ring), capped at MAX_CELLS -- above it the device picks a coarser ring or fails.
+struct MapBound { size_t cells, coarse, qsort; bool finite; };
+static MapBound map_bound(const float* lo, const float* hi, float cell_size) {
+    MapBound b;
+    const float cell = cell_size * 1.0001f / 4.0f, inv = 1.0f / cell;
+    double d[3];
+    b.finite = true;
+    for (int a = 0; a < 3; ++a) {
+        const float w = hi[a] - lo[a];
+        if (!(hi[a] >= lo[a]) || !std::isfinite(w)) { b.finite = false; d[a] = 0; } else d[a] = std::floor((double)w * inv) + 1;
+    }
+    const double cap = (double)MAX_CELLS;
+    const int forced = sort_shift_forced();
+    if (!b.finite) { b.cells = b.coarse = MAX_CELLS; b.qsort = forced < 0 ? 8000000 : MAX_CELLS; return b; }
+    auto blocks = [&](int sh) { double v = 1; for (int a = 0; a < 3; ++a) v *= std::ceil(d[a] / (double)(1 << sh)); return v; };
+    b.cells = (size_t)std::min(cap, d[0] * d[1] * d[2]);
+    b.coarse = (size_t)std::min(cap, blocks(2));
+    // bind_scan's rule keeps the sort grid at <= 8 M counters; a forced granularity is bounded by the voxel count
+    b.qsort = forced < 0 ? (size_t)std::min(8.0e6, blocks(1)) : (size_t)std::min((double)b.cells, blocks(forced));
+    return b;
+}
+
+// bind_scan against the map frame of m (device), its counters sized for `bound`
+static int bind_scan_map(lvb_icp* h, const unsigned char* d_scan, int n, int stride, const float* tf_dev, float max_d2, double thr,
+                         const MapDesc* m, const MapBound& bound, IcpDev& d) {
+    LVB_TRY(bind_buffers(h, d_scan, n, stride, max_d2, thr, d));
+    d.map = h->nx_sorted.p; d.cell_start = h->nx_cell_start.p; d.coarse = h->nx_coarse.p;
+    memset(&d.g, 0, sizeof(d.g)); d.P = 0; d.cbx = d.cby = d.cbz = 0;          // read from m by the kernels
+    if (n >= 4096) {
+        const int nc = (int)std::max<size_t>(1, bound.qsort), nb = (nc + 1023) / 1024;
+        LVB_TRY(h->q_key.ensure(n)); LVB_TRY(h->q_order.ensure(n)); LVB_TRY(h->q_counts.ensure(nc)); LVB_TRY(h->q_fill.ensure(nc));
+        LVB_TRY(h->q_start.ensure((size_t)nc + 1)); LVB_TRY(h->q_sums.ensure(nb)); LVB_TRY(h->q_total.ensure(1));
+        ILAUNCH(h, icp_zero_map_kernel, std::min(inblk(nc, 256), 8 * h->ctx->sm_count), 256, h->q_counts.p, h->q_fill.p, &m->nc);
+        ILAUNCH(h, icp_query_key_map_kernel, (n + 255) / 256, 256, d, tf_dev, m, h->q_key.p, h->q_counts.p);
+        ILAUNCH(h, scan_block_map_kernel, nb, 1024, h->q_counts.p, h->q_start.p, &m->nc, h->q_sums.p);
+        ILAUNCH(h, scan_sums_map_kernel, 1, 1024, h->q_sums.p, &m->nc, h->q_total.p);
+        ILAUNCH(h, scan_add_map_kernel, nb, 1024, h->q_start.p, &m->nc, h->q_sums.p, h->q_total.p);
+        ILAUNCH(h, icp_query_scatter_kernel, (n + 255) / 256, 256, n, h->q_key.p, h->q_start.p, h->q_fill.p, h->q_order.p);
+        d.order = h->q_order.p;
+    }
+    return LVB_OK;
+}
+
+// Mapping::BuildMapFrame (mapping.cpp:114-137) + the body of Mapping::Optimize's loop (:147-185) for one keyframe.  The host knows
+// every size the launches depend on -- the scans, the merged clouds (sums of resident cloud sizes), max_num_iterations -- and an upper
+// bound on each map frame's grid (map_bound of the union of the resident clouds' boxes); the device decides the grid itself
+// (icp_map_grid_kernel) and every counter is used up to that size.  One pinned upload, one read-back, one host synchronisation.
+int lvb_icp_map_build_optimize_keyframe(lvb_icp* ground, lvb_icp* surf, const long long* keys, int n_keys, const float cell_size[2],
+                                        double ground_threshold, const double map_pose[7], long long key, const void* ground_pts, int n_ground,
+                                        const void* surf_pts, int n_surf, int stride, const lvb_map_optimize_params* p, double pose[7],
+                                        double rpyxyz[6], lvb_solve_summary summary[2], int n_map_points[2]) {
+    static const char* fn = "lvb_icp_map_build_optimize_keyframe";
+    lvb_icp* hs[2] = {ground, surf};
+    const void* pts[2] = {ground_pts, surf_pts};
+    const int ns[2] = {n_ground, n_surf};
+    if (!ground || !surf || ground == surf || !cell_size || !map_pose || !p || !pose || !rpyxyz || n_keys < 0 || (n_keys && !keys)) {
+        set_error("%s: null or bad argument", fn); return LVB_ERR_INVALID; }
+    lvb_ctx* ctx = ground->ctx;
+    if (surf->ctx != ctx) { set_error("%s: the two handles belong to different contexts", fn); return LVB_ERR_INVALID; }
+    if (ctx->world > 1) { set_error("%s: sharded contexts register through lvb_icp_scan_to_map", fn); return LVB_ERR_UNSUPPORTED; }
+    const lvb_solve_options& opt = p->options;
+    if (opt.max_solver_time_in_seconds < 1e8) { set_error("%s: no time limit (Mapping::Optimize sets none)", fn); return LVB_ERR_INVALID; }
+    if (opt.max_num_iterations < 0 || stride < 12 || (stride & 3)) { set_error("%s: bad arguments", fn); return LVB_ERR_INVALID; }
+    for (int m = 0; m < 2; ++m) {
+        if (ns[m] < 0 || (ns[m] && !pts[m])) { set_error("%s: bad scan arguments", fn); return LVB_ERR_INVALID; }
+        if (!(cell_size[m] > 0.0f)) { set_error("%s: bad cell size", fn); return LVB_ERR_INVALID; }
+        if ((double)cell_size[m] * cell_size[m] * (1.0 + 1e-6) < p->dist_thr[m]) {
+            set_error("%s: dist_thr %.6g exceeds cell_size^2 %.6g", fn, p->dist_thr[m], (double)cell_size[m] * cell_size[m]); return LVB_ERR_INVALID; }
+    }
+    // the map frame: keys resident on both handles, in merge order; `key` is the keyframe being registered, not one of them
+    std::vector<lvb_icp::Segment*> pick[2];
+    size_t total[2] = {0, 0};
+    for (int k = 0; k < n_keys; ++k) {
+        if (keys[k] == key) { set_error("%s: key %lld is one of the map frame's keys", fn, key); return LVB_ERR_INVALID; }
+        for (int m = 0; m < 2; ++m) {
+            lvb_icp::Segment* f = nullptr;
+            for (auto& sg : hs[m]->segments) if (sg.key == keys[k]) f = &sg;
+            if (!f) { set_error("%s: key %lld is not resident", fn, keys[k]); return LVB_ERR_INVALID; }
+            pick[m].push_back(f); total[m] += f->n;
+        }
+    }
+    if (total[0] > 0x7fffffffull || total[1] > 0x7fffffffull) { set_error("%s: map frame of more than 2^31 points", fn); return LVB_ERR_INVALID; }
+    LVB_CUDA(cudaSetDevice(ctx->device)); lvb::g_alloc_stream = ctx->stream;
+    {   // both handles' missing boxes with one synchronisation
+        std::vector<lvb_icp::Segment*> both(pick[0]);
+        both.insert(both.end(), pick[1].begin(), pick[1].end());
+        LVB_TRY(fill_bboxes(ground, both));
+    }
+    const bool ransac = ground_threshold > 0.0;
+    bool build[2];
+    MapBound bound[2];
+    for (int m = 0; m < 2; ++m) {
+        build[m] = total[m] > 0;           // an empty merged cloud: BuildMapFrame fails on that side and nothing registers (:155,167)
+        if (!build[m]) continue;
+        float lo[3] = {FLT_MAX, FLT_MAX, FLT_MAX}, hi[3] = {-FLT_MAX, -FLT_MAX, -FLT_MAX};
+        for (auto* sg : pick[m]) for (int a = 0; a < 3; ++a) { lo[a] = std::min(lo[a], sg->lo[a]); hi[a] = std::max(hi[a], sg->hi[a]); }
+        bound[m] = map_bound(lo, hi, cell_size[m]);
+        // without SegmentGround the map frame's box is the union: build_hash's check can be made here (after it, on the device)
+        if (!bound[m].finite && !(m == 0 && ransac)) { set_error("%s: map cloud has no finite bounding box", fn); return LVB_ERR_INVALID; }
+    }
+    const auto t0 = std::chrono::steady_clock::now();
+    cudaStream_t s = ctx->stream;
+    lvb::timing_mark(s, "begin");
+    // one upload: [BkBlock | ground scan | surf scan], assembled in the pinned staging area
+    size_t off[2], bytes[2], all = (sizeof(BkBlock) + 255) & ~(size_t)255;
+    for (int m = 0; m < 2; ++m) { bytes[m] = (size_t)ns[m] * stride; off[m] = all; all = (all + bytes[m] + 255) & ~(size_t)255; }
+    LVB_TRY(lvb::stage_wait(ctx));
+    LVB_TRY(lvb::stage_grow(ctx, all, 0));
+    BkBlock* hb = reinterpret_cast<BkBlock*>(ctx->stage_h);
+    memset(hb, 0, sizeof(BkBlock));
+    memcpy(hb->kf.map_pose, map_pose, sizeof(hb->kf.map_pose)); memcpy(hb->kf.pose, pose, sizeof(hb->kf.pose));
+    for (int m = 0; m < 2; ++m) {
+        bbox_seed(hb->map[m].bbox); bbox_seed(hb->out_bbox[m]);
+        hb->map[m].P = build[m] && !(m == 0 && ransac) ? (int)total[m] : 0;      // the ground count comes from SegmentGround
+        if (bytes[m]) memcpy(ctx->stage_h + off[m], pts[m], bytes[m]);
+    }
+    auto arena = std::make_shared<DevBuf<unsigned char>>();
+    LVB_TRY(arena->ensure(all));
+    LVB_CUDA(cudaMemcpyAsync(arena->p, ctx->stage_h, all, cudaMemcpyHostToDevice, s));
+    LVB_TRY(lvb::stage_mark_busy(ctx, s));
+    BkBlock* blk = reinterpret_cast<BkBlock*>(arena->p);
+
+    // BuildMapFrame: merge in key order, SegmentGround on the ground side, voxel hash sized by the bound, grid decided on the device
+    for (int m = 0; m < 2; ++m) {
+        if (!build[m]) continue;
+        lvb_icp* h = hs[m];
+        MapDesc* md = &blk->map[m];
+        const int n = (int)total[m];
+        const MapBound& b = bound[m];
+        LVB_TRY(h->merged.ensure(n));
+        size_t o = 0;
+        for (auto* f : pick[m]) { if (f->n) LVB_CUDA(cudaMemcpyAsync(h->merged.p + o, f->pts->p, (size_t)f->n * sizeof(float4), cudaMemcpyDeviceToDevice, s)); o += f->n; }
+        const float4* cloud = h->merged.p;
+        if (m == 0 && ransac) {
+            LVB_TRY(h->merged2.ensure(n));
+            LVB_TRY(lidar_segment_ground_device_async(ctx, h->merged.p, n, ground_threshold, h->merged2.p, &md->P));
+            lvb::g_alloc_stream = ctx->stream;
+            cloud = h->merged2.p;
+        }
+        const unsigned char* cp = reinterpret_cast<const unsigned char*>(cloud);
+        const int nb = inblk(b.cells, 1024);
+        LVB_TRY(h->cell_of.ensure(n)); LVB_TRY(h->counts.ensure(b.cells)); LVB_TRY(h->fill.ensure(b.cells));
+        LVB_TRY(h->nx_cell_start.ensure(b.cells + 1)); LVB_TRY(h->nx_sorted.ensure(n)); LVB_TRY(h->nx_coarse.ensure(b.coarse));
+        LVB_TRY(h->block_sums.ensure(nb)); LVB_TRY(h->total.ensure(1));
+        ILAUNCH(h, icp_bbox_map_kernel, std::min(1024, inblk(n, 256)), 256, cp, 16, md);
+        ILAUNCH(h, icp_map_grid_kernel, 1, 1, md, cell_size[m], sort_shift_forced());
+        ILAUNCH(h, icp_zero_map_kernel, std::min(inblk(b.cells, 256), 8 * ctx->sm_count), 256, h->counts.p, h->fill.p, &md->ncell);
+        ILAUNCH(h, icp_zero_map_kernel, std::min(inblk(b.coarse, 256), 8 * ctx->sm_count), 256, h->nx_coarse.p, (int*)nullptr, &md->ncb);
+        ILAUNCH(h, icp_count_map_kernel, inblk(n, 256), 256, cp, 16, md, h->cell_of.p, h->counts.p, h->nx_coarse.p);
+        ILAUNCH(h, scan_block_map_kernel, nb, 1024, h->counts.p, h->nx_cell_start.p, &md->ncell, h->block_sums.p);
+        ILAUNCH(h, scan_sums_map_kernel, 1, 1024, h->block_sums.p, &md->ncell, h->total.p);
+        ILAUNCH(h, scan_add_map_kernel, nb, 1024, h->nx_cell_start.p, &md->ncell, h->block_sums.p, h->total.p);
+        ILAUNCH(h, icp_scatter_map_kernel, inblk(n, 256), 256, cp, 16, md, h->cell_of.p, h->nx_cell_start.p, h->fill.p, h->nx_sorted.p);
+        LVB_TRY(icheck("map frame build"));
+    }
+
+    // the registrations (as lvb_icp_map_optimize_keyframe), each against the map frame just built
+    struct ScanState { int n, stride; const unsigned char* dev; std::shared_ptr<DevBuf<unsigned char>> arena; } saved[2];
+    for (int m = 0; m < 2; ++m) saved[m] = {hs[m]->scan_n, hs[m]->scan_stride, hs[m]->scan_dev, hs[m]->kf_arena};
+    KfSeed seed;
+    seed.o = opt; seed.prior_w = p->prior_weight;
+    for (int m = 0; m < 2; ++m) { seed.weight[m] = p->weight[m]; seed.huber_a[m] = p->huber_a[m]; }
+    const int first = build[0] ? 0 : (build[1] ? 1 : -1);
+    ILAUNCH(ground, icp_kf_pose_map_kernel, 1, 1, &blk->kf, -1, first, seed, blk->map);      // rpyxyz from the incoming pose (:154)
+    for (int m = 0; m < 2; ++m) {
+        if (!build[m]) continue;
+        lvb_icp* h = hs[m];
+        const MapDesc* md = &blk->map[m];
+        IcpDev d;
+        LVB_TRY(bind_scan_map(h, arena->p + off[m], ns[m], stride, blk->kf.tf, cell_size[m] * cell_size[m], p->dist_thr[m], md, bound[m], d));
+        d.st = &blk->kf.st[m];
+        ILAUNCH(h, icp_associate_map_kernel, inblk(ns[m], ITPB), ITPB, d, blk->kf.tf, md);
+        const int lin_blocks = std::max(1, std::min(inblk(ns[m], ITPB), 4 * ctx->sm_count));
+        for (int pass = 0; pass <= opt.max_num_iterations; ++pass) {
+            ILAUNCH(h, icp_linearize_kernel<0>, lin_blocks, ITPB, d);
+            ILAUNCH(h, icp_solve_kernel, 1, 1, d.st);
+            ILAUNCH(h, icp_linearize_kernel<1>, lin_blocks, ITPB, d);
+            ILAUNCH(h, icp_post_kernel, 1, 1, d.st);
+        }
+        ILAUNCH(h, icp_kf_pose_map_kernel, 1, 1, &blk->kf, m, m == 0 && build[1] ? 1 : -1, seed, blk->map);
+    }
+    // ToWorld (:205-220): both robot-frame clouds, transformed by the final pose.cast<float>(), with their bounding boxes
+    lvb_icp::Segment fresh[2];
+    for (int m = 0; m < 2; ++m) {
+        fresh[m].key = key; fresh[m].n = ns[m]; fresh[m].pts = new DevBuf<float4>();
+        const int rc = fresh[m].pts->ensure(std::max(1, ns[m]));
+        if (rc != LVB_OK) { delete fresh[0].pts; if (m) delete fresh[1].pts; return rc; }
+        ILAUNCH(hs[m], icp_to_world_bbox_kernel, inblk(ns[m], 256), 256, arena->p + off[m], fresh[m].pts->p, ns[m], stride, blk->kf.tf, blk->out_bbox[m]);
+    }
+    int rc = icheck("map_build_optimize_keyframe");
+    // the one read-back: solver states, pose, rpyxyz, both map descriptors (grid, point count, failure), the stored clouds' boxes
+    if (rc == LVB_OK && cudaMemcpyAsync(ctx->stage_h, blk, sizeof(BkBlock), cudaMemcpyDeviceToHost, s) != cudaSuccess) rc = lvb::cuda_fail(cudaGetLastError(), "read-back", __FILE__, __LINE__);
+    if (rc == LVB_OK) rc = host_sync(ctx, s);
+    if (rc == LVB_OK) ctx->stage_busy = false;
+    for (int m = 0; m < 2 && rc == LVB_OK; ++m) {
+        if (!build[m] || !hb->map[m].err) continue;
+        if (hb->map[m].err == 1) { set_error("%s: map cloud has no finite bounding box", fn); rc = LVB_ERR_INVALID; }
+        else { set_error("%s: voxel grid of the %s map frame exceeds %d cells; increase cell_size or crop the map", fn, m ? "surf" : "ground", (int)MAX_CELLS); rc = LVB_ERR_UNSUPPORTED; }
+    }
+    if (rc != LVB_OK) {        // nothing was committed: the resident clouds and the map frames are as they were
+        delete fresh[0].pts; delete fresh[1].pts;
+        for (int m = 0; m < 2; ++m) { hs[m]->scan_n = saved[m].n; hs[m]->scan_stride = saved[m].stride; hs[m]->scan_dev = saved[m].dev; hs[m]->kf_arena = saved[m].arena; }
+        return rc;
+    }
+    const double el = std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
+    for (int m = 0; m < 2; ++m) {
+        lvb_icp* h = hs[m];
+        const MapDesc& md = hb->map[m];
+        const bool built = build[m] && md.P > 0;
+        if (built) {           // the new map frame replaces the one before, as lvb_icp_map_build would
+            swap_buf(h->map_sorted, h->nx_sorted); swap_buf(h->cell_start, h->nx_cell_start); swap_buf(h->coarse, h->nx_coarse);
+            h->grid = md.g; h->P = md.P; h->cbx = md.cbx; h->cby = md.cby; h->cbz = md.cbz; h->cell_size = cell_size[m]; h->have_map = true;
+        }
+        bbox_store(fresh[m], hb->out_bbox[m]);
+        bool replaced = false;
+        for (auto& sg : h->segments) if (sg.key == key) { delete sg.pts; sg = fresh[m]; replaced = true; }
+        if (!replaced) h->segments.push_back(fresh[m]);
+        h->scan_n = ns[m]; h->scan_stride = stride; h->scan_dev = arena->p + off[m]; h->kf_arena = arena;
+        if (n_map_points) n_map_points[m] = built ? md.P : 0;
+        if (summary) {
+            if (built) fill_summary(hb->kf.st[m], p->prior_weight, el, &summary[m]);
+            else { memset(&summary[m], 0, sizeof(summary[m])); summary[m].termination_type = -1; }
+        }
+    }
+    memcpy(pose, hb->kf.pose, sizeof(hb->kf.pose)); memcpy(rpyxyz, hb->kf.rpyxyz, sizeof(hb->kf.rpyxyz));
     return LVB_OK;
 }
 

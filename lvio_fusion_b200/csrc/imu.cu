@@ -164,6 +164,6 @@ extern "C" int lvb_imu_preintegrate(lvb_ctx* ctx, int n, const int32_t* first, c
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) { lvb::set_error("imu_preintegrate launch failed: %s", cudaGetErrorString(e)); return LVB_ERR_CUDA; }
     LVB_TRY(d_out.download(consts, (size_t)n * IMU_OUT, s));
-    LVB_CUDA(cudaStreamSynchronize(s));
+    LVB_TRY(lvb::host_sync(ctx, s));
     return LVB_OK;
 }

@@ -32,8 +32,9 @@ __device__ __forceinline__ float3 transform_f32(const float* tf, float3 p) {
     return make_float3(__fadd_rn(rx, tf[4]), __fadd_rn(ry, tf[5]), __fadd_rn(rz, tf[6]));
 }
 
-// exclusive scan, 1024 elements per block: (1) per-block scan + block totals, (2) scan of totals, (3) add
-__global__ void scan_block_kernel(const int* in, int* out, int n, int* block_sums) {
+// exclusive scan, 1024 elements per block: (1) per-block scan + block totals, (2) scan of totals, (3) add.  The bodies are shared with
+// icp.cu's variants that read the element count from device memory.
+__device__ __forceinline__ void scan_block(const int* in, int* out, int n, int* block_sums) {
     __shared__ int s[1024];
     const int i = blockIdx.x * 1024 + threadIdx.x;
     const int v = i < n ? in[i] : 0;
@@ -48,7 +49,7 @@ __global__ void scan_block_kernel(const int* in, int* out, int n, int* block_sum
     if (i < n) out[i] = s[threadIdx.x] - v;
     if (threadIdx.x == 1023) block_sums[blockIdx.x] = s[1023];
 }
-__global__ void scan_sums_kernel(int* block_sums, int nb, int* total_out) {
+__device__ __forceinline__ void scan_sums(int* block_sums, int nb, int* total_out) {
     __shared__ int s[1024];
     __shared__ int carry;
     if (threadIdx.x == 0) carry = 0;
@@ -71,10 +72,13 @@ __global__ void scan_sums_kernel(int* block_sums, int nb, int* total_out) {
     }
     if (threadIdx.x == 0) *total_out = carry;
 }
-__global__ void scan_add_kernel(int* out, int n, const int* block_sums, int* last /*out[n] = total*/, const int* total) {
+__device__ __forceinline__ void scan_add(int* out, int n, const int* block_sums, int* last, const int* total) {
     const int i = blockIdx.x * 1024 + threadIdx.x;
     if (i < n) out[i] += block_sums[blockIdx.x];
     if (i == 0) *last = *total;
 }
+__global__ void scan_block_kernel(const int* in, int* out, int n, int* block_sums) { scan_block(in, out, n, block_sums); }
+__global__ void scan_sums_kernel(int* block_sums, int nb, int* total_out) { scan_sums(block_sums, nb, total_out); }
+__global__ void scan_add_kernel(int* out, int n, const int* block_sums, int* last /*out[n] = total*/, const int* total) { scan_add(out, n, block_sums, last, total); }
 
 }  // namespace

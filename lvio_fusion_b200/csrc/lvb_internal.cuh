@@ -27,6 +27,7 @@ struct lvb_ctx {
     cudaEvent_t ev_fork = nullptr, ev_join = nullptr;
     bool use_side = true;               // env LVB_NO_SIDE=1 disables
     long long launches = 0;
+    long long syncs = 0;                // host waits on this context's stream (lvb::host_sync, lvb::stage_wait)
     int sm_count = 132;
     bool use_tma = true;          // cp.async.bulk staging of the pose array (env LVB_NO_TMA=1 disables)
     bool use_graph = true;        // replay the LM pass as a CUDA graph (env LVB_NO_GRAPH=1 disables)
@@ -66,6 +67,11 @@ int comm_allreduce_max_i32(lvb_ctx* ctx, int* buf, size_t count);
 extern bool g_timing;
 void timing_mark(cudaStream_t s, const char* name);
 int lidar_segment_ground_device(lvb_ctx* ctx, const float4* in, int n, double thr, float4* out, int* n_out);   // lidar.cu
+// the same without a read-back: the inlier count stays on the device at n_out_dev (0 when n < 3 or no plane is found), `out` holds
+// n records; nothing is waited for
+int lidar_segment_ground_device_async(lvb_ctx* ctx, const float4* in, int n, double thr, float4* out, int* n_out_dev);
+// every host wait on a context's stream goes through here and is counted in ctx->syncs (lvb_sync_count)
+int host_sync(lvb_ctx* ctx, cudaStream_t s);
 // The context's pinned staging area (lvb_ctx::stage_h), used by ba.cu (Stager) and icp.cu (lvb_icp_map_optimize_keyframe):
 //   stage_wait        wait until the last copy that read it has run (then it may be written)
 //   stage_grow        at least `need` bytes, the first `keep` bytes carried over (grows to max(2 x capacity, need, 4 MB))

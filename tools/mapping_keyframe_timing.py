@@ -1,13 +1,16 @@
-"""Per-keyframe wall time of Mapping::Optimize (mapping.cpp:147-185) on the device-resident map, two ways, alternated:
+"""Per-keyframe wall time of Mapping::Optimize (mapping.cpp:114-185) on the device-resident map, three ways, alternated:
 
   step  the existing entry points: lvb_icp_map_build x2, lvb_icp_scan_to_map (ground), the pose composed on the host,
         lvb_icp_scan_to_map (surf) from that pose, lvb_icp_map_append(NULL) x2 -- a host synchronisation after every LM pass
   call  lvb_icp_map_build x2, then lvb_icp_map_optimize_keyframe -- one synchronisation at the end
-  build lvb_icp_map_build x2 alone (the part both share)
+  one   lvb_icp_map_build_optimize_keyframe: the two builds and the registrations in one call, one synchronisation
+  build lvb_icp_map_build x2 alone (the part step and call share)
 
 Clouds are configs[2]-shaped: a 120 k-point scan against a 1 M-point map frame merged from three resident keyframes, for the surf and
 for the ground registration; the keyframe appended by each iteration is evicted again so that every iteration sees the same map.
-Prints one JSON line (min / median ms per keyframe, launches per keyframe, the GPU's name and power limit); --out also writes it there.
+The reference's own load is a few thousand voxel-filtered points per feature cloud: --scan 3000 --map 9000.
+Prints one JSON line (min / median ms per keyframe, launches and host synchronisations per keyframe, the GPU's name and power
+limit); --out also writes it there.
 
     python tools/mapping_keyframe_timing.py [--reps 20] [--warmup 3] [--scan 120000] [--map 1000000] [--out FILE]
 """
@@ -66,7 +69,7 @@ def main():
         fg.map_evict(3)
         fs.map_evict(3)
 
-    hs, hc, hb = handles(), handles(), handles()
+    hs, hc, ho, hb = handles(), handles(), handles(), handles()
 
     def step():
         fg, fs = hs
@@ -89,33 +92,46 @@ def main():
         evict(fg, fs)
         return p
 
+    def one():
+        fg, fs = ho
+        p, _, _, _ = backend.build_and_optimize_keyframe(fg, fs, [0, 1, 2], (g["cell_size"], s["cell_size"]), -1.0, 3, map_pose, guess,
+                                                         g["scan"], s["scan"], (g["weight"], s["weight"]), pw, (g["huber_a"], s["huber_a"]),
+                                                         (g["thr"], s["thr"]))
+        evict(fg, fs)
+        return p
+
     def build_only():
         build(*hb)
         ctx.synchronize()
 
-    variants = {"step": step, "call": call, "build": build_only}
-    launches = {}
+    variants = {"step": step, "call": call, "one": one, "build": build_only}
+    launches, syncs = {}, {}
     for name, fn in variants.items():
         for _ in range(a.warmup):
             fn()
-        n0 = ctx.launch_count()
+        n0, s0 = ctx.launch_count(), ctx.sync_count()
         fn()
         launches[name] = ctx.launch_count() - n0
-    pose_diff = float(np.max(np.abs(step() - call())))
+        syncs[name] = ctx.sync_count() - s0
+    ps, pc, po = step(), call(), one()
+    pose_diff = float(np.max(np.abs(ps - pc)))
+    pose_diff_one = float(np.max(np.abs(ps - po)))
     times = {k: [] for k in variants}
     order = list(variants)
     for r in range(a.reps):
-        for name in order[r % 3:] + order[:r % 3]:          # rotate who goes first
+        for name in order[r % len(order):] + order[:r % len(order)]:          # rotate who goes first
             ctx.synchronize()
             t0 = time.perf_counter()
             variants[name]()
             times[name].append((time.perf_counter() - t0) * 1e3)
     res = {"workload": "Mapping::Optimize per keyframe: %d-point ground + %d-point surf scans vs %d-point map frames (3 resident keyframes), "
                        "map builds included" % (a.scan, a.scan, a.map),
-           "gpu": gpu_info(), "reps": a.reps, "launches_per_keyframe": launches, "max_pose_difference_step_vs_call": pose_diff}
+           "gpu": gpu_info(), "reps": a.reps, "launches_per_keyframe": launches, "syncs_per_keyframe": syncs,
+           "max_pose_difference_step_vs_call": pose_diff, "max_pose_difference_step_vs_one": pose_diff_one}
     for k, v in times.items():
         res[k] = {"min_ms": float(np.min(v)), "median_ms": float(np.median(v)), "max_ms": float(np.max(v))}
     res["step_minus_call_median_ms"] = res["step"]["median_ms"] - res["call"]["median_ms"]
+    res["call_minus_one_median_ms"] = res["call"]["median_ms"] - res["one"]["median_ms"]
     line = json.dumps(res)
     print(line)
     if a.out:
