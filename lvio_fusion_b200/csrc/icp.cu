@@ -33,6 +33,7 @@ struct Grid {
     float minx, miny, minz, inv_cell, cell;   // cell = voxel edge = (search radius * 1.0001) / ring
     int gx, gy, gz;
     int ring;                                 // voxels per search radius: neighbours within the radius lie within `ring` voxels
+    int cbx, cby, cbz;                        // the coarse occupancy grid: blocks of 4 x 4 x 4 voxels
 };
 
 struct IcpState {
@@ -46,35 +47,32 @@ struct IcpState {
     double part[16];     // per-pass partial sums written by the linearize kernels (all-reduced when world > 1): [0..13] as acc, [14] candidate cost
 };
 
-struct IcpDev {
-    const float4* map;       // sorted by cell
-    const int* cell_start;
+// A map frame: its voxel grid and the sizes that follow from it, decided on the device by icp_map_grid_kernel from the cloud's bounding
+// box and read by every kernel that looks at the map.  The host keeps the copy it reads back after the build.
+struct MapDesc {
     Grid g;
-    int P;
+    int P;                       // map points; 0: an empty map frame (SegmentGround kept no point), which accepts no query
+    int ncell, ncb;              // gx * gy * gz; cbx * cby * cbz
+    int shift, cgx, cgy, cgz, nc;           // query visiting order (bind_scan): key granularity and its grid
+    int err;                     // 0, 1: no finite bounding box, 2: more than MAX_CELLS voxels at ring 1
+    int bbox[6];                 // the cloud's bounding box (ordered ints, icp_bbox_kernel's layout), uploaded with its seed values
+};
+
+struct IcpDev {
+    const float4* map;           // sorted by cell
+    const int* cell_start;
+    const int* coarse;           // occupancy of the coarse blocks of the map grid (1: holds points)
+    const MapDesc* m;            // the map frame's grid (device)
+    const float* tf;             // float[7]: the frame pose cast to float (association.cpp:287), in device memory
     const unsigned char* scan;   // device copy of the caller's records
     int K, stride;
-    float tf[7];                 // frame pose cast to float (association.cpp:287)
     float max_d2;
     double thr;
     unsigned char* accepted;
     float* pa;                   // 3 planes
     double* nrm;                 // 3 planes
     IcpState* st;
-    int rank, world;
     const int* order;            // query visiting order (spatially sorted) or nullptr
-    const int* coarse;           // occupancy of the 4 x 4 x 4-voxel blocks of the map grid (1: holds points)
-    int cbx, cby, cbz;           // its dimensions
-};
-
-// A map frame whose grid is decided on the device (lvb_icp_map_build_optimize_keyframe): what build_hash and bind_scan decide on the
-// host for the other entry points, written by icp_map_grid_kernel and read by the *_map kernels below.
-struct MapDesc {
-    Grid g;
-    int P;                       // map points (the surf merge: uploaded; the ground merge: SegmentGround's inlier count)
-    int ncell, cbx, cby, cbz, ncb;          // gx * gy * gz; coarse-block grid and its size
-    int shift, cgx, cgy, cgz, nc;           // query visiting order (bind_scan): key granularity and its grid
-    int err;                     // 0, 1: no finite bounding box, 2: more than MAX_CELLS voxels at ring 1
-    int bbox[6];                 // the cloud's bounding box (ordered ints, icp_bbox_kernel's layout), uploaded with its seed values
 };
 
 __device__ __forceinline__ float3 load_xyz(const unsigned char* base, int i, int stride) {
@@ -89,25 +87,25 @@ __device__ __forceinline__ void bbox_merge(float* mn, float* mx, int* bbox) {
         if ((threadIdx.x & 31) == 0) { atomicMin(&bbox[a], f2ord(mn[a])); atomicMax(&bbox[3 + a], f2ord(mx[a])); }
     }
 }
-__device__ __forceinline__ void bbox_points(const unsigned char* pts, int n, int stride, int* bbox) {
+// the bounding box of the map frame's m->P points into m->bbox (uploaded with its seed values)
+__global__ void icp_bbox_kernel(const unsigned char* pts, int stride, MapDesc* m) {
+    const int n = m->P;
     float mn[3] = {FLT_MAX, FLT_MAX, FLT_MAX}, mx[3] = {-FLT_MAX, -FLT_MAX, -FLT_MAX};
     for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
         const float3 p = load_xyz(pts, i, stride);
         mn[0] = fminf(mn[0], p.x); mn[1] = fminf(mn[1], p.y); mn[2] = fminf(mn[2], p.z);
         mx[0] = fmaxf(mx[0], p.x); mx[1] = fmaxf(mx[1], p.y); mx[2] = fmaxf(mx[2], p.z);
     }
-    bbox_merge(mn, mx, bbox);
+    bbox_merge(mn, mx, m->bbox);
 }
-__global__ void icp_bbox_kernel(const unsigned char* pts, int n, int stride, int* bbox /*6: min xyz, max xyz (ordered ints)*/) {
-    bbox_points(pts, n, stride, bbox);
-}
-// the same over the map frame of a MapDesc (its point count is known on the device only)
-__global__ void icp_bbox_map_kernel(const unsigned char* pts, int stride, MapDesc* m) { bbox_points(pts, m->P, stride, m->bbox); }
 
 __device__ __forceinline__ int cell_coord(float v, float mn, float inv_cell) { return (int)floorf((v - mn) * inv_cell); }
 __device__ __forceinline__ int clampi(int v, int lo, int hi) { return v < lo ? lo : (v > hi ? hi : v); }
 
-__device__ __forceinline__ void count_point(const unsigned char* pts, int i, int stride, const Grid& g, int* cell_of, int* counts, int* coarse, int cbx, int cby) {
+__global__ void icp_count_kernel(const unsigned char* pts, int stride, const MapDesc* m, int* cell_of, int* counts, int* coarse) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= m->P) return;
+    const Grid& g = m->g;
     const float3 p = load_xyz(pts, i, stride);
     const int ix = clampi(cell_coord(p.x, g.minx, g.inv_cell), 0, g.gx - 1);
     const int iy = clampi(cell_coord(p.y, g.miny, g.inv_cell), 0, g.gy - 1);
@@ -115,34 +113,16 @@ __device__ __forceinline__ void count_point(const unsigned char* pts, int i, int
     const int c = ix + g.gx * (iy + g.gy * iz);
     cell_of[i] = c;
     atomicAdd(&counts[c], 1);
-    coarse[(ix >> 2) + cbx * ((iy >> 2) + cby * (iz >> 2))] = 1;       // benign race: every writer stores 1
-}
-__global__ void icp_count_kernel(const unsigned char* pts, int n, int stride, Grid g, int* cell_of, int* counts, int* coarse, int cbx, int cby) {
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    count_point(pts, i, stride, g, cell_of, counts, coarse, cbx, cby);
-}
-__global__ void icp_count_map_kernel(const unsigned char* pts, int stride, const MapDesc* m, int* cell_of, int* counts, int* coarse) {
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= m->P) return;
-    count_point(pts, i, stride, m->g, cell_of, counts, coarse, m->cbx, m->cby);
+    coarse[(ix >> 2) + g.cbx * ((iy >> 2) + g.cby * (iz >> 2))] = 1;       // benign race: every writer stores 1
 }
 
-__device__ __forceinline__ void scatter_point(const unsigned char* pts, int i, int stride, const int* cell_of, const int* cell_start, int* fill, float4* sorted) {
+__global__ void icp_scatter_kernel(const unsigned char* pts, int stride, const MapDesc* m, const int* cell_of, const int* cell_start, int* fill, float4* sorted) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= m->P) return;
     const float3 p = load_xyz(pts, i, stride);
     const int c = cell_of[i];
     const int pos = cell_start[c] + atomicAdd(&fill[c], 1);
     sorted[pos] = make_float4(p.x, p.y, p.z, __int_as_float(i));
-}
-__global__ void icp_scatter_kernel(const unsigned char* pts, int n, int stride, const int* cell_of, const int* cell_start, int* fill, float4* sorted) {
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    scatter_point(pts, i, stride, cell_of, cell_start, fill, sorted);
-}
-__global__ void icp_scatter_map_kernel(const unsigned char* pts, int stride, const MapDesc* m, const int* cell_of, const int* cell_start, int* fill, float4* sorted) {
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= m->P) return;
-    scatter_point(pts, i, stride, cell_of, cell_start, fill, sorted);
 }
 
 // zero a[0..*n) (and b[0..*n) unless null): counters sized on the host by an upper bound, used up to the size the device decided
@@ -150,7 +130,7 @@ __global__ void icp_zero_map_kernel(int* a, int* b, const int* n) {
     const int cnt = *n;
     for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < cnt; i += gridDim.x * blockDim.x) { a[i] = 0; if (b) b[i] = 0; }
 }
-// the exclusive scan of lvb_cloud.cuh over the first *n entries (blocks launched for an upper bound of *n)
+// the exclusive scan of lvb_cloud.cuh over the first *n entries (a count the device decided; blocks launched for it or an upper bound)
 __global__ void scan_block_map_kernel(const int* in, int* out, const int* n, int* block_sums) {
     const int cnt = *n;
     if ((int)blockIdx.x * 1024 >= cnt) return;
@@ -177,30 +157,21 @@ __global__ void icp_transform_cloud_kernel(const unsigned char* __restrict__ in,
     for (int k = 3; k < stride / 4; ++k) dst[k] = src[k];
 }
 
-// Mapping::ToWorld (mapping.cpp:205-220) into the resident store: records of any stride -> packed (x, y, z, intensity) in the world frame
-__device__ __forceinline__ float3 to_world_point(const unsigned char* __restrict__ in, float4* __restrict__ out, int i, int stride, const float* __restrict__ tf7) {
-    float tf[7];
-    for (int k = 0; k < 7; ++k) tf[k] = tf7[k];
-    const float* src = reinterpret_cast<const float*>(in + (size_t)i * stride);
-    const float3 q = transform_f32(tf, make_float3(src[0], src[1], src[2]));
-    out[i] = make_float4(q.x, q.y, q.z, stride >= 16 ? src[3] : 0.0f);
-    return q;
-}
-__global__ void icp_to_world_kernel(const unsigned char* __restrict__ in, float4* __restrict__ out, int n, int stride, const float* __restrict__ tf7) {
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    to_world_point(in, out, i, stride, tf7);
-}
-// the same, and the bounding box of the stored cloud into bbox[6] (icp_bbox_kernel's min / max: equal to what it finds on `out`)
-__global__ void icp_to_world_bbox_kernel(const unsigned char* __restrict__ in, float4* __restrict__ out, int n, int stride, const float* __restrict__ tf7, int* bbox) {
+// Mapping::ToWorld (mapping.cpp:205-220) into the resident store: records of any stride -> packed (x, y, z, intensity) in the world
+// frame; with bbox, also the bounding box of the stored cloud into bbox[6] (icp_bbox_kernel's min / max: equal to what it finds on `out`)
+__global__ void icp_to_world_kernel(const unsigned char* __restrict__ in, float4* __restrict__ out, int n, int stride, const float* __restrict__ tf7, int* bbox) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     float mn[3] = {FLT_MAX, FLT_MAX, FLT_MAX}, mx[3] = {-FLT_MAX, -FLT_MAX, -FLT_MAX};
     if (i < n) {
-        const float3 q = to_world_point(in, out, i, stride, tf7);
+        float tf[7];
+        for (int k = 0; k < 7; ++k) tf[k] = tf7[k];
+        const float* src = reinterpret_cast<const float*>(in + (size_t)i * stride);
+        const float3 q = transform_f32(tf, make_float3(src[0], src[1], src[2]));
+        out[i] = make_float4(q.x, q.y, q.z, stride >= 16 ? src[3] : 0.0f);
         mn[0] = fminf(mn[0], q.x); mn[1] = fminf(mn[1], q.y); mn[2] = fminf(mn[2], q.z);
         mx[0] = fmaxf(mx[0], q.x); mx[1] = fmaxf(mx[1], q.y); mx[2] = fmaxf(mx[2], q.z);
     }
-    bbox_merge(mn, mx, bbox);
+    if (bbox) bbox_merge(mn, mx, bbox);
 }
 
 struct Best3 { float d[3]; int i[3]; int p[3]; };   // d2, original index, position in the sorted array
@@ -240,17 +211,17 @@ __device__ __forceinline__ void scan_voxel(const IcpDev& d, const Grid& g, float
     }
 }
 
-__device__ __forceinline__ Best3 knn3_query(const IcpDev& d, float3 q) {
+// g: the map frame's grid, loaded from its MapDesc once per thread
+__device__ __forceinline__ Best3 knn3_query(const IcpDev& d, const Grid& g, float3 q) {
     Best3 b;
     b.d[0] = b.d[1] = b.d[2] = INFINITY; b.i[0] = b.i[1] = b.i[2] = 0x7fffffff; b.p[0] = b.p[1] = b.p[2] = -1;
-    const Grid& g = d.g;
     const int cx = cell_coord(q.x, g.minx, g.inv_cell), cy = cell_coord(q.y, g.miny, g.inv_cell), cz = cell_coord(q.z, g.minz, g.inv_cell);
     Occ occ; occ.mask = 0u; occ.bx = cx >> 2; occ.by = cy >> 2; occ.bz = cz >> 2;       // (ring <= 4 voxels: every probed voxel lies in these 27 blocks)
 #pragma unroll
     for (int k = 0; k < 27; ++k) {                  // 27 independent loads, one round trip
         const int x = occ.bx + k % 3 - 1, y = occ.by + (k / 3) % 3 - 1, z = occ.bz + k / 9 - 1;
-        const bool in = x >= 0 && y >= 0 && z >= 0 && x < d.cbx && y < d.cby && z < d.cbz;
-        if (in && __ldg(&d.coarse[x + d.cbx * (y + d.cby * z)])) occ.mask |= 1u << k;
+        const bool in = x >= 0 && y >= 0 && z >= 0 && x < g.cbx && y < g.cby && z < g.cbz;
+        if (in && __ldg(&d.coarse[x + g.cbx * (y + g.cby * z)])) occ.mask |= 1u << k;
     }
     scan_voxel(d, g, q, cx, cy, cz, b, occ);
     for (int r = 1; r <= g.ring; ++r) {
@@ -281,33 +252,24 @@ __device__ __forceinline__ Best3 knn3_query(const IcpDev& d, float3 q) {
 // every ring): 0.57 ms -- the lanes prune with their own looser bounds and scan more voxels than the chain they shorten; runs only for
 // the face rows of the outer rings (r >= 2): 0.57 ms.  The kernel takes ~0.47 - 0.50 ms whether a rank holds 120 k, 60 k or 30 k of
 // the queries (round-2 runs at 1 / 2 / 4 GPUs): its duration is set by its slowest warps, not by the query count.
-__device__ __forceinline__ void query_key(const IcpDev& d, const float* tf, int shift, int cgx, int cgy, int cgz, int* __restrict__ key, int* __restrict__ counts) {
+__device__ __forceinline__ float3 query_point(const IcpDev& d, int i) {
+    float tf[7];
+    for (int k = 0; k < 7; ++k) tf[k] = d.tf[k];
+    return transform_f32(tf, load_xyz(d.scan, i, d.stride));
+}
+__global__ void icp_query_key_kernel(IcpDev d, int* __restrict__ key, int* __restrict__ counts) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= d.K) return;
-    const float3 q = transform_f32(tf, load_xyz(d.scan, i, d.stride));
-    const Grid& g = d.g;
+    const float3 q = query_point(d, i);
+    const MapDesc* m = d.m;
+    const Grid g = m->g;
+    const int shift = m->shift;
     const int ix = clampi(cell_coord(q.x, g.minx, g.inv_cell), 0, g.gx - 1) >> shift;
     const int iy = clampi(cell_coord(q.y, g.miny, g.inv_cell), 0, g.gy - 1) >> shift;
     const int iz = clampi(cell_coord(q.z, g.minz, g.inv_cell), 0, g.gz - 1) >> shift;
-    const int c = ix + cgx * (iy + cgy * iz);
+    const int c = ix + m->cgx * (iy + m->cgy * iz);
     key[i] = c;
     atomicAdd(&counts[c], 1);
-}
-__global__ void icp_query_key_kernel(IcpDev d, int shift, int cgx, int cgy, int cgz, int* __restrict__ key, int* __restrict__ counts) {
-    query_key(d, d.tf, shift, cgx, cgy, cgz, key, counts);
-}
-// the same with the query transform read from device memory (float[7], written by an earlier kernel: lvb_icp_map_optimize_keyframe)
-__global__ void icp_query_key_dev_tf_kernel(IcpDev d, const float* __restrict__ tf7, int shift, int cgx, int cgy, int cgz, int* __restrict__ key, int* __restrict__ counts) {
-    float tf[7];
-    for (int k = 0; k < 7; ++k) tf[k] = tf7[k];
-    query_key(d, tf, shift, cgx, cgy, cgz, key, counts);
-}
-// ... and with the map grid and the key granularity of a MapDesc
-__global__ void icp_query_key_map_kernel(IcpDev d, const float* __restrict__ tf7, const MapDesc* __restrict__ m, int* __restrict__ key, int* __restrict__ counts) {
-    float tf[7];
-    for (int k = 0; k < 7; ++k) tf[k] = tf7[k];
-    d.g = m->g;
-    query_key(d, tf, m->shift, m->cgx, m->cgy, m->cgz, key, counts);
 }
 __global__ void icp_query_scatter_kernel(int n, const int* __restrict__ key, const int* __restrict__ start, int* __restrict__ fill, int* __restrict__ order) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -320,20 +282,25 @@ __global__ void __launch_bounds__(ITPB) icp_knn_kernel(IcpDev d, int* __restrict
     const int t = blockIdx.x * ITPB + threadIdx.x;
     if (t >= d.K) return;
     const int i = d.order ? d.order[t] : t;
-    const float3 q = transform_f32(d.tf, load_xyz(d.scan, i, d.stride));
-    const Best3 b = knn3_query(d, q);
+    const float3 q = query_point(d, i);
+    const Grid g = d.m->g;               // loaded after the transform: not held across its division and square root
+    const Best3 b = knn3_query(d, g, q);
     for (int j = 0; j < 3; ++j) { idx_out[3 * i + j] = b.i[j]; d2_out[3 * i + j] = b.d[j]; }
 }
 
-// K8: transform + 3-NN + gate (association.cpp:296-300) + plane constants (lidar_error.hpp:13-18)
-__device__ __forceinline__ void associate_query(const IcpDev& d, const float* tf) {
+// K8: transform + 3-NN + gate (association.cpp:296-300) + plane constants (lidar_error.hpp:13-18).  An empty map frame (P = 0:
+// SegmentGround kept no point) accepts no query.
+__global__ void __launch_bounds__(ITPB) icp_associate_kernel(IcpDev d) {
     const int t = blockIdx.x * ITPB + threadIdx.x;
     if (t >= d.K) return;
     const int i = d.order ? d.order[t] : t;
-    const float3 q = transform_f32(tf, load_xyz(d.scan, i, d.stride));
-    const Best3 b = knn3_query(d, q);
+    const float3 q = query_point(d, i);
+    const int P = d.m->P;
+    if (P == 0) { d.accepted[i] = 0; return; }
+    const Grid g = d.m->g;
+    const Best3 b = knn3_query(d, g, q);
     int ok = 1;
-    for (int j = 0; j < 3; ++j) if (!(b.i[j] >= 0 && b.i[j] < d.P && (double)b.d[j] < d.thr)) ok = 0;
+    for (int j = 0; j < 3; ++j) if (!(b.i[j] >= 0 && b.i[j] < P && (double)b.d[j] < d.thr)) ok = 0;
     d.accepted[i] = (unsigned char)ok;
     if (!ok) return;
     const float4 a = d.map[b.p[0]], bb = d.map[b.p[1]], c = d.map[b.p[2]];
@@ -341,31 +308,11 @@ __device__ __forceinline__ void associate_query(const IcpDev& d, const float* tf
     d.pa[i] = a.x; d.pa[d.K + i] = a.y; d.pa[2 * d.K + i] = a.z;
     d.nrm[i] = n.x; d.nrm[d.K + i] = n.y; d.nrm[2 * (size_t)d.K + i] = n.z;
 }
-__global__ void __launch_bounds__(ITPB) icp_associate_kernel(IcpDev d) { associate_query(d, d.tf); }
-// the same with the query transform read from device memory (see icp_query_key_dev_tf_kernel)
-__global__ void __launch_bounds__(ITPB) icp_associate_dev_tf_kernel(IcpDev d, const float* __restrict__ tf7) {
-    float tf[7];
-    for (int k = 0; k < 7; ++k) tf[k] = tf7[k];
-    associate_query(d, tf);
-}
-// ... and with the map frame of a MapDesc; an empty one (SegmentGround kept no point) accepts no query
-__global__ void __launch_bounds__(ITPB) icp_associate_map_kernel(IcpDev d, const float* __restrict__ tf7, const MapDesc* __restrict__ m) {
-    if (m->P == 0) {
-        const int t = blockIdx.x * ITPB + threadIdx.x;
-        if (t < d.K) d.accepted[t] = 0;
-        return;
-    }
-    float tf[7];
-    for (int k = 0; k < 7; ++k) tf[k] = tf7[k];
-    d.g = m->g; d.P = m->P; d.cbx = m->cbx; d.cby = m->cby; d.cbz = m->cbz;
-    associate_query(d, tf);
-}
 
-// build_hash's grid and bind_scan's key granularity on one thread, from the bounding box in m->bbox: the same float / double
-// operations in the same order, each rounded on its own (no contraction), so the voxels, the neighbours and the query visiting
-// order are those of the step-by-step path.  An empty or failed map frame gets a one-voxel grid and P = 0, which every *_map kernel
-// treats as "nothing to do".
-__global__ void icp_map_grid_kernel(MapDesc* m, float cell_size, int forced_shift) {
+// The voxel grid of a map frame and the key granularity of its queries' visiting order, on one thread, from the bounding box in
+// m->bbox.  Every float / double operation is rounded on its own (no contraction), so the grid does not depend on how this file is
+// compiled.  An empty or failed map frame gets a one-voxel grid and P = 0, which every kernel treats as "nothing to do".
+__global__ void icp_map_grid_kernel(MapDesc* m, float cell_size) {
     Grid g;
     int P = m->P, err = 0;
     double dx = 1, dy = 1, dz = 1;
@@ -376,6 +323,9 @@ __global__ void icp_map_grid_kernel(MapDesc* m, float cell_size, int forced_shif
         const float wx = __fsub_rn(mx, g.minx), wy = __fsub_rn(my, g.miny), wz = __fsub_rn(mz, g.minz);
         if (!(mx >= g.minx) || !(my >= g.miny) || !(mz >= g.minz) || !isfinite(wx) || !isfinite(wy) || !isfinite(wz)) err = 1;
         else {
+            // The voxel edge is (radius * 1.0001) / ring: the hair of slack guarantees that float rounding of the voxel coordinate
+            // never separates two points closer than the radius by more than `ring` voxels.  ring = 4 unless the bounding box would
+            // need more than MAX_CELLS voxels.
             int ring = 4;
             for (;; ring >>= 1) {
                 g.cell = __fdiv_rn(__fmul_rn(cell_size, 1.0001f), (float)ring); g.inv_cell = __fdiv_rn(1.0f, g.cell);
@@ -393,13 +343,15 @@ __global__ void icp_map_grid_kernel(MapDesc* m, float cell_size, int forced_shif
         g.minx = g.miny = g.minz = 0.0f; g.cell = g.inv_cell = 1.0f; g.ring = 1;
     }
     g.gx = (int)dx; g.gy = (int)dy; g.gz = (int)dz;
+    g.cbx = (g.gx + 3) >> 2; g.cby = (g.gy + 3) >> 2; g.cbz = (g.gz + 3) >> 2;
     m->g = g; m->P = P; m->err = err;
     m->ncell = g.gx * g.gy * g.gz;
-    m->cbx = (g.gx + 3) >> 2; m->cby = (g.gy + 3) >> 2; m->cbz = (g.gz + 3) >> 2;
-    m->ncb = m->cbx * m->cby * m->cbz;
+    m->ncb = g.cbx * g.cby * g.cbz;
+    // key granularity of the query visiting order: blocks of 2 x 2 x 2 voxels (measured on configs[2], association kernel: 4 x 4 x 4
+    // blocks 0.51 ms, 2 x 2 x 2 0.44 ms, single voxels 0.50 ms plus a slower sort) -- coarser only when the grid would need more
+    // than 8 M counters
     int shift = 1;
-    while (forced_shift < 0 && __dmul_rn(__dmul_rn((double)((g.gx >> shift) + 1), (double)((g.gy >> shift) + 1)), (double)((g.gz >> shift) + 1)) > 8.0e6) ++shift;
-    if (forced_shift >= 0) shift = forced_shift;
+    while (__dmul_rn(__dmul_rn((double)((g.gx >> shift) + 1), (double)((g.gy >> shift) + 1)), (double)((g.gz >> shift) + 1)) > 8.0e6) ++shift;
     const int rnd = (1 << shift) - 1;
     m->shift = shift;
     m->cgx = (g.gx + rnd) >> shift; m->cgy = (g.gy + rnd) >> shift; m->cgz = (g.gz + rnd) >> shift;
@@ -534,15 +486,18 @@ __global__ void icp_post_kernel(IcpState* st) {
     }
 }
 
-// ---- Mapping::Optimize for one keyframe on the device (lvb_icp_map_optimize_keyframe): the pose arithmetic between the two
-// registrations.  FP64 on one thread; every product and sum is rounded on its own (__dmul_rn / __dadd_rn / __dsub_rn: no FMA
-// contraction), in the operation order of the host formulas cited at each function.  Poses are [qx qy qz qw tx ty tz].
-struct KfBlock {             // the call's device state, read back with one copy at its end
+// ---- Mapping::Optimize for one keyframe on the device (lvb_icp_map_optimize_keyframe, lvb_icp_map_build_optimize_keyframe): the
+// pose arithmetic between the two registrations.  FP64 on one thread; every product and sum is rounded on its own (__dmul_rn /
+// __dadd_rn / __dsub_rn: no FMA contraction), in the operation order of the host formulas cited at each function.  Poses are
+// [qx qy qz qw tx ty tz].
+struct KfBlock {             // the call's device state, uploaded and read back with one copy each
     IcpState st[2];          // [0] ground (mode 0), [1] surf (mode 1)
     double map_pose[7];      // map_frame->pose                                   (uploaded)
     double pose[7];          // frame->pose: the incoming one, then after each registration
     double rpyxyz[6];
     float tf[8];             // pose.cast<float>(): the query transform of the next association, then of ToWorld
+    MapDesc map[2];          // [0] ground, [1] surf map frame: the handles' (uploaded), or built in the call; P = 0: no registration
+    int out_bbox[2][6];      // bounding boxes of the two clouds ToWorld stores (lvb_icp_map_build_optimize_keyframe)
 };
 struct KfSeed {              // what ScanToMapWith* put in each problem (association.cpp:270-384) and the solver options
     lvb_solve_options o;
@@ -637,21 +592,15 @@ __device__ __forceinline__ void kf_seed(KfBlock* b, int seed, const KfSeed& p) {
     for (int k = 0; k < 3; ++k) { s.x[k] = b->rpyxyz[c_free[seed][k]]; s.cand[k] = s.x[k]; s.prior_target[k] = s.x[k]; }
     s.prior_w = p.prior_w; s.huber_a = p.huber_a[seed]; s.weight = p.weight[seed];
 }
+// A registration whose map frame is empty (map[m].P == 0: SegmentGround kept no point in the in-call build) is not solved -- its LM
+// passes return at once -- and leaves rpyxyz and the pose as they were, as BuildMapFrame's failure on that side does in the
+// step-by-step path.
 __global__ void icp_kf_pose_kernel(KfBlock* b, int from, int seed, KfSeed p) {
-    kf_pose_update(b, from);
+    if (from < 0 || b->map[from].P > 0) kf_pose_update(b, from);
     for (int k = 0; k < 7; ++k) b->tf[k] = __double2float_rn(b->pose[k]);
     if (seed < 0) return;
     kf_seed(b, seed, p);
-}
-// The same when the map frames were built in the same call (lvb_icp_map_build_optimize_keyframe): a registration whose map frame is
-// empty (maps[m].P == 0: SegmentGround kept no point) is not solved -- its LM passes return at once -- and leaves rpyxyz and the pose
-// as they were, as BuildMapFrame's failure on that side does in the step-by-step path.
-__global__ void icp_kf_pose_map_kernel(KfBlock* b, int from, int seed, KfSeed p, const MapDesc* maps) {
-    if (from < 0 || maps[from].P > 0) kf_pose_update(b, from);
-    for (int k = 0; k < 7; ++k) b->tf[k] = __double2float_rn(b->pose[k]);
-    if (seed < 0) return;
-    kf_seed(b, seed, p);
-    if (maps[seed].P == 0) b->st[seed].lm.done = 1;
+    if (b->map[seed].P == 0) b->st[seed].lm.done = 1;
 }
 
 }  // namespace
@@ -660,13 +609,15 @@ __global__ void icp_kf_pose_map_kernel(KfBlock* b, int from, int seed, KfSeed p,
 struct lvb_icp {
     lvb_ctx* ctx = nullptr;
     bool have_map = false;
-    int P = 0;
     float cell_size = 0;
-    Grid grid;
+    MapDesc map;                 // the current map frame's descriptor, as read back after its build
+    // What the kernels of a set_map / lvb_icp_map_build build, and of a knn3 / eval / scan_to_map call, read on the device: the
+    // descriptor (the build's working copy, then `map` uploaded with each call's scan) and the query transform
+    struct Frame { MapDesc map; float tf[8]; };
+    DevBuf<Frame> frame;
     DevBuf<unsigned char> map_raw, scan_raw, accepted;
     DevBuf<float4> map_sorted;
-    DevBuf<int> cell_of, counts, cell_start, fill, block_sums, bbox, total, coarse;
-    int cbx = 0, cby = 0, cbz = 0;
+    DevBuf<int> cell_of, counts, cell_start, fill, block_sums, total, coarse;
     DevBuf<float> pa;
     DevBuf<double> nrm, eval_r, eval_J;
     DevBuf<int> knn_idx;
@@ -679,12 +630,12 @@ struct lvb_icp {
     struct Segment { long long key; DevBuf<float4>* pts; int n; bool has_bbox = false; float lo[3], hi[3]; };
     std::vector<Segment> segments;
     DevBuf<float4> merged, merged2;
-    // lvb_icp_map_build_optimize_keyframe builds the map frame here and swaps it in only when the device found no failure
+    // every build writes its map frame here; it is swapped in only when the build succeeded
     DevBuf<float4> nx_sorted;
     DevBuf<int> nx_cell_start, nx_coarse;
     int scan_n = 0, scan_stride = 0;          // the scan of the last upload_scan (reusable by lvb_icp_map_append)
     const unsigned char* scan_dev = nullptr;  // where that scan lies: scan_raw, or this handle's part of kf_arena
-    // lvb_icp_map_optimize_keyframe's upload: [KfBlock | ground scan | surf scan] in one allocation, held by both handles of the call
+    // the keyframe calls' upload: [KfBlock | ground scan | surf scan] in one allocation, held by both handles of the call
     // so that either one's scan stays valid for lvb_icp_map_append(NULL) until that handle uploads another scan
     std::shared_ptr<DevBuf<unsigned char>> kf_arena;
     ~lvb_icp() { for (auto& sg : segments) delete sg.pts; }
@@ -699,72 +650,150 @@ static int icheck(const char* what) {
     if (e != cudaSuccess) { set_error("kernel launch failed in %s: %s", what, cudaGetErrorString(e)); return LVB_ERR_CUDA; }
     return LVB_OK;
 }
+// exchange two buffers' ownership (DevBuf has no move operations)
+template <class T> static void swap_buf(DevBuf<T>& a, DevBuf<T>& b) { std::swap(a.p, b.p); std::swap(a.n, b.n); std::swap(a.s, b.s); std::swap(a.view, b.view); }
 
-// key granularity of the query visiting order: blocks of 2 x 2 x 2 voxels (measured on configs[2], association kernel: 4 x 4 x 4
-// blocks 0.51 ms, 2 x 2 x 2 0.44 ms, single voxels 0.50 ms plus a slower sort) -- coarser only when the grid would need more than
-// 8 M counters; env LVB_ICP_SORT_SHIFT forces one (A/B)
-static int sort_shift_forced() {
-    static const int forced = getenv("LVB_ICP_SORT_SHIFT") ? atoi(getenv("LVB_ICP_SORT_SHIFT")) : -1;
-    return forced;
+static void bbox_seed(int* b) {       // icp_bbox_kernel's starting values: min = FLT_MAX, max = -FLT_MAX as ordered ints
+    float big = FLT_MAX, small = -FLT_MAX; int bi, si; memcpy(&bi, &big, 4); memcpy(&si, &small, 4);
+    const int so = si >= 0 ? si : si ^ 0x7fffffff;
+    b[0] = b[1] = b[2] = bi; b[3] = b[4] = b[5] = so;
+}
+// a map frame's descriptor as uploaded before its build: P points (or 0 when an earlier kernel writes the count) and the box seeds
+static MapDesc desc_seed(int P) {
+    MapDesc m;
+    memset(&m, 0, sizeof(m));
+    m.P = P;
+    bbox_seed(m.bbox);
+    return m;
+}
+// the failure icp_map_grid_kernel reported in a map frame's descriptor
+static int grid_error(const MapDesc& m, const char* fn, const char* side) {
+    if (m.err == 1) { set_error("%s: map cloud has no finite bounding box", fn); return LVB_ERR_INVALID; }
+    if (m.err) { set_error("%s: voxel grid of the %smap frame exceeds %d cells; increase cell_size or crop the map", fn, side, (int)MAX_CELLS); return LVB_ERR_UNSUPPORTED; }
+    return LVB_OK;
 }
 
-// the association buffers of the n queries at d_scan and everything of d but the map grid
-static int bind_buffers(lvb_icp* h, const unsigned char* d_scan, int n, int stride, float max_d2, double thr, IcpDev& d) {
+// The association buffers and the visiting order of the n queries at d_scan (device, stride bytes each), against the map frame whose
+// descriptor lies at m and with the query transform at tf (both device); d.map, d.cell_start and d.coarse are the caller's.  The nc
+// counters of the sort are cleared with cudaMemsetAsync when nc is the map frame's own count (exact), and by a kernel up to m->nc when
+// nc only bounds it (a map frame built in the same call).
+static int bind_scan(lvb_icp* h, const unsigned char* d_scan, int n, int stride, const MapDesc* m, const float* tf, float max_d2, double thr,
+                     size_t nc, bool exact, IcpDev& d) {
+    cudaStream_t s = h->ctx->stream;
     h->scan_n = n; h->scan_stride = stride; h->scan_dev = d_scan;
     LVB_TRY(h->accepted.ensure(std::max(1, n)));
     LVB_TRY(h->pa.ensure((size_t)std::max(1, n) * 3));
     LVB_TRY(h->nrm.ensure((size_t)std::max(1, n) * 3));
     LVB_TRY(h->st.ensure(1));
+    d.m = m; d.tf = tf;
     d.scan = d_scan; d.K = n; d.stride = stride;
     d.max_d2 = max_d2; d.thr = thr;
     d.accepted = h->accepted.p; d.pa = h->pa.p; d.nrm = h->nrm.p; d.st = h->st.p;
-    d.rank = h->ctx->rank; d.world = h->ctx->world;
     d.order = nullptr;
-    return LVB_OK;
-}
-
-// The association buffers and the visiting order of the n queries at d_scan (device, stride bytes each).  The query transform is
-// d.tf (set by the caller), or, when tf_dev is given, the float[7] at tf_dev in device memory.
-static int bind_scan(lvb_icp* h, const unsigned char* d_scan, int n, int stride, const float* tf_dev, float max_d2, double thr, IcpDev& d) {
-    cudaStream_t s = h->ctx->stream;
-    LVB_TRY(bind_buffers(h, d_scan, n, stride, max_d2, thr, d));
-    d.map = h->map_sorted.p; d.cell_start = h->cell_start.p; d.g = h->grid; d.P = h->P;
-    d.coarse = h->coarse.p; d.cbx = h->cbx; d.cby = h->cby; d.cbz = h->cbz;
     if (n >= 4096) {       // spatial visiting order: counting sort of the queries by coarse voxel block
-        const Grid& g = h->grid;
-        const int forced = sort_shift_forced();
-        int shift = 1;
-        while (forced < 0 && (double)((g.gx >> shift) + 1) * ((g.gy >> shift) + 1) * ((g.gz >> shift) + 1) > 8.0e6) ++shift;
-        if (forced >= 0) shift = forced;
-        const int rnd = (1 << shift) - 1;
-        const int cgx = (g.gx + rnd) >> shift, cgy = (g.gy + rnd) >> shift, cgz = (g.gz + rnd) >> shift;
-        const int nc = cgx * cgy * cgz, nb = (nc + 1023) / 1024;
+        const int nb = inblk(nc, 1024);
         LVB_TRY(h->q_key.ensure(n)); LVB_TRY(h->q_order.ensure(n)); LVB_TRY(h->q_counts.ensure(nc)); LVB_TRY(h->q_fill.ensure(nc));
-        LVB_TRY(h->q_start.ensure((size_t)nc + 1)); LVB_TRY(h->q_sums.ensure(nb)); LVB_TRY(h->q_total.ensure(1));
-        LVB_CUDA(cudaMemsetAsync(h->q_counts.p, 0, (size_t)nc * sizeof(int), s));
-        LVB_CUDA(cudaMemsetAsync(h->q_fill.p, 0, (size_t)nc * sizeof(int), s));
-        if (tf_dev) ILAUNCH(h, icp_query_key_dev_tf_kernel, (n + 255) / 256, 256, d, tf_dev, shift, cgx, cgy, cgz, h->q_key.p, h->q_counts.p);
-        else ILAUNCH(h, icp_query_key_kernel, (n + 255) / 256, 256, d, shift, cgx, cgy, cgz, h->q_key.p, h->q_counts.p);
-        ILAUNCH(h, scan_block_kernel, nb, 1024, h->q_counts.p, h->q_start.p, nc, h->q_sums.p);
-        ILAUNCH(h, scan_sums_kernel, 1, 1024, h->q_sums.p, nb, h->q_total.p);
-        ILAUNCH(h, scan_add_kernel, nb, 1024, h->q_start.p, nc, h->q_sums.p, h->q_start.p + nc, h->q_total.p);
-        ILAUNCH(h, icp_query_scatter_kernel, (n + 255) / 256, 256, n, h->q_key.p, h->q_start.p, h->q_fill.p, h->q_order.p);
+        LVB_TRY(h->q_start.ensure(nc + 1)); LVB_TRY(h->q_sums.ensure(nb)); LVB_TRY(h->q_total.ensure(1));
+        if (exact) {
+            LVB_CUDA(cudaMemsetAsync(h->q_counts.p, 0, nc * sizeof(int), s));
+            LVB_CUDA(cudaMemsetAsync(h->q_fill.p, 0, nc * sizeof(int), s));
+        } else ILAUNCH(h, icp_zero_map_kernel, std::min(inblk(nc, 256), 8 * h->ctx->sm_count), 256, h->q_counts.p, h->q_fill.p, &m->nc);
+        ILAUNCH(h, icp_query_key_kernel, inblk(n, 256), 256, d, h->q_key.p, h->q_counts.p);
+        ILAUNCH(h, scan_block_map_kernel, nb, 1024, h->q_counts.p, h->q_start.p, &m->nc, h->q_sums.p);
+        ILAUNCH(h, scan_sums_map_kernel, 1, 1024, h->q_sums.p, &m->nc, h->q_total.p);
+        ILAUNCH(h, scan_add_map_kernel, nb, 1024, h->q_start.p, &m->nc, h->q_sums.p, h->q_total.p);
+        ILAUNCH(h, icp_query_scatter_kernel, inblk(n, 256), 256, n, h->q_key.p, h->q_start.p, h->q_fill.p, h->q_order.p);
         d.order = h->q_order.p;
     }
     return LVB_OK;
 }
 
+// knn3 / eval / scan_to_map: the scan, the current map frame's descriptor and the frame pose cast to float go to the device on the
+// context's stream
 static int upload_scan(lvb_icp* h, const void* scan, int n, int stride, const double* frame_pose, float max_d2, double thr, IcpDev& d) {
     if (!h->have_map) { set_error("set_map first"); return LVB_ERR_STATE; }
     if (n < 0 || stride < 12 || (stride & 3) || (n && !scan)) { set_error("bad scan arguments"); return LVB_ERR_INVALID; }
-    LVB_TRY(h->scan_raw.upload((const unsigned char*)scan, (size_t)n * stride, h->ctx->stream));
+    cudaStream_t s = h->ctx->stream;
+    LVB_TRY(h->scan_raw.upload((const unsigned char*)scan, (size_t)n * stride, s));
     h->kf_arena.reset();
-    for (int i = 0; i < 7; ++i) d.tf[i] = (float)frame_pose[i];
-    return bind_scan(h, h->scan_raw.p, n, stride, nullptr, max_d2, thr, d);
+    lvb_icp::Frame f;
+    f.map = h->map;
+    for (int i = 0; i < 7; ++i) f.tf[i] = (float)frame_pose[i];
+    f.tf[7] = 0.0f;
+    LVB_TRY(h->frame.upload(&f, 1, s));
+    d.map = h->map_sorted.p; d.cell_start = h->cell_start.p; d.coarse = h->coarse.p;
+    return bind_scan(h, h->scan_raw.p, n, stride, &h->frame.p->map, h->frame.p->tf, max_d2, thr, h->map.nc, true, d);
 }
 
-// exchange two buffers' ownership (DevBuf has no move operations)
-template <class T> static void swap_buf(DevBuf<T>& a, DevBuf<T>& b) { std::swap(a.p, b.p); std::swap(a.n, b.n); std::swap(a.s, b.s); std::swap(a.view, b.view); }
+// one LM pass on d.st: linearise at x, solve, the cost at the candidate, accept or reject (the partial sums all-reduced over the ranks)
+static int enqueue_pass(lvb_icp* h, const IcpDev& d) {
+    lvb_ctx* ctx = h->ctx;
+    const int lin_blocks = std::max(1, std::min(inblk(d.K, ITPB), 4 * ctx->sm_count));
+    ILAUNCH(h, icp_linearize_kernel<0>, lin_blocks, ITPB, d);
+    if (ctx->world > 1) LVB_TRY(comm_allreduce_sum_f64(ctx, d.st->part, 14));
+    ILAUNCH(h, icp_solve_kernel, 1, 1, d.st);
+    ILAUNCH(h, icp_linearize_kernel<1>, lin_blocks, ITPB, d);
+    if (ctx->world > 1) LVB_TRY(comm_allreduce_sum_f64(ctx, d.st->part + 14, 1));
+    ILAUNCH(h, icp_post_kernel, 1, 1, d.st);
+    return LVB_OK;
+}
+
+// The counting sort by voxel key of the map frame at m (device; icp_map_grid_kernel has decided its grid): its m->P records (stride
+// bytes each, at most n) at d_points into the nx_* buffers.  The cells / coarse counters are cleared with cudaMemsetAsync when they
+// are the map frame's own counts (exact), and by kernels up to m->ncell / m->ncb when they only bound them (map_bound).
+static int enqueue_hash(lvb_icp* h, const unsigned char* d_points, int n, int stride, const MapDesc* m, size_t cells, size_t coarse, bool exact) {
+    lvb_ctx* ctx = h->ctx;
+    cudaStream_t s = ctx->stream;
+    const int nb = inblk(cells, 1024);
+    LVB_TRY(h->cell_of.ensure(n)); LVB_TRY(h->counts.ensure(cells)); LVB_TRY(h->fill.ensure(cells));
+    LVB_TRY(h->nx_cell_start.ensure(cells + 1)); LVB_TRY(h->nx_sorted.ensure(n)); LVB_TRY(h->nx_coarse.ensure(coarse));
+    LVB_TRY(h->block_sums.ensure(nb)); LVB_TRY(h->total.ensure(1));
+    if (exact) {
+        LVB_CUDA(cudaMemsetAsync(h->counts.p, 0, cells * sizeof(int), s));
+        LVB_CUDA(cudaMemsetAsync(h->fill.p, 0, cells * sizeof(int), s));
+        LVB_CUDA(cudaMemsetAsync(h->nx_coarse.p, 0, coarse * sizeof(int), s));
+    } else {
+        ILAUNCH(h, icp_zero_map_kernel, std::min(inblk(cells, 256), 8 * ctx->sm_count), 256, h->counts.p, h->fill.p, &m->ncell);
+        ILAUNCH(h, icp_zero_map_kernel, std::min(inblk(coarse, 256), 8 * ctx->sm_count), 256, h->nx_coarse.p, (int*)nullptr, &m->ncb);
+    }
+    ILAUNCH(h, icp_count_kernel, inblk(n, 256), 256, d_points, stride, m, h->cell_of.p, h->counts.p, h->nx_coarse.p);
+    ILAUNCH(h, scan_block_map_kernel, nb, 1024, h->counts.p, h->nx_cell_start.p, &m->ncell, h->block_sums.p);
+    ILAUNCH(h, scan_sums_map_kernel, 1, 1024, h->block_sums.p, &m->ncell, h->total.p);
+    ILAUNCH(h, scan_add_map_kernel, nb, 1024, h->nx_cell_start.p, &m->ncell, h->block_sums.p, h->total.p);
+    ILAUNCH(h, icp_scatter_kernel, inblk(n, 256), 256, d_points, stride, m, h->cell_of.p, h->nx_cell_start.p, h->fill.p, h->nx_sorted.p);
+    return icheck("map frame build");
+}
+
+// set_map / lvb_icp_map_build: upload the descriptor's seed, P points, before the build (P = 0 when SegmentGround writes the count)
+static int seed_frame(lvb_icp* h, int P) {
+    LVB_TRY(h->frame.ensure(1));
+    const MapDesc seed = desc_seed(P);
+    LVB_CUDA(cudaMemcpyAsync(&h->frame.p->map, &seed, sizeof(seed), cudaMemcpyHostToDevice, h->ctx->stream));
+    return LVB_OK;
+}
+
+// Voxel hash of the map frame at d_points (device, stride bytes per record, at most n of them: the count lies in the seeded
+// descriptor): bounding box and grid on the device, the descriptor read back (the one synchronisation before the sort), the
+// counting sort sized by it, and the new map frame swapped in on success -- a failed build leaves the previous one in place.
+static int build_map(lvb_icp* h, const unsigned char* d_points, int n, int stride, float cell_size, const char* fn, int* n_points) {
+    lvb_ctx* ctx = h->ctx;
+    cudaStream_t s = ctx->stream;
+    MapDesc* md = &h->frame.p->map;
+    ILAUNCH(h, icp_bbox_kernel, std::min(1024, inblk(n, 256)), 256, d_points, stride, md);
+    ILAUNCH(h, icp_map_grid_kernel, 1, 1, md, cell_size);
+    LVB_TRY(icheck("map grid"));
+    MapDesc m;
+    LVB_CUDA(cudaMemcpyAsync(&m, md, sizeof(m), cudaMemcpyDeviceToHost, s));
+    LVB_TRY(host_sync(ctx, s));
+    if (m.P == 0 && !m.err) { set_error("%s: the ground plane fit kept no point", fn); return LVB_ERR_NUMERIC; }
+    if (n_points) *n_points = m.P;
+    LVB_TRY(grid_error(m, fn, ""));
+    LVB_TRY(enqueue_hash(h, d_points, m.P, stride, md, m.ncell, m.ncb, true));
+    LVB_TRY(host_sync(ctx, s));
+    swap_buf(h->map_sorted, h->nx_sorted); swap_buf(h->cell_start, h->nx_cell_start); swap_buf(h->coarse, h->nx_coarse);
+    h->map = m; h->cell_size = cell_size; h->have_map = true;
+    return LVB_OK;
+}
 
 extern "C" {
 
@@ -777,65 +806,13 @@ int lvb_icp_create(lvb_ctx* ctx, lvb_icp** out) {
 }
 void lvb_icp_destroy(lvb_icp* icp) { if (icp) { cudaSetDevice(icp->ctx->device); delete icp; } }
 
-// voxel hash over the n records (stride bytes each) at d_points (device): bounding box, grid, counting sort by voxel key
-static int build_hash(lvb_icp* h, const unsigned char* d_points, int n, int stride, float cell_size) {
-    lvb_ctx* ctx = h->ctx;
-    cudaStream_t s = ctx->stream;
-    LVB_TRY(h->bbox.ensure(6));
-    int init[6];
-    { float big = FLT_MAX, small = -FLT_MAX; int bi, si; memcpy(&bi, &big, 4); memcpy(&si, &small, 4);
-      const int so = si >= 0 ? si : si ^ 0x7fffffff; init[0] = init[1] = init[2] = bi; init[3] = init[4] = init[5] = so; }
-    LVB_CUDA(cudaMemcpyAsync(h->bbox.p, init, sizeof(init), cudaMemcpyHostToDevice, s));
-    ILAUNCH(h, icp_bbox_kernel, std::min(1024, inblk(n, 256)), 256, d_points, n, stride, h->bbox.p);
-    LVB_TRY(icheck("bbox"));
-    int hb[6];
-    LVB_TRY(h->bbox.download(hb, 6, s));
-    LVB_TRY(host_sync(h->ctx, s));
-    Grid g;
-    // The voxel edge is (radius * 1.0001) / ring: the hair of slack guarantees that float rounding of the voxel
-    // coordinate never separates two points closer than the radius by more than `ring` voxels.  ring = 4 unless the
-    // bounding box would need more than MAX_CELLS voxels.
-    g.minx = ord2f(hb[0]); g.miny = ord2f(hb[1]); g.minz = ord2f(hb[2]);
-    const float mx = ord2f(hb[3]), my = ord2f(hb[4]), mz = ord2f(hb[5]);
-    if (!(mx >= g.minx) || !(my >= g.miny) || !(mz >= g.minz) || !std::isfinite(mx - g.minx) || !std::isfinite(my - g.miny) || !std::isfinite(mz - g.minz)) {
-        set_error("map cloud has no finite bounding box"); return LVB_ERR_INVALID; }
-    double dx = 0, dy = 0, dz = 0;
-    int ring = 4;
-    for (;; ring >>= 1) {
-        g.cell = cell_size * 1.0001f / (float)ring; g.inv_cell = 1.0f / g.cell;
-        dx = std::floor((double)(mx - g.minx) * g.inv_cell) + 1; dy = std::floor((double)(my - g.miny) * g.inv_cell) + 1; dz = std::floor((double)(mz - g.minz) * g.inv_cell) + 1;
-        if (dx * dy * dz <= (double)MAX_CELLS || ring == 1) break;
-    }
-    if (dx * dy * dz > (double)MAX_CELLS) { set_error("voxel grid of %.0f cells exceeds %d; increase cell_size or crop the map", dx * dy * dz, (int)MAX_CELLS); return LVB_ERR_UNSUPPORTED; }
-    g.ring = ring;
-    g.gx = (int)dx; g.gy = (int)dy; g.gz = (int)dz;
-    const int ncell = g.gx * g.gy * g.gz;
-    LVB_TRY(h->cell_of.ensure(n)); LVB_TRY(h->counts.ensure(ncell)); LVB_TRY(h->fill.ensure(ncell));
-    LVB_TRY(h->cell_start.ensure((size_t)ncell + 1)); LVB_TRY(h->map_sorted.ensure(n));
-    const int nb = inblk(ncell, 1024);
-    LVB_TRY(h->block_sums.ensure(nb)); LVB_TRY(h->total.ensure(1));
-    LVB_CUDA(cudaMemsetAsync(h->counts.p, 0, (size_t)ncell * sizeof(int), s));
-    LVB_CUDA(cudaMemsetAsync(h->fill.p, 0, (size_t)ncell * sizeof(int), s));
-    h->cbx = (g.gx + 3) >> 2; h->cby = (g.gy + 3) >> 2; h->cbz = (g.gz + 3) >> 2;
-    LVB_TRY(h->coarse.ensure((size_t)h->cbx * h->cby * h->cbz));
-    LVB_CUDA(cudaMemsetAsync(h->coarse.p, 0, (size_t)h->cbx * h->cby * h->cbz * sizeof(int), s));
-    ILAUNCH(h, icp_count_kernel, inblk(n, 256), 256, d_points, n, stride, g, h->cell_of.p, h->counts.p, h->coarse.p, h->cbx, h->cby);
-    ILAUNCH(h, scan_block_kernel, nb, 1024, h->counts.p, h->cell_start.p, ncell, h->block_sums.p);
-    ILAUNCH(h, scan_sums_kernel, 1, 1024, h->block_sums.p, nb, h->total.p);
-    ILAUNCH(h, scan_add_kernel, nb, 1024, h->cell_start.p, ncell, h->block_sums.p, h->cell_start.p + ncell, h->total.p);
-    ILAUNCH(h, icp_scatter_kernel, inblk(n, 256), 256, d_points, n, stride, h->cell_of.p, h->cell_start.p, h->fill.p, h->map_sorted.p);
-    LVB_TRY(icheck("set_map"));
-    LVB_TRY(host_sync(h->ctx, s));
-    h->grid = g; h->P = n; h->cell_size = cell_size; h->have_map = true;
-    return LVB_OK;
-}
-
 int lvb_icp_set_map(lvb_icp* h, const void* points, int n, int stride, float cell_size) {
     if (n <= 0 || !points || stride < 12 || (stride & 3) || !(cell_size > 0.0f)) { set_error("bad map arguments"); return LVB_ERR_INVALID; }
     lvb_ctx* ctx = h->ctx;
     LVB_CUDA(cudaSetDevice(ctx->device)); lvb::g_alloc_stream = ctx->stream;
     LVB_TRY(h->map_raw.upload((const unsigned char*)points, (size_t)n * stride, ctx->stream));
-    return build_hash(h, h->map_raw.p, n, stride, cell_size);
+    LVB_TRY(seed_frame(h, n));
+    return build_map(h, h->map_raw.p, n, stride, cell_size, "lvb_icp_set_map", nullptr);
 }
 
 // ---- device-resident map (SURVEY 8(f).2): the per-keyframe world clouds stay in HBM, the map frame is merged and hashed there
@@ -861,7 +838,7 @@ int lvb_icp_map_append(lvb_icp* h, long long key, const void* robot_points, int 
     float tf[7]; for (int i = 0; i < 7; ++i) tf[i] = (float)pose[i];      // Twc.cast<float>() (mapping.cpp:195)
     if (rc == LVB_OK) rc = d_tf.upload(tf, 7, s);
     if (rc != LVB_OK) { delete sg.pts; return rc; }
-    ILAUNCH(h, icp_to_world_kernel, inblk(n, 256), 256, src, sg.pts->p, n, stride, d_tf.p);
+    ILAUNCH(h, icp_to_world_kernel, inblk(n, 256), 256, src, sg.pts->p, n, stride, d_tf.p, (int*)nullptr);
     rc = icheck("map_append");
     if (rc != LVB_OK) { delete sg.pts; return rc; }
     LVB_TRY(host_sync(h->ctx, s));
@@ -899,29 +876,30 @@ int lvb_icp_map_build(lvb_icp* h, const long long* keys, int n_keys, float cell_
     size_t off = 0;
     for (auto* f : pick) { if (f->n) LVB_CUDA(cudaMemcpyAsync(h->merged.p + off, f->pts->p, (size_t)f->n * sizeof(float4), cudaMemcpyDeviceToDevice, s)); off += f->n; }
     const float4* cloud = h->merged.p;
-    int n = (int)total;
-    if (ground_threshold > 0.0) {      // association_->SegmentGround(points_ground_merged) (mapping.cpp:126)
+    const int n = (int)total;
+    const bool ransac = ground_threshold > 0.0;
+    LVB_TRY(seed_frame(h, ransac ? 0 : n));
+    if (ransac) {      // association_->SegmentGround(points_ground_merged) (mapping.cpp:126): the inlier count stays on the device
         LVB_TRY(h->merged2.ensure(total));
-        LVB_TRY(lidar_segment_ground_device(ctx, h->merged.p, n, ground_threshold, h->merged2.p, &n));
+        LVB_TRY(lidar_segment_ground_device_async(ctx, h->merged.p, n, ground_threshold, h->merged2.p, &h->frame.p->map.P));
         lvb::g_alloc_stream = ctx->stream;
         cloud = h->merged2.p;
-        if (n <= 0) { set_error("lvb_icp_map_build: the ground plane fit kept no point"); return LVB_ERR_NUMERIC; }
     }
-    if (n_points) *n_points = n;
-    return build_hash(h, reinterpret_cast<const unsigned char*>(cloud), n, 16, cell_size);
+    return build_map(h, reinterpret_cast<const unsigned char*>(cloud), n, 16, cell_size, "lvb_icp_map_build", n_points);
 }
 
 int lvb_icp_map_download(lvb_icp* h, float* xyzi, int capacity, int* n_out) {
     if (!h || !h->have_map) { set_error("no map"); return LVB_ERR_STATE; }
     LVB_CUDA(cudaSetDevice(h->ctx->device));
-    if (n_out) *n_out = h->P;
+    const int P = h->map.P;
+    if (n_out) *n_out = P;
     if (!xyzi) return LVB_OK;
-    if (capacity < h->P) { set_error("capacity %d < %d map points", capacity, h->P); return LVB_ERR_INVALID; }
+    if (capacity < P) { set_error("capacity %d < %d map points", capacity, P); return LVB_ERR_INVALID; }
     // hand the cloud back in its original (merge) order: map_sorted carries the original index in .w
-    std::vector<float4> tmp(h->P);
-    LVB_CUDA(cudaMemcpyAsync(tmp.data(), h->map_sorted.p, (size_t)h->P * sizeof(float4), cudaMemcpyDeviceToHost, h->ctx->stream));
+    std::vector<float4> tmp(P);
+    LVB_CUDA(cudaMemcpyAsync(tmp.data(), h->map_sorted.p, (size_t)P * sizeof(float4), cudaMemcpyDeviceToHost, h->ctx->stream));
     LVB_TRY(host_sync(h->ctx, h->ctx->stream));
-    for (int j = 0; j < h->P; ++j) { int i; memcpy(&i, &tmp[j].w, 4); if (i < 0 || i >= h->P) { set_error("corrupt index"); return LVB_ERR_NUMERIC; } xyzi[4 * (size_t)i] = tmp[j].x; xyzi[4 * (size_t)i + 1] = tmp[j].y; xyzi[4 * (size_t)i + 2] = tmp[j].z; xyzi[4 * (size_t)i + 3] = 0.0f; }
+    for (int j = 0; j < P; ++j) { int i; memcpy(&i, &tmp[j].w, 4); if (i < 0 || i >= P) { set_error("corrupt index"); return LVB_ERR_NUMERIC; } xyzi[4 * (size_t)i] = tmp[j].x; xyzi[4 * (size_t)i + 1] = tmp[j].y; xyzi[4 * (size_t)i + 2] = tmp[j].z; xyzi[4 * (size_t)i + 3] = 0.0f; }
     return LVB_OK;
 }
 
@@ -1018,16 +996,10 @@ int lvb_icp_scan_to_map(lvb_icp* h, int mode, const void* scan, int n, int strid
     cudaStream_t s = h->ctx->stream;
     lvb_ctx* ctx = h->ctx;
     ILAUNCH(h, icp_associate_kernel, inblk(n, ITPB), ITPB, d);
-    const int lin_blocks = std::max(1, std::min(inblk(n, ITPB), 4 * ctx->sm_count));
     IcpState hs;
     memset(&hs, 0, sizeof(hs));
     for (int pass = 0; pass <= opt.max_num_iterations; ++pass) {
-        ILAUNCH(h, icp_linearize_kernel<0>, lin_blocks, ITPB, d);
-        if (ctx->world > 1) LVB_TRY(comm_allreduce_sum_f64(ctx, d.st->part, 14));
-        ILAUNCH(h, icp_solve_kernel, 1, 1, d.st);
-        ILAUNCH(h, icp_linearize_kernel<1>, lin_blocks, ITPB, d);
-        if (ctx->world > 1) LVB_TRY(comm_allreduce_sum_f64(ctx, d.st->part + 14, 1));
-        ILAUNCH(h, icp_post_kernel, 1, 1, d.st);
+        LVB_TRY(enqueue_pass(h, d));
         LVB_TRY(icheck("icp iteration"));
         LVB_CUDA(cudaMemcpyAsync(&hs, h->st.p, sizeof(hs), cudaMemcpyDeviceToHost, s));
         LVB_TRY(host_sync(h->ctx, s));
@@ -1045,11 +1017,94 @@ int lvb_icp_scan_to_map(lvb_icp* h, int mode, const void* scan, int n, int strid
     return LVB_OK;
 }
 
-// Mapping::Optimize for one keyframe (mapping.cpp:147-185, after BuildMapFrame): se32rpyxyz, ScanToMapWithGround + Solve, the pose
-// hand-off, ScanToMapWithSegmented + Solve, ToWorld.  Every step is enqueued on the context's stream without a host decision in
-// between: the LM passes run max_num_iterations + 1 times unconditionally (the kernels return at once after the solver stopped), the
-// pose kernels write the query transform the next association reads, and the host synchronises once, at the end, to read the two
-// solver states and the pose back in one copy.
+// ---- Mapping::Optimize for one keyframe on the device: lvb_icp_map_optimize_keyframe against the handles' map frames, and
+// lvb_icp_map_build_optimize_keyframe, which builds them in the same call
+struct KfUpload {
+    std::shared_ptr<DevBuf<unsigned char>> arena;     // [KfBlock | ground scan | surf scan]
+    KfBlock* blk;                                     // its KfBlock (device)
+    KfBlock* hb;                                      // the pinned staging area: the upload, then the read-back
+    size_t off[2];                                    // where the scans lie in the arena
+};
+
+// One copy from the pinned staging area: the poses, the two map frames' descriptors (map[m]), and the scans of the handles given.
+// The staging area stays busy until the caller's read-back.
+static int kf_upload(lvb_ctx* ctx, lvb_icp* const hs[2], const double* map_pose, const double* pose, const MapDesc map[2],
+                     const void* const pts[2], const int ns[2], int stride, KfUpload& u) {
+    size_t bytes[2], all = (sizeof(KfBlock) + 255) & ~(size_t)255;
+    for (int m = 0; m < 2; ++m) {
+        bytes[m] = hs[m] ? (size_t)ns[m] * stride : 0;
+        u.off[m] = all; all = (all + bytes[m] + 255) & ~(size_t)255;
+    }
+    LVB_TRY(lvb::stage_wait(ctx));
+    LVB_TRY(lvb::stage_grow(ctx, all, 0));
+    u.hb = reinterpret_cast<KfBlock*>(ctx->stage_h);
+    memset(u.hb, 0, sizeof(KfBlock));
+    memcpy(u.hb->map_pose, map_pose, sizeof(u.hb->map_pose)); memcpy(u.hb->pose, pose, sizeof(u.hb->pose));
+    for (int m = 0; m < 2; ++m) {
+        u.hb->map[m] = map[m];
+        bbox_seed(u.hb->out_bbox[m]);
+        if (bytes[m]) memcpy(ctx->stage_h + u.off[m], pts[m], bytes[m]);
+    }
+    u.arena = std::make_shared<DevBuf<unsigned char>>();
+    LVB_TRY(u.arena->ensure(all));
+    LVB_CUDA(cudaMemcpyAsync(u.arena->p, ctx->stage_h, all, cudaMemcpyHostToDevice, ctx->stream));
+    LVB_TRY(lvb::stage_mark_busy(ctx, ctx->stream));
+    u.blk = reinterpret_cast<KfBlock*>(u.arena->p);
+    return LVB_OK;
+}
+
+// What registration m reads of its map frame besides blk->map[m]: the sorted cloud and its hash, the cell size (the kNN radius) and
+// the sort counters (nc, exact: see bind_scan).
+struct KfMap { const float4* sorted; const int* cell_start; const int* coarse; float cell_size; size_t nc; bool exact; };
+
+// Mapping::Optimize's loop body (mapping.cpp:147-185) for the registrations that run (run[m]): se32rpyxyz, ScanToMapWithGround +
+// Solve, the pose hand-off, ScanToMapWithSegmented + Solve, then ToWorld of the scans of every handle given into fresh[] (not yet
+// stored; with `boxes`, their bounding boxes into blk->out_bbox).  Nothing waits for the host: each registration runs
+// max_num_iterations + 1 LM passes (the kernels return at once after the solver stopped), and the pose kernels write the query
+// transform the next association reads.
+static int kf_register(lvb_icp* const hs[2], const bool run[2], const KfMap maps[2], const KfUpload& u, const int ns[2], int stride,
+                       const lvb_map_optimize_params* p, bool boxes, lvb_icp::Segment fresh[2]) {
+    KfSeed seed;
+    seed.o = p->options; seed.prior_w = p->prior_weight;
+    for (int m = 0; m < 2; ++m) { seed.weight[m] = p->weight[m]; seed.huber_a[m] = p->huber_a[m]; fresh[m].pts = nullptr; }
+    const int first = run[0] ? 0 : (run[1] ? 1 : -1);
+    ILAUNCH(hs[0] ? hs[0] : hs[1], icp_kf_pose_kernel, 1, 1, u.blk, -1, first, seed);      // rpyxyz from the incoming pose (:154)
+    for (int m = 0; m < 2; ++m) {
+        if (!run[m]) continue;
+        lvb_icp* h = hs[m];
+        const KfMap& km = maps[m];
+        IcpDev d;
+        d.map = km.sorted; d.cell_start = km.cell_start; d.coarse = km.coarse;
+        LVB_TRY(bind_scan(h, u.arena->p + u.off[m], ns[m], stride, &u.blk->map[m], u.blk->tf, km.cell_size * km.cell_size, p->dist_thr[m],
+                          km.nc, km.exact, d));
+        h->kf_arena = u.arena;
+        d.st = &u.blk->st[m];
+        ILAUNCH(h, icp_associate_kernel, inblk(ns[m], ITPB), ITPB, d);
+        for (int pass = 0; pass <= p->options.max_num_iterations; ++pass) LVB_TRY(enqueue_pass(h, d));
+        // pose = map_pose * rpyxyz2se3(rpyxyz) (:165, :177); after the ground solve it also seeds the surf registration
+        ILAUNCH(h, icp_kf_pose_kernel, 1, 1, u.blk, m, m == 0 && run[1] ? 1 : -1, seed);
+    }
+    // ToWorld (:205-220): the robot-frame clouds, transformed by the final pose.cast<float>()
+    for (int m = 0; m < 2; ++m) {
+        if (!hs[m]) continue;
+        fresh[m].key = -1; fresh[m].n = ns[m]; fresh[m].pts = new DevBuf<float4>();
+        const int rc = fresh[m].pts->ensure(std::max(1, ns[m]));
+        if (rc != LVB_OK) { delete fresh[0].pts; delete fresh[1].pts; fresh[0].pts = fresh[1].pts = nullptr; return rc; }
+        ILAUNCH(hs[m], icp_to_world_kernel, inblk(ns[m], 256), 256, u.arena->p + u.off[m], fresh[m].pts->p, ns[m], stride, u.blk->tf,
+                boxes ? u.blk->out_bbox[m] : nullptr);
+    }
+    return LVB_OK;
+}
+
+// replace the cloud under `key` with sg, or add it
+static void store_segment(lvb_icp* h, long long key, lvb_icp::Segment& sg) {
+    sg.key = key;
+    for (auto& old : h->segments) if (old.key == key) { delete old.pts; old = sg; return; }
+    h->segments.push_back(sg);
+}
+
+// Mapping::Optimize for one keyframe (mapping.cpp:147-185, after BuildMapFrame) against the map frames lvb_icp_map_build made, with
+// one host synchronisation at the end to read the two solver states and the pose back in one copy.
 int lvb_icp_map_optimize_keyframe(lvb_icp* ground, lvb_icp* surf, const double map_pose[7], long long key,
                                   const void* ground_pts, int n_ground, const void* surf_pts, int n_surf, int stride,
                                   const lvb_map_optimize_params* p, double pose[7], double rpyxyz[6], lvb_solve_summary summary[2]) {
@@ -1076,74 +1131,29 @@ int lvb_icp_map_optimize_keyframe(lvb_icp* ground, lvb_icp* surf, const double m
     const auto t0 = std::chrono::steady_clock::now();
     cudaStream_t s = ctx->stream;
     lvb::timing_mark(s, "begin");
-    // one upload: [KfBlock | ground scan | surf scan], assembled in the pinned staging area
-    size_t off[2], bytes[2], total = (sizeof(KfBlock) + 255) & ~(size_t)255;
+    const bool run[2] = {ground != nullptr, surf != nullptr};
+    MapDesc desc[2];
+    KfMap maps[2];
     for (int m = 0; m < 2; ++m) {
-        bytes[m] = hs[m] ? (size_t)ns[m] * stride : 0;
-        off[m] = total; total = (total + bytes[m] + 255) & ~(size_t)255;
+        desc[m] = hs[m] ? hs[m]->map : desc_seed(0);          // P = 0: no registration on that side
+        if (hs[m]) maps[m] = {hs[m]->map_sorted.p, hs[m]->cell_start.p, hs[m]->coarse.p, hs[m]->cell_size, (size_t)hs[m]->map.nc, true};
     }
-    LVB_TRY(lvb::stage_wait(ctx));
-    LVB_TRY(lvb::stage_grow(ctx, total, 0));
-    KfBlock* hb = reinterpret_cast<KfBlock*>(ctx->stage_h);
-    memset(hb, 0, sizeof(KfBlock));
-    memcpy(hb->map_pose, map_pose, sizeof(hb->map_pose)); memcpy(hb->pose, pose, sizeof(hb->pose));
-    for (int m = 0; m < 2; ++m) if (bytes[m]) memcpy(ctx->stage_h + off[m], pts[m], bytes[m]);
-    auto arena = std::make_shared<DevBuf<unsigned char>>();
-    LVB_TRY(arena->ensure(total));
-    LVB_CUDA(cudaMemcpyAsync(arena->p, ctx->stage_h, total, cudaMemcpyHostToDevice, s));
-    LVB_TRY(lvb::stage_mark_busy(ctx, s));
-    KfBlock* blk = reinterpret_cast<KfBlock*>(arena->p);
-
-    KfSeed seed;
-    seed.o = opt; seed.prior_w = p->prior_weight;
-    for (int m = 0; m < 2; ++m) { seed.weight[m] = p->weight[m]; seed.huber_a[m] = p->huber_a[m]; }
-    const int first = ground ? 0 : 1;
-    ILAUNCH(h0, icp_kf_pose_kernel, 1, 1, blk, -1, first, seed);                   // rpyxyz from the incoming pose (mapping.cpp:154)
-    for (int m = first; m < 2 && hs[m]; ++m) {
-        lvb_icp* h = hs[m];
-        IcpDev d;
-        LVB_TRY(bind_scan(h, arena->p + off[m], ns[m], stride, blk->tf, h->cell_size * h->cell_size, p->dist_thr[m], d));
-        h->kf_arena = arena;
-        d.st = &blk->st[m];
-        ILAUNCH(h, icp_associate_dev_tf_kernel, inblk(ns[m], ITPB), ITPB, d, blk->tf);
-        const int lin_blocks = std::max(1, std::min(inblk(ns[m], ITPB), 4 * ctx->sm_count));
-        for (int pass = 0; pass <= opt.max_num_iterations; ++pass) {
-            ILAUNCH(h, icp_linearize_kernel<0>, lin_blocks, ITPB, d);
-            ILAUNCH(h, icp_solve_kernel, 1, 1, d.st);
-            ILAUNCH(h, icp_linearize_kernel<1>, lin_blocks, ITPB, d);
-            ILAUNCH(h, icp_post_kernel, 1, 1, d.st);
-        }
-        // pose = map_pose * rpyxyz2se3(rpyxyz) (:165, :177); after the ground solve it also seeds the surf registration
-        ILAUNCH(h, icp_kf_pose_kernel, 1, 1, blk, m, m == 0 && surf ? 1 : -1, seed);
-    }
-    // ToWorld (mapping.cpp:205-220): the robot-frame clouds, transformed by pose.cast<float>(), replace whatever `key` held
+    KfUpload u;
+    LVB_TRY(kf_upload(ctx, hs, map_pose, pose, desc, pts, ns, stride, u));
     lvb_icp::Segment fresh[2];
-    for (int m = 0; m < 2; ++m) {
-        fresh[m].pts = nullptr;
-        if (!hs[m]) continue;
-        fresh[m].key = key; fresh[m].n = ns[m]; fresh[m].pts = new DevBuf<float4>();
-        int rc = fresh[m].pts->ensure(std::max(1, ns[m]));
-        if (rc != LVB_OK) { delete fresh[0].pts; delete fresh[1].pts; return rc; }
-        ILAUNCH(hs[m], icp_to_world_kernel, inblk(ns[m], 256), 256, arena->p + off[m], fresh[m].pts->p, ns[m], stride, blk->tf);
-    }
+    LVB_TRY(kf_register(hs, run, maps, u, ns, stride, p, false, fresh));
     int rc = icheck("map_optimize_keyframe");
     if (rc != LVB_OK) { delete fresh[0].pts; delete fresh[1].pts; return rc; }
-    for (int m = 0; m < 2; ++m) {
-        if (!hs[m]) continue;
-        auto& segs = hs[m]->segments;
-        bool replaced = false;
-        for (auto& sg : segs) if (sg.key == key) { delete sg.pts; sg = fresh[m]; replaced = true; }
-        if (!replaced) segs.push_back(fresh[m]);
-    }
+    for (int m = 0; m < 2; ++m) if (hs[m]) store_segment(hs[m], key, fresh[m]);
     // the one read-back: both solver states, rpyxyz and the pose
-    LVB_CUDA(cudaMemcpyAsync(ctx->stage_h, blk, sizeof(KfBlock), cudaMemcpyDeviceToHost, s));
+    LVB_CUDA(cudaMemcpyAsync(u.hb, u.blk, sizeof(KfBlock), cudaMemcpyDeviceToHost, s));
     LVB_TRY(host_sync(ctx, s));
     ctx->stage_busy = false;
     const double el = std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
-    memcpy(pose, hb->pose, sizeof(hb->pose)); memcpy(rpyxyz, hb->rpyxyz, sizeof(hb->rpyxyz));
+    memcpy(pose, u.hb->pose, sizeof(u.hb->pose)); memcpy(rpyxyz, u.hb->rpyxyz, sizeof(u.hb->rpyxyz));
     if (summary) {
         for (int m = 0; m < 2; ++m) {
-            if (hs[m]) { fill_summary(hb->st[m], p->prior_weight, el, &summary[m]); continue; }
+            if (hs[m]) { fill_summary(u.hb->st[m], p->prior_weight, el, &summary[m]); continue; }
             memset(&summary[m], 0, sizeof(summary[m]));
             summary[m].termination_type = -1;          // registration skipped (mapping.cpp:155,167: empty map cloud)
         }
@@ -1152,17 +1162,6 @@ int lvb_icp_map_optimize_keyframe(lvb_icp* ground, lvb_icp* surf, const double m
 }
 
 // ---- Mapping::BuildMapFrame + Mapping::Optimize for one keyframe in one call (lvb_icp_map_build_optimize_keyframe)
-struct BkBlock {             // the call's device state, uploaded and read back with one copy each
-    KfBlock kf;
-    MapDesc map[2];          // [0] ground, [1] surf map frame
-    int out_bbox[2][6];      // bounding boxes of the two clouds ToWorld stores
-};
-
-static void bbox_seed(int* b) {       // icp_bbox_kernel's starting values: min = FLT_MAX, max = -FLT_MAX as ordered ints
-    float big = FLT_MAX, small = -FLT_MAX; int bi, si; memcpy(&bi, &big, 4); memcpy(&si, &small, 4);
-    const int so = si >= 0 ? si : si ^ 0x7fffffff;
-    b[0] = b[1] = b[2] = bi; b[3] = b[4] = b[5] = so;
-}
 static void bbox_store(lvb_icp::Segment& sg, const int* b) {
     for (int a = 0; a < 3; ++a) { sg.lo[a] = ord2f(b[a]); sg.hi[a] = ord2f(b[3 + a]); }
     sg.has_bbox = true;
@@ -1176,25 +1175,25 @@ static int fill_bboxes(lvb_icp* h, const std::vector<lvb_icp::Segment*>& segs) {
     if (todo.empty()) return LVB_OK;
     lvb_ctx* ctx = h->ctx;
     cudaStream_t s = ctx->stream;
-    const size_t bytes = todo.size() * 6 * sizeof(int);
+    const size_t bytes = todo.size() * sizeof(MapDesc);
     LVB_TRY(lvb::stage_wait(ctx));
     LVB_TRY(lvb::stage_grow(ctx, bytes, 0));
-    int* hb = reinterpret_cast<int*>(ctx->stage_h);
-    for (size_t i = 0; i < todo.size(); ++i) bbox_seed(hb + 6 * i);
-    DevBuf<int> d;
-    LVB_TRY(d.ensure(todo.size() * 6));
+    MapDesc* hb = reinterpret_cast<MapDesc*>(ctx->stage_h);
+    for (size_t i = 0; i < todo.size(); ++i) hb[i] = desc_seed(todo[i]->n);
+    DevBuf<MapDesc> d;
+    LVB_TRY(d.ensure(todo.size()));
     LVB_CUDA(cudaMemcpyAsync(d.p, hb, bytes, cudaMemcpyHostToDevice, s));
     for (size_t i = 0; i < todo.size(); ++i)
-        ILAUNCH(h, icp_bbox_kernel, std::min(1024, inblk(todo[i]->n, 256)), 256, reinterpret_cast<const unsigned char*>(todo[i]->pts->p), todo[i]->n, 16, d.p + 6 * i);
+        ILAUNCH(h, icp_bbox_kernel, std::min(1024, inblk(todo[i]->n, 256)), 256, reinterpret_cast<const unsigned char*>(todo[i]->pts->p), 16, d.p + i);
     LVB_TRY(icheck("map frame bounding boxes"));
     LVB_CUDA(cudaMemcpyAsync(hb, d.p, bytes, cudaMemcpyDeviceToHost, s));
     LVB_TRY(host_sync(ctx, s));
-    for (size_t i = 0; i < todo.size(); ++i) bbox_store(*todo[i], hb + 6 * i);
+    for (size_t i = 0; i < todo.size(); ++i) bbox_store(*todo[i], hb[i].bbox);
     return LVB_OK;
 }
 
-// Capacities of a map frame whose cloud lies inside the box lo..hi: build_hash's ring-4 grid of the box (the voxel counts per axis
-// only shrink with a smaller box or a coarser ring), capped at MAX_CELLS -- above it the device picks a coarser ring or fails.
+// Capacities of a map frame whose cloud lies inside the box lo..hi: icp_map_grid_kernel's ring-4 grid of the box (the voxel counts per
+// axis only shrink with a smaller box or a coarser ring), capped at MAX_CELLS -- above it the device picks a coarser ring or fails.
 struct MapBound { size_t cells, coarse, qsort; bool finite; };
 static MapBound map_bound(const float* lo, const float* hi, float cell_size) {
     MapBound b;
@@ -1206,35 +1205,12 @@ static MapBound map_bound(const float* lo, const float* hi, float cell_size) {
         if (!(hi[a] >= lo[a]) || !std::isfinite(w)) { b.finite = false; d[a] = 0; } else d[a] = std::floor((double)w * inv) + 1;
     }
     const double cap = (double)MAX_CELLS;
-    const int forced = sort_shift_forced();
-    if (!b.finite) { b.cells = b.coarse = MAX_CELLS; b.qsort = forced < 0 ? 8000000 : MAX_CELLS; return b; }
+    if (!b.finite) { b.cells = b.coarse = MAX_CELLS; b.qsort = 8000000; return b; }
     auto blocks = [&](int sh) { double v = 1; for (int a = 0; a < 3; ++a) v *= std::ceil(d[a] / (double)(1 << sh)); return v; };
     b.cells = (size_t)std::min(cap, d[0] * d[1] * d[2]);
     b.coarse = (size_t)std::min(cap, blocks(2));
-    // bind_scan's rule keeps the sort grid at <= 8 M counters; a forced granularity is bounded by the voxel count
-    b.qsort = forced < 0 ? (size_t)std::min(8.0e6, blocks(1)) : (size_t)std::min((double)b.cells, blocks(forced));
+    b.qsort = (size_t)std::min(8.0e6, blocks(1));          // the grid kernel keeps the sort grid at <= 8 M counters
     return b;
-}
-
-// bind_scan against the map frame of m (device), its counters sized for `bound`
-static int bind_scan_map(lvb_icp* h, const unsigned char* d_scan, int n, int stride, const float* tf_dev, float max_d2, double thr,
-                         const MapDesc* m, const MapBound& bound, IcpDev& d) {
-    LVB_TRY(bind_buffers(h, d_scan, n, stride, max_d2, thr, d));
-    d.map = h->nx_sorted.p; d.cell_start = h->nx_cell_start.p; d.coarse = h->nx_coarse.p;
-    memset(&d.g, 0, sizeof(d.g)); d.P = 0; d.cbx = d.cby = d.cbz = 0;          // read from m by the kernels
-    if (n >= 4096) {
-        const int nc = (int)std::max<size_t>(1, bound.qsort), nb = (nc + 1023) / 1024;
-        LVB_TRY(h->q_key.ensure(n)); LVB_TRY(h->q_order.ensure(n)); LVB_TRY(h->q_counts.ensure(nc)); LVB_TRY(h->q_fill.ensure(nc));
-        LVB_TRY(h->q_start.ensure((size_t)nc + 1)); LVB_TRY(h->q_sums.ensure(nb)); LVB_TRY(h->q_total.ensure(1));
-        ILAUNCH(h, icp_zero_map_kernel, std::min(inblk(nc, 256), 8 * h->ctx->sm_count), 256, h->q_counts.p, h->q_fill.p, &m->nc);
-        ILAUNCH(h, icp_query_key_map_kernel, (n + 255) / 256, 256, d, tf_dev, m, h->q_key.p, h->q_counts.p);
-        ILAUNCH(h, scan_block_map_kernel, nb, 1024, h->q_counts.p, h->q_start.p, &m->nc, h->q_sums.p);
-        ILAUNCH(h, scan_sums_map_kernel, 1, 1024, h->q_sums.p, &m->nc, h->q_total.p);
-        ILAUNCH(h, scan_add_map_kernel, nb, 1024, h->q_start.p, &m->nc, h->q_sums.p, h->q_total.p);
-        ILAUNCH(h, icp_query_scatter_kernel, (n + 255) / 256, 256, n, h->q_key.p, h->q_start.p, h->q_fill.p, h->q_order.p);
-        d.order = h->q_order.p;
-    }
-    return LVB_OK;
 }
 
 // Mapping::BuildMapFrame (mapping.cpp:114-137) + the body of Mapping::Optimize's loop (:147-185) for one keyframe.  The host knows
@@ -1285,44 +1261,30 @@ int lvb_icp_map_build_optimize_keyframe(lvb_icp* ground, lvb_icp* surf, const lo
     const bool ransac = ground_threshold > 0.0;
     bool build[2];
     MapBound bound[2];
+    MapDesc seed[2];
     for (int m = 0; m < 2; ++m) {
         build[m] = total[m] > 0;           // an empty merged cloud: BuildMapFrame fails on that side and nothing registers (:155,167)
+        seed[m] = desc_seed(build[m] && !(m == 0 && ransac) ? (int)total[m] : 0);      // the ground count comes from SegmentGround
         if (!build[m]) continue;
         float lo[3] = {FLT_MAX, FLT_MAX, FLT_MAX}, hi[3] = {-FLT_MAX, -FLT_MAX, -FLT_MAX};
         for (auto* sg : pick[m]) for (int a = 0; a < 3; ++a) { lo[a] = std::min(lo[a], sg->lo[a]); hi[a] = std::max(hi[a], sg->hi[a]); }
         bound[m] = map_bound(lo, hi, cell_size[m]);
-        // without SegmentGround the map frame's box is the union: build_hash's check can be made here (after it, on the device)
+        // without SegmentGround the map frame's box is the union: the grid kernel's check can be made here (after it, on the device)
         if (!bound[m].finite && !(m == 0 && ransac)) { set_error("%s: map cloud has no finite bounding box", fn); return LVB_ERR_INVALID; }
     }
     const auto t0 = std::chrono::steady_clock::now();
     cudaStream_t s = ctx->stream;
     lvb::timing_mark(s, "begin");
-    // one upload: [BkBlock | ground scan | surf scan], assembled in the pinned staging area
-    size_t off[2], bytes[2], all = (sizeof(BkBlock) + 255) & ~(size_t)255;
-    for (int m = 0; m < 2; ++m) { bytes[m] = (size_t)ns[m] * stride; off[m] = all; all = (all + bytes[m] + 255) & ~(size_t)255; }
-    LVB_TRY(lvb::stage_wait(ctx));
-    LVB_TRY(lvb::stage_grow(ctx, all, 0));
-    BkBlock* hb = reinterpret_cast<BkBlock*>(ctx->stage_h);
-    memset(hb, 0, sizeof(BkBlock));
-    memcpy(hb->kf.map_pose, map_pose, sizeof(hb->kf.map_pose)); memcpy(hb->kf.pose, pose, sizeof(hb->kf.pose));
-    for (int m = 0; m < 2; ++m) {
-        bbox_seed(hb->map[m].bbox); bbox_seed(hb->out_bbox[m]);
-        hb->map[m].P = build[m] && !(m == 0 && ransac) ? (int)total[m] : 0;      // the ground count comes from SegmentGround
-        if (bytes[m]) memcpy(ctx->stage_h + off[m], pts[m], bytes[m]);
-    }
-    auto arena = std::make_shared<DevBuf<unsigned char>>();
-    LVB_TRY(arena->ensure(all));
-    LVB_CUDA(cudaMemcpyAsync(arena->p, ctx->stage_h, all, cudaMemcpyHostToDevice, s));
-    LVB_TRY(lvb::stage_mark_busy(ctx, s));
-    BkBlock* blk = reinterpret_cast<BkBlock*>(arena->p);
+    KfUpload u;
+    LVB_TRY(kf_upload(ctx, hs, map_pose, pose, seed, pts, ns, stride, u));
 
     // BuildMapFrame: merge in key order, SegmentGround on the ground side, voxel hash sized by the bound, grid decided on the device
+    KfMap maps[2];
     for (int m = 0; m < 2; ++m) {
         if (!build[m]) continue;
         lvb_icp* h = hs[m];
-        MapDesc* md = &blk->map[m];
+        MapDesc* md = &u.blk->map[m];
         const int n = (int)total[m];
-        const MapBound& b = bound[m];
         LVB_TRY(h->merged.ensure(n));
         size_t o = 0;
         for (auto* f : pick[m]) { if (f->n) LVB_CUDA(cudaMemcpyAsync(h->merged.p + o, f->pts->p, (size_t)f->n * sizeof(float4), cudaMemcpyDeviceToDevice, s)); o += f->n; }
@@ -1334,65 +1296,23 @@ int lvb_icp_map_build_optimize_keyframe(lvb_icp* ground, lvb_icp* surf, const lo
             cloud = h->merged2.p;
         }
         const unsigned char* cp = reinterpret_cast<const unsigned char*>(cloud);
-        const int nb = inblk(b.cells, 1024);
-        LVB_TRY(h->cell_of.ensure(n)); LVB_TRY(h->counts.ensure(b.cells)); LVB_TRY(h->fill.ensure(b.cells));
-        LVB_TRY(h->nx_cell_start.ensure(b.cells + 1)); LVB_TRY(h->nx_sorted.ensure(n)); LVB_TRY(h->nx_coarse.ensure(b.coarse));
-        LVB_TRY(h->block_sums.ensure(nb)); LVB_TRY(h->total.ensure(1));
-        ILAUNCH(h, icp_bbox_map_kernel, std::min(1024, inblk(n, 256)), 256, cp, 16, md);
-        ILAUNCH(h, icp_map_grid_kernel, 1, 1, md, cell_size[m], sort_shift_forced());
-        ILAUNCH(h, icp_zero_map_kernel, std::min(inblk(b.cells, 256), 8 * ctx->sm_count), 256, h->counts.p, h->fill.p, &md->ncell);
-        ILAUNCH(h, icp_zero_map_kernel, std::min(inblk(b.coarse, 256), 8 * ctx->sm_count), 256, h->nx_coarse.p, (int*)nullptr, &md->ncb);
-        ILAUNCH(h, icp_count_map_kernel, inblk(n, 256), 256, cp, 16, md, h->cell_of.p, h->counts.p, h->nx_coarse.p);
-        ILAUNCH(h, scan_block_map_kernel, nb, 1024, h->counts.p, h->nx_cell_start.p, &md->ncell, h->block_sums.p);
-        ILAUNCH(h, scan_sums_map_kernel, 1, 1024, h->block_sums.p, &md->ncell, h->total.p);
-        ILAUNCH(h, scan_add_map_kernel, nb, 1024, h->nx_cell_start.p, &md->ncell, h->block_sums.p, h->total.p);
-        ILAUNCH(h, icp_scatter_map_kernel, inblk(n, 256), 256, cp, 16, md, h->cell_of.p, h->nx_cell_start.p, h->fill.p, h->nx_sorted.p);
-        LVB_TRY(icheck("map frame build"));
+        ILAUNCH(h, icp_bbox_kernel, std::min(1024, inblk(n, 256)), 256, cp, 16, md);
+        ILAUNCH(h, icp_map_grid_kernel, 1, 1, md, cell_size[m]);
+        LVB_TRY(enqueue_hash(h, cp, n, 16, md, bound[m].cells, bound[m].coarse, false));
+        maps[m] = {h->nx_sorted.p, h->nx_cell_start.p, h->nx_coarse.p, cell_size[m], bound[m].qsort, false};
     }
 
-    // the registrations (as lvb_icp_map_optimize_keyframe), each against the map frame just built
+    // the registrations, each against the map frame just built
     struct ScanState { int n, stride; const unsigned char* dev; std::shared_ptr<DevBuf<unsigned char>> arena; } saved[2];
     for (int m = 0; m < 2; ++m) saved[m] = {hs[m]->scan_n, hs[m]->scan_stride, hs[m]->scan_dev, hs[m]->kf_arena};
-    KfSeed seed;
-    seed.o = opt; seed.prior_w = p->prior_weight;
-    for (int m = 0; m < 2; ++m) { seed.weight[m] = p->weight[m]; seed.huber_a[m] = p->huber_a[m]; }
-    const int first = build[0] ? 0 : (build[1] ? 1 : -1);
-    ILAUNCH(ground, icp_kf_pose_map_kernel, 1, 1, &blk->kf, -1, first, seed, blk->map);      // rpyxyz from the incoming pose (:154)
-    for (int m = 0; m < 2; ++m) {
-        if (!build[m]) continue;
-        lvb_icp* h = hs[m];
-        const MapDesc* md = &blk->map[m];
-        IcpDev d;
-        LVB_TRY(bind_scan_map(h, arena->p + off[m], ns[m], stride, blk->kf.tf, cell_size[m] * cell_size[m], p->dist_thr[m], md, bound[m], d));
-        d.st = &blk->kf.st[m];
-        ILAUNCH(h, icp_associate_map_kernel, inblk(ns[m], ITPB), ITPB, d, blk->kf.tf, md);
-        const int lin_blocks = std::max(1, std::min(inblk(ns[m], ITPB), 4 * ctx->sm_count));
-        for (int pass = 0; pass <= opt.max_num_iterations; ++pass) {
-            ILAUNCH(h, icp_linearize_kernel<0>, lin_blocks, ITPB, d);
-            ILAUNCH(h, icp_solve_kernel, 1, 1, d.st);
-            ILAUNCH(h, icp_linearize_kernel<1>, lin_blocks, ITPB, d);
-            ILAUNCH(h, icp_post_kernel, 1, 1, d.st);
-        }
-        ILAUNCH(h, icp_kf_pose_map_kernel, 1, 1, &blk->kf, m, m == 0 && build[1] ? 1 : -1, seed, blk->map);
-    }
-    // ToWorld (:205-220): both robot-frame clouds, transformed by the final pose.cast<float>(), with their bounding boxes
     lvb_icp::Segment fresh[2];
-    for (int m = 0; m < 2; ++m) {
-        fresh[m].key = key; fresh[m].n = ns[m]; fresh[m].pts = new DevBuf<float4>();
-        const int rc = fresh[m].pts->ensure(std::max(1, ns[m]));
-        if (rc != LVB_OK) { delete fresh[0].pts; if (m) delete fresh[1].pts; return rc; }
-        ILAUNCH(hs[m], icp_to_world_bbox_kernel, inblk(ns[m], 256), 256, arena->p + off[m], fresh[m].pts->p, ns[m], stride, blk->kf.tf, blk->out_bbox[m]);
-    }
-    int rc = icheck("map_build_optimize_keyframe");
+    int rc = kf_register(hs, build, maps, u, ns, stride, p, true, fresh);
+    if (rc == LVB_OK) rc = icheck("map_build_optimize_keyframe");
     // the one read-back: solver states, pose, rpyxyz, both map descriptors (grid, point count, failure), the stored clouds' boxes
-    if (rc == LVB_OK && cudaMemcpyAsync(ctx->stage_h, blk, sizeof(BkBlock), cudaMemcpyDeviceToHost, s) != cudaSuccess) rc = lvb::cuda_fail(cudaGetLastError(), "read-back", __FILE__, __LINE__);
+    if (rc == LVB_OK && cudaMemcpyAsync(u.hb, u.blk, sizeof(KfBlock), cudaMemcpyDeviceToHost, s) != cudaSuccess) rc = lvb::cuda_fail(cudaGetLastError(), "read-back", __FILE__, __LINE__);
     if (rc == LVB_OK) rc = host_sync(ctx, s);
     if (rc == LVB_OK) ctx->stage_busy = false;
-    for (int m = 0; m < 2 && rc == LVB_OK; ++m) {
-        if (!build[m] || !hb->map[m].err) continue;
-        if (hb->map[m].err == 1) { set_error("%s: map cloud has no finite bounding box", fn); rc = LVB_ERR_INVALID; }
-        else { set_error("%s: voxel grid of the %s map frame exceeds %d cells; increase cell_size or crop the map", fn, m ? "surf" : "ground", (int)MAX_CELLS); rc = LVB_ERR_UNSUPPORTED; }
-    }
+    for (int m = 0; m < 2 && rc == LVB_OK; ++m) if (build[m]) rc = grid_error(u.hb->map[m], fn, m ? "surf " : "ground ");
     if (rc != LVB_OK) {        // nothing was committed: the resident clouds and the map frames are as they were
         delete fresh[0].pts; delete fresh[1].pts;
         for (int m = 0; m < 2; ++m) { hs[m]->scan_n = saved[m].n; hs[m]->scan_stride = saved[m].stride; hs[m]->scan_dev = saved[m].dev; hs[m]->kf_arena = saved[m].arena; }
@@ -1401,24 +1321,22 @@ int lvb_icp_map_build_optimize_keyframe(lvb_icp* ground, lvb_icp* surf, const lo
     const double el = std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
     for (int m = 0; m < 2; ++m) {
         lvb_icp* h = hs[m];
-        const MapDesc& md = hb->map[m];
+        const MapDesc& md = u.hb->map[m];
         const bool built = build[m] && md.P > 0;
         if (built) {           // the new map frame replaces the one before, as lvb_icp_map_build would
             swap_buf(h->map_sorted, h->nx_sorted); swap_buf(h->cell_start, h->nx_cell_start); swap_buf(h->coarse, h->nx_coarse);
-            h->grid = md.g; h->P = md.P; h->cbx = md.cbx; h->cby = md.cby; h->cbz = md.cbz; h->cell_size = cell_size[m]; h->have_map = true;
+            h->map = md; h->cell_size = cell_size[m]; h->have_map = true;
         }
-        bbox_store(fresh[m], hb->out_bbox[m]);
-        bool replaced = false;
-        for (auto& sg : h->segments) if (sg.key == key) { delete sg.pts; sg = fresh[m]; replaced = true; }
-        if (!replaced) h->segments.push_back(fresh[m]);
-        h->scan_n = ns[m]; h->scan_stride = stride; h->scan_dev = arena->p + off[m]; h->kf_arena = arena;
+        bbox_store(fresh[m], u.hb->out_bbox[m]);
+        store_segment(h, key, fresh[m]);
+        h->scan_n = ns[m]; h->scan_stride = stride; h->scan_dev = u.arena->p + u.off[m]; h->kf_arena = u.arena;
         if (n_map_points) n_map_points[m] = built ? md.P : 0;
         if (summary) {
-            if (built) fill_summary(hb->kf.st[m], p->prior_weight, el, &summary[m]);
+            if (built) fill_summary(u.hb->st[m], p->prior_weight, el, &summary[m]);
             else { memset(&summary[m], 0, sizeof(summary[m])); summary[m].termination_type = -1; }
         }
     }
-    memcpy(pose, hb->kf.pose, sizeof(hb->kf.pose)); memcpy(rpyxyz, hb->kf.rpyxyz, sizeof(hb->kf.rpyxyz));
+    memcpy(pose, u.hb->pose, sizeof(u.hb->pose)); memcpy(rpyxyz, u.hb->rpyxyz, sizeof(u.hb->rpyxyz));
     return LVB_OK;
 }
 

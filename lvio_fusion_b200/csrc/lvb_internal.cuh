@@ -66,9 +66,8 @@ int comm_allreduce_max_i32(lvb_ctx* ctx, int* buf, size_t count);
 // per-kernel timing (lvb_debug_timing): a CUDA event on the launching stream after every kernel, named; off by default
 extern bool g_timing;
 void timing_mark(cudaStream_t s, const char* name);
-int lidar_segment_ground_device(lvb_ctx* ctx, const float4* in, int n, double thr, float4* out, int* n_out);   // lidar.cu
-// the same without a read-back: the inlier count stays on the device at n_out_dev (0 when n < 3 or no plane is found), `out` holds
-// n records; nothing is waited for
+// SegmentGround on a device cloud (lidar.cu): the inlier count stays on the device at n_out_dev (0 when n < 3 or no plane is found),
+// `out` holds n records; nothing is waited for
 int lidar_segment_ground_device_async(lvb_ctx* ctx, const float4* in, int n, double thr, float4* out, int* n_out_dev);
 // every host wait on a context's stream goes through here and is counted in ctx->syncs (lvb_sync_count)
 int host_sync(lvb_ctx* ctx, cudaStream_t s);
