@@ -292,6 +292,32 @@ LVB_API int lvb_icp_map_build_optimize_keyframe(lvb_icp* ground, lvb_icp* surf, 
                                                 const void* ground_pts, int n_ground, const void* surf_pts, int n_surf, int stride_bytes,
                                                 const lvb_map_optimize_params* p, double pose[7] /* in: frame->pose, out: optimised */,
                                                 double rpyxyz[6] /* out */, lvb_solve_summary summary[2], int n_map_points[2]);
+/* Mapping::Relocate for one loop-closure candidate (mapping.cpp:78-112, 251-300), with one host synchronisation:
+ *   pose = old_pose * relative_guess                                 (clone_frame->pose, :256)
+ *   BuildOldMapFrame: the map frame of keys / n_keys (1 to 3: the lidar keyframe before the old one, the old one if it has lidar, the
+ *                  one after it, in time order), resident on both handles, merged in that order, SegmentGround (ground_threshold > 0)
+ *                  on the ground side, hashed with cell_size[2] -- into a relocation slot of each handle, reused by every call and never
+ *                  made the handle's map frame.  map_pose: the pose of the EARLIEST of the keys (old_frames.begin(), :106-108).
+ *   `rounds` rounds (the reference runs 4; 1 to 16): rpyxyz = se32rpyxyz(map_pose^-1 * pose), ScanToMapWithGround + Solve, pose =
+ *                  map_pose * rpyxyz2se3(rpyxyz), ScanToMapWithSegmented + Solve, pose again -- as in lvb_icp_map_optimize_keyframe,
+ *                  and always without the prior: p->prior_weight must be < 0 (relocate = true).
+ *   relative_o_c = old_pose^-1 * pose (:298); pose: the final clone pose.
+ *   score[m] = min(n / 10, cap) - 2 final_cost / n of the last round's registration m (:281-282, :294-295; n =
+ *                  num_residual_blocks_reduced, cap 20 ground / 30 surf), in FP64; NaN when that side did not run or n == 0.  The
+ *                  reference returns (int)(score[0] + score[1]).
+ * summary[2] is the last round's (may be NULL, as may score and n_map_points).  A side whose merged cloud is empty or whose
+ * SegmentGround keeps no point is skipped in every round: summary zero with termination_type = -1, score NaN, n_map_points 0.
+ * Nothing is stored: knn3, map_download, scan_to_map and map_append(NULL) on either handle behave afterwards as before the call, and
+ * every resident cloud is unchanged.  The launch sequence depends only on the sizes and options, not on when a solver stops or how
+ * many points SegmentGround keeps.  A resident cloud without a recorded bounding box costs one more synchronisation, once.
+ * Errors, all before any state changes: as lvb_icp_map_build_optimize_keyframe (unknown key, time limit set, sharded context), and
+ * LVB_ERR_INVALID for n_keys outside 1..3, rounds outside 1..16 or prior_weight >= 0; failures found on the device (no finite bounding
+ * box, grid overflow) leave every cloud and map frame as they were. */
+LVB_API int lvb_icp_map_relocate(lvb_icp* ground, lvb_icp* surf, const long long* keys, int n_keys, const float cell_size[2],
+                                 double ground_threshold, const double map_pose[7], const double old_pose[7], const double relative_guess[7],
+                                 const void* ground_pts, int n_ground, const void* surf_pts, int n_surf, int stride_bytes,
+                                 const lvb_map_optimize_params* p, int rounds, double relative_o_c[7] /* out */, double pose[7] /* out */,
+                                 lvb_solve_summary summary[2], double score[2], int n_map_points[2]);
 
 /* ---- lidar feature pipeline, the producer of the scan-to-map inputs (SURVEY 8(f).2).
  * Stands behind FeatureAssociation::Process (association.cpp:88-268: Preprocess, AdjustDistortion, CalculateSmoothness,

@@ -12,6 +12,7 @@
 //       (anything with .size() and .data() whose records start with float x, y, z)
 //   frame->weights.lidar_ground / lidar_surf / visual,  frame->features_left.size()
 #pragma once
+#include <algorithm>
 #include <cmath>
 #include <type_traits>
 #include <unordered_map>
@@ -73,6 +74,7 @@ public:
     bool AppendKeyframe(long long key, const Cloud& ground_robot, const Cloud& surf_robot, const double* pose7) {
         Handles& h = handles_of_thread()[this];
         if (!ensure_handles(h)) return false;
+        resident_ = &h;
         const int stride = (int)sizeof(assoc_detail::cloud_data(ground_robot, 0)[0]);
         lvb_icp_map_evict(h.ground, key); lvb_icp_map_evict(h.surf, key);            // re-registering a keyframe (ToWorld(start)) replaces its clouds
         return lvb_icp_map_append(h.ground, key, assoc_detail::cloud_data(ground_robot, 0), (int)ground_robot.size(), stride, pose7) == LVB_OK &&
@@ -118,6 +120,7 @@ public:
     bool OptimizeKeyframe(FramePtr frame, const double* map_pose7, long long key, lvb_solve_summary* summary = nullptr) {
         Handles& h = handles_of_thread()[this];
         if (!ensure_handles(h)) return false;
+        resident_ = &h;
         const auto& g = frame->feature_lidar->points_ground;
         const auto& s = frame->feature_lidar->points_surf;
         const int stride = (int)sizeof(assoc_detail::cloud_data(g, 0)[0]);
@@ -169,7 +172,43 @@ public:
             return false;
         h.ground_map = n_map[0] > 0; h.surf_map = n_map[1] > 0;
         h.resident = h.ground_map && h.surf_map;
+        resident_ = &h;
         return true;
+    }
+
+    // Mapping::Relocate for one loop-closure candidate (mapping.cpp:78-112, 251-300) in ONE device call with one host synchronisation
+    // (lvb_icp_map_relocate): BuildOldMapFrame of `keys` (1 to 3 resident keyframes in time order: the lidar keyframe before the old
+    // one, the old one if it has lidar, the one after it; map_pose7 = the earliest one's pose) with BuildMapFrame's cell sizes and
+    // SegmentGround threshold, then the reference's four rounds of ScanToMapWithGround / ScanToMapWithSegmented with relocate = true,
+    // from old_pose7 * relative_o_c.  relative_o_c (anything with .data() in the Sophus layout; frame->loop_closure->relative_o_c in
+    // the reference) is the guess on entry and old_pose^-1 * the final pose on return; frame->pose is not touched, nothing is stored
+    // and the resident map frames stay as they were.  Returns (int)(score_ground + score_surf) as mapping.cpp:299 does.
+    // Deviation: where the reference adds a score that was never set (a side whose map frame cloud is empty is skipped in every round)
+    // or that is NaN (no accepted point), this returns 0 -- a rejected candidate -- so that `score - 20` (relocator.cpp:178) cannot
+    // overflow; a sum below -1e9 is returned as -1e9 (the truncation of a larger one is undefined).  A failed library call also
+    // returns 0 and leaves relative_o_c as it was (lvb_last_error() says why).
+    // The call runs on the handles that keep the resident map -- those of the thread that stored the keyframes (AppendKeyframe,
+    // OptimizeKeyframe) -- from whichever thread calls it: the caller serialises it with that thread's device calls
+    // (INTEGRATION.md 3a: Relocator::RelocateByPoints holds backend_->mutex, as Backend::Optimize does around Mapping::Optimize).
+    template <class FramePtr, class Pose>
+    int RelocateKeyframe(FramePtr frame, const long long* keys, int n_keys, const double* map_pose7, const double* old_pose7, Pose& relative_o_c,
+                         double ground_ransac_threshold, lvb_solve_summary* summary = nullptr) {
+        Handles& h = resident_ ? *resident_ : handles_of_thread()[this];
+        if (!ensure_handles(h)) return 0;
+        const auto& g = frame->feature_lidar->points_ground;
+        const auto& s = frame->feature_lidar->points_surf;
+        const int stride = (int)sizeof(assoc_detail::cloud_data(g, 0)[0]);
+        const lvb_map_optimize_params p = MapOptimizeParams(frame, true);
+        const float cells[2] = {cell_of(resolution_ * resolution_ * 100), cell_of(resolution_ * resolution_ * 25)};
+        double rel[7], pose[7], score[2];
+        if (lvb_icp_map_relocate(h.ground, h.surf, keys, n_keys, cells, ground_ransac_threshold, map_pose7, old_pose7, relative_o_c.data(),
+                                 assoc_detail::cloud_data(g, 0), (int)g.size(), assoc_detail::cloud_data(s, 0), (int)s.size(), stride, &p, 4,
+                                 rel, pose, summary, score, nullptr) != LVB_OK)
+            return 0;
+        std::memcpy(relative_o_c.data(), rel, sizeof(rel));
+        const double sum = score[0] + score[1];
+        if (!std::isfinite(sum)) return 0;
+        return (int)std::max(sum, -1e9);
     }
 
 private:
@@ -213,6 +252,7 @@ private:
     }
     static std::unordered_map<const void*, Handles>& handles_of_thread() { static thread_local std::unordered_map<const void*, Handles> m; return m; }
     double resolution_;
+    Handles* resident_ = nullptr;      // the handles that keep the resident keyframe clouds (RelocateKeyframe); map nodes do not move
 };
 
 }  // namespace lvio_fusion

@@ -415,6 +415,32 @@ def build_and_optimize_keyframe(ground, surf, keys, cell_sizes, ground_threshold
     return p, e, (s[0], s[1]), (int(nm[0]), int(nm[1]))
 
 
+def relocate(ground, surf, keys, cell_sizes, ground_threshold, map_pose, old_pose, relative_guess, ground_points, surf_points,
+             weight, huber_a, dist_thr, rounds=4, options=None, **kw):
+    """Mapping::Relocate for one loop-closure candidate (mapping.cpp:78-112, 251-300) in one device call with one host
+    synchronisation (CUDA library only): BuildOldMapFrame of `keys` (1 to 3 keyframes resident on both handles, in time order;
+    map_pose is the earliest one's pose) into a relocation slot of each handle, then `rounds` rounds of both registrations without a
+    prior, starting from old_pose * relative_guess.  Nothing is stored and the handles' map frames stay as they were.  weight, huber_a,
+    dist_thr and cell_sizes are (ground, surf) pairs as for build_and_optimize_keyframe.  Returns (relative_o_c, pose, (ground summary,
+    surf summary), (ground score, surf score), (ground map points, surf map points)) of the last round; a skipped side has
+    termination_type -1 and a NaN score."""
+    if ground is None or surf is None:
+        raise ValueError("relocate: both the ground and the surf handle are needed")
+    api, pts, vp, n, stride, prm = _keyframe_args("relocate", ground, surf, ground_points, surf_points, weight, -1.0, huber_a, dist_thr,
+                                                  options, kw)
+    k = (C.c_longlong * max(1, len(keys)))(*[int(x) for x in keys])
+    cs = np.asarray(cell_sizes, dtype=np.float32).reshape(2).copy()
+    mp, op, rg = (_f64(x).reshape(7) for x in (map_pose, old_pose, relative_guess))
+    rel, p = np.zeros(7), np.zeros(7)
+    s = (SolveSummary * 2)()
+    score = np.zeros(2)
+    nm = np.zeros(2, dtype=np.int32)
+    api.check(api.icp_map_relocate(ground.h, surf.h, k, len(keys), cs.ctypes.data_as(_capi.c_float_p), float(ground_threshold), _dp(mp),
+                                   _dp(op), _dp(rg), vp[0], n[0], vp[1], n[1], stride, C.byref(prm), int(rounds), _dp(rel), _dp(p), s,
+                                   _dp(score), nm.ctypes.data_as(_capi.c_int_p)), "icp_map_relocate")
+    return rel, p, (s[0], s[1]), (float(score[0]), float(score[1])), (int(nm[0]), int(nm[1]))
+
+
 def _fp(a):
     return None if a is None else a.ctypes.data_as(_capi.c_float_p)
 

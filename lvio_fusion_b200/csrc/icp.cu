@@ -498,6 +498,10 @@ struct KfBlock {             // the call's device state, uploaded and read back 
     float tf[8];             // pose.cast<float>(): the query transform of the next association, then of ToWorld
     MapDesc map[2];          // [0] ground, [1] surf map frame: the handles' (uploaded), or built in the call; P = 0: no registration
     int out_bbox[2][6];      // bounding boxes of the two clouds ToWorld stores (lvb_icp_map_build_optimize_keyframe)
+    // lvb_icp_map_relocate (Mapping::Relocate, mapping.cpp:251-300)
+    double old_pose[7];      // last_frame->pose                                  (uploaded)
+    double rel[7];           // relative_o_c: the caller's guess (uploaded), then old_pose^-1 * pose after the last round
+    double score[2];         // score_ground, score_surf of the last round
 };
 struct KfSeed {              // what ScanToMapWith* put in each problem (association.cpp:270-384) and the solver options
     lvb_solve_options o;
@@ -603,6 +607,24 @@ __global__ void icp_kf_pose_kernel(KfBlock* b, int from, int seed, KfSeed p) {
     if (b->map[seed].P == 0) b->st[seed].lm.done = 1;
 }
 
+// Mapping::Relocate's pose arithmetic around its rounds, on one thread with the rounding rules above:
+//   stage 0: clone pose = old_pose * relative_o_c (mapping.cpp:256)
+//   stage 1: relative_o_c = old_pose^-1 * pose (:298), and the scores of the last round (:281-282, :294-295):
+//            min(n / 10, cap) - 2 final_cost / n with n = num_residual_blocks_reduced (no prior: the accepted points), cap 20 for
+//            the ground registration and 30 for the surf one; NaN for a registration that did not run and for n = 0
+__global__ void icp_reloc_pose_kernel(KfBlock* b, int stage) {
+    if (stage == 0) { kf_se3_mul(b->old_pose, b->rel, b->pose); return; }
+    double inv[7];
+    kf_se3_inv(b->old_pose, inv);
+    kf_se3_mul(inv, b->pose, b->rel);
+    for (int m = 0; m < 2; ++m) {
+        const double n = (double)b->st[m].lm.n_accepted;
+        b->score[m] = b->map[m].P > 0 && n > 0.0
+                          ? ds(fmin(__ddiv_rn(n, 10.0), m ? 30.0 : 20.0), __ddiv_rn(dm(2.0, b->st[m].lm.x_cost), n))
+                          : __longlong_as_double(0x7ff8000000000000LL);
+    }
+}
+
 }  // namespace
 
 // ====================================================================================== host side
@@ -627,12 +649,12 @@ struct lvb_icp {
     // device-resident world clouds per keyframe (Mapping::pointclouds_surf / _ground, mapping.cpp:208-219) and the merged map frame
     // lo / hi: the cloud's bounding box (icp_bbox_kernel's), recorded by lvb_icp_map_build_optimize_keyframe for the clouds it stores
     // and computed by it once for the others (has_bbox false)
-    struct Segment { long long key; DevBuf<float4>* pts; int n; bool has_bbox = false; float lo[3], hi[3]; };
+    struct Segment { long long key; DevBuf<float4>* pts = nullptr; int n; bool has_bbox = false; float lo[3], hi[3]; };
     std::vector<Segment> segments;
     DevBuf<float4> merged, merged2;
-    // every build writes its map frame here; it is swapped in only when the build succeeded
-    DevBuf<float4> nx_sorted;
-    DevBuf<int> nx_cell_start, nx_coarse;
+    struct MapBufs { DevBuf<float4> sorted; DevBuf<int> cell_start, coarse; };      // a map frame's sorted cloud and voxel hash
+    MapBufs nx;          // every build writes its map frame here; it is swapped in only when the build succeeded
+    MapBufs reloc;       // lvb_icp_map_relocate's old map frame: reused by every relocation, never swapped in
     int scan_n = 0, scan_stride = 0;          // the scan of the last upload_scan (reusable by lvb_icp_map_append)
     const unsigned char* scan_dev = nullptr;  // where that scan lies: scan_raw, or this handle's part of kf_arena
     // the keyframe calls' upload: [KfBlock | ground scan | surf scan] in one allocation, held by both handles of the call
@@ -739,28 +761,29 @@ static int enqueue_pass(lvb_icp* h, const IcpDev& d) {
 }
 
 // The counting sort by voxel key of the map frame at m (device; icp_map_grid_kernel has decided its grid): its m->P records (stride
-// bytes each, at most n) at d_points into the nx_* buffers.  The cells / coarse counters are cleared with cudaMemsetAsync when they
-// are the map frame's own counts (exact), and by kernels up to m->ncell / m->ncb when they only bound them (map_bound).
-static int enqueue_hash(lvb_icp* h, const unsigned char* d_points, int n, int stride, const MapDesc* m, size_t cells, size_t coarse, bool exact) {
+// bytes each, at most n) at d_points into `out`.  The cells / coarse counters are cleared with cudaMemsetAsync when they are the map
+// frame's own counts (exact), and by kernels up to m->ncell / m->ncb when they only bound them (map_bound).
+static int enqueue_hash(lvb_icp* h, const unsigned char* d_points, int n, int stride, const MapDesc* m, size_t cells, size_t coarse, bool exact,
+                        lvb_icp::MapBufs& out) {
     lvb_ctx* ctx = h->ctx;
     cudaStream_t s = ctx->stream;
     const int nb = inblk(cells, 1024);
     LVB_TRY(h->cell_of.ensure(n)); LVB_TRY(h->counts.ensure(cells)); LVB_TRY(h->fill.ensure(cells));
-    LVB_TRY(h->nx_cell_start.ensure(cells + 1)); LVB_TRY(h->nx_sorted.ensure(n)); LVB_TRY(h->nx_coarse.ensure(coarse));
+    LVB_TRY(out.cell_start.ensure(cells + 1)); LVB_TRY(out.sorted.ensure(n)); LVB_TRY(out.coarse.ensure(coarse));
     LVB_TRY(h->block_sums.ensure(nb)); LVB_TRY(h->total.ensure(1));
     if (exact) {
         LVB_CUDA(cudaMemsetAsync(h->counts.p, 0, cells * sizeof(int), s));
         LVB_CUDA(cudaMemsetAsync(h->fill.p, 0, cells * sizeof(int), s));
-        LVB_CUDA(cudaMemsetAsync(h->nx_coarse.p, 0, coarse * sizeof(int), s));
+        LVB_CUDA(cudaMemsetAsync(out.coarse.p, 0, coarse * sizeof(int), s));
     } else {
         ILAUNCH(h, icp_zero_map_kernel, std::min(inblk(cells, 256), 8 * ctx->sm_count), 256, h->counts.p, h->fill.p, &m->ncell);
-        ILAUNCH(h, icp_zero_map_kernel, std::min(inblk(coarse, 256), 8 * ctx->sm_count), 256, h->nx_coarse.p, (int*)nullptr, &m->ncb);
+        ILAUNCH(h, icp_zero_map_kernel, std::min(inblk(coarse, 256), 8 * ctx->sm_count), 256, out.coarse.p, (int*)nullptr, &m->ncb);
     }
-    ILAUNCH(h, icp_count_kernel, inblk(n, 256), 256, d_points, stride, m, h->cell_of.p, h->counts.p, h->nx_coarse.p);
-    ILAUNCH(h, scan_block_map_kernel, nb, 1024, h->counts.p, h->nx_cell_start.p, &m->ncell, h->block_sums.p);
+    ILAUNCH(h, icp_count_kernel, inblk(n, 256), 256, d_points, stride, m, h->cell_of.p, h->counts.p, out.coarse.p);
+    ILAUNCH(h, scan_block_map_kernel, nb, 1024, h->counts.p, out.cell_start.p, &m->ncell, h->block_sums.p);
     ILAUNCH(h, scan_sums_map_kernel, 1, 1024, h->block_sums.p, &m->ncell, h->total.p);
-    ILAUNCH(h, scan_add_map_kernel, nb, 1024, h->nx_cell_start.p, &m->ncell, h->block_sums.p, h->total.p);
-    ILAUNCH(h, icp_scatter_kernel, inblk(n, 256), 256, d_points, stride, m, h->cell_of.p, h->nx_cell_start.p, h->fill.p, h->nx_sorted.p);
+    ILAUNCH(h, scan_add_map_kernel, nb, 1024, out.cell_start.p, &m->ncell, h->block_sums.p, h->total.p);
+    ILAUNCH(h, icp_scatter_kernel, inblk(n, 256), 256, d_points, stride, m, h->cell_of.p, out.cell_start.p, h->fill.p, out.sorted.p);
     return icheck("map frame build");
 }
 
@@ -788,9 +811,9 @@ static int build_map(lvb_icp* h, const unsigned char* d_points, int n, int strid
     if (m.P == 0 && !m.err) { set_error("%s: the ground plane fit kept no point", fn); return LVB_ERR_NUMERIC; }
     if (n_points) *n_points = m.P;
     LVB_TRY(grid_error(m, fn, ""));
-    LVB_TRY(enqueue_hash(h, d_points, m.P, stride, md, m.ncell, m.ncb, true));
+    LVB_TRY(enqueue_hash(h, d_points, m.P, stride, md, m.ncell, m.ncb, true, h->nx));
     LVB_TRY(host_sync(ctx, s));
-    swap_buf(h->map_sorted, h->nx_sorted); swap_buf(h->cell_start, h->nx_cell_start); swap_buf(h->coarse, h->nx_coarse);
+    swap_buf(h->map_sorted, h->nx.sorted); swap_buf(h->cell_start, h->nx.cell_start); swap_buf(h->coarse, h->nx.coarse);
     h->map = m; h->cell_size = cell_size; h->have_map = true;
     return LVB_OK;
 }
@@ -1026,10 +1049,10 @@ struct KfUpload {
     size_t off[2];                                    // where the scans lie in the arena
 };
 
-// One copy from the pinned staging area: the poses, the two map frames' descriptors (map[m]), and the scans of the handles given.
-// The staging area stays busy until the caller's read-back.
+// One copy from the pinned staging area: the poses (with `reloc`, lvb_icp_map_relocate's old_pose and relative guess), the two map
+// frames' descriptors (map[m]), and the scans of the handles given.  The staging area stays busy until the caller's read-back.
 static int kf_upload(lvb_ctx* ctx, lvb_icp* const hs[2], const double* map_pose, const double* pose, const MapDesc map[2],
-                     const void* const pts[2], const int ns[2], int stride, KfUpload& u) {
+                     const void* const pts[2], const int ns[2], int stride, KfUpload& u, const double* const reloc[2] = nullptr) {
     size_t bytes[2], all = (sizeof(KfBlock) + 255) & ~(size_t)255;
     for (int m = 0; m < 2; ++m) {
         bytes[m] = hs[m] ? (size_t)ns[m] * stride : 0;
@@ -1040,6 +1063,7 @@ static int kf_upload(lvb_ctx* ctx, lvb_icp* const hs[2], const double* map_pose,
     u.hb = reinterpret_cast<KfBlock*>(ctx->stage_h);
     memset(u.hb, 0, sizeof(KfBlock));
     memcpy(u.hb->map_pose, map_pose, sizeof(u.hb->map_pose)); memcpy(u.hb->pose, pose, sizeof(u.hb->pose));
+    if (reloc) { memcpy(u.hb->old_pose, reloc[0], sizeof(u.hb->old_pose)); memcpy(u.hb->rel, reloc[1], sizeof(u.hb->rel)); }
     for (int m = 0; m < 2; ++m) {
         u.hb->map[m] = map[m];
         bbox_seed(u.hb->out_bbox[m]);
@@ -1057,16 +1081,15 @@ static int kf_upload(lvb_ctx* ctx, lvb_icp* const hs[2], const double* map_pose,
 // the sort counters (nc, exact: see bind_scan).
 struct KfMap { const float4* sorted; const int* cell_start; const int* coarse; float cell_size; size_t nc; bool exact; };
 
-// Mapping::Optimize's loop body (mapping.cpp:147-185) for the registrations that run (run[m]): se32rpyxyz, ScanToMapWithGround +
-// Solve, the pose hand-off, ScanToMapWithSegmented + Solve, then ToWorld of the scans of every handle given into fresh[] (not yet
-// stored; with `boxes`, their bounding boxes into blk->out_bbox).  Nothing waits for the host: each registration runs
-// max_num_iterations + 1 LM passes (the kernels return at once after the solver stopped), and the pose kernels write the query
-// transform the next association reads.
+// Mapping::Optimize's loop body (mapping.cpp:147-177), and one round of Mapping::Relocate's (:264-296), for the registrations that
+// run (run[m]): se32rpyxyz of the pose on the device, ScanToMapWithGround + Solve, the pose hand-off, ScanToMapWithSegmented + Solve,
+// the pose hand-off.  Nothing waits for the host: each registration runs max_num_iterations + 1 LM passes (the kernels return at once
+// after the solver stopped), and the pose kernels write the query transform the next association reads.
 static int kf_register(lvb_icp* const hs[2], const bool run[2], const KfMap maps[2], const KfUpload& u, const int ns[2], int stride,
-                       const lvb_map_optimize_params* p, bool boxes, lvb_icp::Segment fresh[2]) {
+                       const lvb_map_optimize_params* p) {
     KfSeed seed;
     seed.o = p->options; seed.prior_w = p->prior_weight;
-    for (int m = 0; m < 2; ++m) { seed.weight[m] = p->weight[m]; seed.huber_a[m] = p->huber_a[m]; fresh[m].pts = nullptr; }
+    for (int m = 0; m < 2; ++m) { seed.weight[m] = p->weight[m]; seed.huber_a[m] = p->huber_a[m]; }
     const int first = run[0] ? 0 : (run[1] ? 1 : -1);
     ILAUNCH(hs[0] ? hs[0] : hs[1], icp_kf_pose_kernel, 1, 1, u.blk, -1, first, seed);      // rpyxyz from the incoming pose (:154)
     for (int m = 0; m < 2; ++m) {
@@ -1084,7 +1107,12 @@ static int kf_register(lvb_icp* const hs[2], const bool run[2], const KfMap maps
         // pose = map_pose * rpyxyz2se3(rpyxyz) (:165, :177); after the ground solve it also seeds the surf registration
         ILAUNCH(h, icp_kf_pose_kernel, 1, 1, u.blk, m, m == 0 && run[1] ? 1 : -1, seed);
     }
-    // ToWorld (:205-220): the robot-frame clouds, transformed by the final pose.cast<float>()
+    return LVB_OK;
+}
+
+// The end of Mapping::Optimize's loop body: ToWorld (:185, :205-220) of the scans of every handle given, transformed by the final
+// pose.cast<float>(), into fresh[] (not yet stored; with `boxes`, their bounding boxes into blk->out_bbox)
+static int kf_to_world(lvb_icp* const hs[2], const KfUpload& u, const int ns[2], int stride, bool boxes, lvb_icp::Segment fresh[2]) {
     for (int m = 0; m < 2; ++m) {
         if (!hs[m]) continue;
         fresh[m].key = -1; fresh[m].n = ns[m]; fresh[m].pts = new DevBuf<float4>();
@@ -1141,7 +1169,8 @@ int lvb_icp_map_optimize_keyframe(lvb_icp* ground, lvb_icp* surf, const double m
     KfUpload u;
     LVB_TRY(kf_upload(ctx, hs, map_pose, pose, desc, pts, ns, stride, u));
     lvb_icp::Segment fresh[2];
-    LVB_TRY(kf_register(hs, run, maps, u, ns, stride, p, false, fresh));
+    LVB_TRY(kf_register(hs, run, maps, u, ns, stride, p));
+    LVB_TRY(kf_to_world(hs, u, ns, stride, false, fresh));
     int rc = icheck("map_optimize_keyframe");
     if (rc != LVB_OK) { delete fresh[0].pts; delete fresh[1].pts; return rc; }
     for (int m = 0; m < 2; ++m) if (hs[m]) store_segment(hs[m], key, fresh[m]);
@@ -1213,6 +1242,95 @@ static MapBound map_bound(const float* lo, const float* hi, float cell_size) {
     return b;
 }
 
+// The map frame of `keys` (BuildMapFrame, mapping.cpp:114-137; BuildOldMapFrame, :78-112) on both handles: the resident clouds in
+// merge order, the merged sizes, which side is built (an empty merged cloud: BuildMapFrame fails on that side and nothing registers,
+// :155,167), the descriptor seeds and the capacity bounds of the builds.  The missing bounding boxes of both handles are computed here,
+// with one synchronisation.
+struct KfPlan { std::vector<lvb_icp::Segment*> pick[2]; size_t total[2] = {0, 0}; bool build[2]; MapBound bound[2]; MapDesc seed[2]; };
+static int kf_plan(lvb_icp* const hs[2], const long long* keys, int n_keys, const float cell_size[2], bool ransac, const char* fn, KfPlan& pl) {
+    for (int k = 0; k < n_keys; ++k) {
+        for (int m = 0; m < 2; ++m) {
+            lvb_icp::Segment* f = nullptr;
+            for (auto& sg : hs[m]->segments) if (sg.key == keys[k]) f = &sg;
+            if (!f) { set_error("%s: key %lld is not resident", fn, keys[k]); return LVB_ERR_INVALID; }
+            pl.pick[m].push_back(f); pl.total[m] += f->n;
+        }
+    }
+    if (pl.total[0] > 0x7fffffffull || pl.total[1] > 0x7fffffffull) { set_error("%s: map frame of more than 2^31 points", fn); return LVB_ERR_INVALID; }
+    {   // both handles' missing boxes with one synchronisation
+        std::vector<lvb_icp::Segment*> both(pl.pick[0]);
+        both.insert(both.end(), pl.pick[1].begin(), pl.pick[1].end());
+        LVB_TRY(fill_bboxes(hs[0], both));
+    }
+    for (int m = 0; m < 2; ++m) {
+        pl.build[m] = pl.total[m] > 0;
+        pl.seed[m] = desc_seed(pl.build[m] && !(m == 0 && ransac) ? (int)pl.total[m] : 0);      // the ground count comes from SegmentGround
+        if (!pl.build[m]) continue;
+        float lo[3] = {FLT_MAX, FLT_MAX, FLT_MAX}, hi[3] = {-FLT_MAX, -FLT_MAX, -FLT_MAX};
+        for (auto* sg : pl.pick[m]) for (int a = 0; a < 3; ++a) { lo[a] = std::min(lo[a], sg->lo[a]); hi[a] = std::max(hi[a], sg->hi[a]); }
+        pl.bound[m] = map_bound(lo, hi, cell_size[m]);
+        // without SegmentGround the map frame's box is the union: the grid kernel's check can be made here (after it, on the device)
+        if (!pl.bound[m].finite && !(m == 0 && ransac)) { set_error("%s: map cloud has no finite bounding box", fn); return LVB_ERR_INVALID; }
+    }
+    return LVB_OK;
+}
+
+// The builds of a plan: merge in key order, SegmentGround on the ground side (ground_threshold > 0), voxel hash sized by the bound into
+// the handle's buffers `slot`, grid decided on the device into u.blk->map[m].  maps[m]: what registration m reads of it.
+static int kf_build(lvb_icp* const hs[2], const KfPlan& pl, const float cell_size[2], double ground_threshold, const KfUpload& u,
+                    lvb_icp::MapBufs lvb_icp::* slot, KfMap maps[2]) {
+    lvb_ctx* ctx = hs[0]->ctx;
+    cudaStream_t s = ctx->stream;
+    for (int m = 0; m < 2; ++m) {
+        if (!pl.build[m]) continue;
+        lvb_icp* h = hs[m];
+        lvb_icp::MapBufs& out = h->*slot;
+        MapDesc* md = &u.blk->map[m];
+        const int n = (int)pl.total[m];
+        LVB_TRY(h->merged.ensure(n));
+        size_t o = 0;
+        for (auto* f : pl.pick[m]) { if (f->n) LVB_CUDA(cudaMemcpyAsync(h->merged.p + o, f->pts->p, (size_t)f->n * sizeof(float4), cudaMemcpyDeviceToDevice, s)); o += f->n; }
+        const float4* cloud = h->merged.p;
+        if (m == 0 && ground_threshold > 0.0) {
+            LVB_TRY(h->merged2.ensure(n));
+            LVB_TRY(lidar_segment_ground_device_async(ctx, h->merged.p, n, ground_threshold, h->merged2.p, &md->P));
+            lvb::g_alloc_stream = ctx->stream;
+            cloud = h->merged2.p;
+        }
+        const unsigned char* cp = reinterpret_cast<const unsigned char*>(cloud);
+        ILAUNCH(h, icp_bbox_kernel, std::min(1024, inblk(n, 256)), 256, cp, 16, md);
+        ILAUNCH(h, icp_map_grid_kernel, 1, 1, md, cell_size[m]);
+        LVB_TRY(enqueue_hash(h, cp, n, 16, md, pl.bound[m].cells, pl.bound[m].coarse, false, out));
+        maps[m] = {out.sorted.p, out.cell_start.p, out.coarse.p, cell_size[m], pl.bound[m].qsort, false};
+    }
+    return LVB_OK;
+}
+
+// The scan a handle's lvb_icp_map_append(NULL) refers to (bind_scan moves it to the registration's scan)
+struct ScanState {
+    int n, stride; const unsigned char* dev; std::shared_ptr<DevBuf<unsigned char>> arena;
+    void save(const lvb_icp* h) { n = h->scan_n; stride = h->scan_stride; dev = h->scan_dev; arena = h->kf_arena; }
+    void restore(lvb_icp* h) const { h->scan_n = n; h->scan_stride = stride; h->scan_dev = dev; h->kf_arena = arena; }
+};
+
+// The argument checks both map-building calls share; they come before any state changes
+static int kf_check_args(lvb_icp* const hs[2], const float cell_size[2], const void* const pts[2], const int ns[2], int stride,
+                         const lvb_map_optimize_params* p, const char* fn) {
+    lvb_ctx* ctx = hs[0]->ctx;
+    if (hs[1]->ctx != ctx) { set_error("%s: the two handles belong to different contexts", fn); return LVB_ERR_INVALID; }
+    if (ctx->world > 1) { set_error("%s: sharded contexts register through lvb_icp_scan_to_map", fn); return LVB_ERR_UNSUPPORTED; }
+    const lvb_solve_options& opt = p->options;
+    if (opt.max_solver_time_in_seconds < 1e8) { set_error("%s: no time limit (Mapping::Optimize and Mapping::Relocate set none)", fn); return LVB_ERR_INVALID; }
+    if (opt.max_num_iterations < 0 || stride < 12 || (stride & 3)) { set_error("%s: bad arguments", fn); return LVB_ERR_INVALID; }
+    for (int m = 0; m < 2; ++m) {
+        if (ns[m] < 0 || (ns[m] && !pts[m])) { set_error("%s: bad scan arguments", fn); return LVB_ERR_INVALID; }
+        if (!(cell_size[m] > 0.0f)) { set_error("%s: bad cell size", fn); return LVB_ERR_INVALID; }
+        if ((double)cell_size[m] * cell_size[m] * (1.0 + 1e-6) < p->dist_thr[m]) {
+            set_error("%s: dist_thr %.6g exceeds cell_size^2 %.6g", fn, p->dist_thr[m], (double)cell_size[m] * cell_size[m]); return LVB_ERR_INVALID; }
+    }
+    return LVB_OK;
+}
+
 // Mapping::BuildMapFrame (mapping.cpp:114-137) + the body of Mapping::Optimize's loop (:147-185) for one keyframe.  The host knows
 // every size the launches depend on -- the scans, the merged clouds (sums of resident cloud sizes), max_num_iterations -- and an upper
 // bound on each map frame's grid (map_bound of the union of the resident clouds' boxes); the device decides the grid itself
@@ -1227,104 +1345,46 @@ int lvb_icp_map_build_optimize_keyframe(lvb_icp* ground, lvb_icp* surf, const lo
     const int ns[2] = {n_ground, n_surf};
     if (!ground || !surf || ground == surf || !cell_size || !map_pose || !p || !pose || !rpyxyz || n_keys < 0 || (n_keys && !keys)) {
         set_error("%s: null or bad argument", fn); return LVB_ERR_INVALID; }
+    LVB_TRY(kf_check_args(hs, cell_size, pts, ns, stride, p, fn));
     lvb_ctx* ctx = ground->ctx;
-    if (surf->ctx != ctx) { set_error("%s: the two handles belong to different contexts", fn); return LVB_ERR_INVALID; }
-    if (ctx->world > 1) { set_error("%s: sharded contexts register through lvb_icp_scan_to_map", fn); return LVB_ERR_UNSUPPORTED; }
-    const lvb_solve_options& opt = p->options;
-    if (opt.max_solver_time_in_seconds < 1e8) { set_error("%s: no time limit (Mapping::Optimize sets none)", fn); return LVB_ERR_INVALID; }
-    if (opt.max_num_iterations < 0 || stride < 12 || (stride & 3)) { set_error("%s: bad arguments", fn); return LVB_ERR_INVALID; }
-    for (int m = 0; m < 2; ++m) {
-        if (ns[m] < 0 || (ns[m] && !pts[m])) { set_error("%s: bad scan arguments", fn); return LVB_ERR_INVALID; }
-        if (!(cell_size[m] > 0.0f)) { set_error("%s: bad cell size", fn); return LVB_ERR_INVALID; }
-        if ((double)cell_size[m] * cell_size[m] * (1.0 + 1e-6) < p->dist_thr[m]) {
-            set_error("%s: dist_thr %.6g exceeds cell_size^2 %.6g", fn, p->dist_thr[m], (double)cell_size[m] * cell_size[m]); return LVB_ERR_INVALID; }
-    }
     // the map frame: keys resident on both handles, in merge order; `key` is the keyframe being registered, not one of them
-    std::vector<lvb_icp::Segment*> pick[2];
-    size_t total[2] = {0, 0};
-    for (int k = 0; k < n_keys; ++k) {
+    for (int k = 0; k < n_keys; ++k)
         if (keys[k] == key) { set_error("%s: key %lld is one of the map frame's keys", fn, key); return LVB_ERR_INVALID; }
-        for (int m = 0; m < 2; ++m) {
-            lvb_icp::Segment* f = nullptr;
-            for (auto& sg : hs[m]->segments) if (sg.key == keys[k]) f = &sg;
-            if (!f) { set_error("%s: key %lld is not resident", fn, keys[k]); return LVB_ERR_INVALID; }
-            pick[m].push_back(f); total[m] += f->n;
-        }
-    }
-    if (total[0] > 0x7fffffffull || total[1] > 0x7fffffffull) { set_error("%s: map frame of more than 2^31 points", fn); return LVB_ERR_INVALID; }
     LVB_CUDA(cudaSetDevice(ctx->device)); lvb::g_alloc_stream = ctx->stream;
-    {   // both handles' missing boxes with one synchronisation
-        std::vector<lvb_icp::Segment*> both(pick[0]);
-        both.insert(both.end(), pick[1].begin(), pick[1].end());
-        LVB_TRY(fill_bboxes(ground, both));
-    }
-    const bool ransac = ground_threshold > 0.0;
-    bool build[2];
-    MapBound bound[2];
-    MapDesc seed[2];
-    for (int m = 0; m < 2; ++m) {
-        build[m] = total[m] > 0;           // an empty merged cloud: BuildMapFrame fails on that side and nothing registers (:155,167)
-        seed[m] = desc_seed(build[m] && !(m == 0 && ransac) ? (int)total[m] : 0);      // the ground count comes from SegmentGround
-        if (!build[m]) continue;
-        float lo[3] = {FLT_MAX, FLT_MAX, FLT_MAX}, hi[3] = {-FLT_MAX, -FLT_MAX, -FLT_MAX};
-        for (auto* sg : pick[m]) for (int a = 0; a < 3; ++a) { lo[a] = std::min(lo[a], sg->lo[a]); hi[a] = std::max(hi[a], sg->hi[a]); }
-        bound[m] = map_bound(lo, hi, cell_size[m]);
-        // without SegmentGround the map frame's box is the union: the grid kernel's check can be made here (after it, on the device)
-        if (!bound[m].finite && !(m == 0 && ransac)) { set_error("%s: map cloud has no finite bounding box", fn); return LVB_ERR_INVALID; }
-    }
+    KfPlan pl;
+    LVB_TRY(kf_plan(hs, keys, n_keys, cell_size, ground_threshold > 0.0, fn, pl));
     const auto t0 = std::chrono::steady_clock::now();
     cudaStream_t s = ctx->stream;
     lvb::timing_mark(s, "begin");
     KfUpload u;
-    LVB_TRY(kf_upload(ctx, hs, map_pose, pose, seed, pts, ns, stride, u));
-
-    // BuildMapFrame: merge in key order, SegmentGround on the ground side, voxel hash sized by the bound, grid decided on the device
+    LVB_TRY(kf_upload(ctx, hs, map_pose, pose, pl.seed, pts, ns, stride, u));
     KfMap maps[2];
-    for (int m = 0; m < 2; ++m) {
-        if (!build[m]) continue;
-        lvb_icp* h = hs[m];
-        MapDesc* md = &u.blk->map[m];
-        const int n = (int)total[m];
-        LVB_TRY(h->merged.ensure(n));
-        size_t o = 0;
-        for (auto* f : pick[m]) { if (f->n) LVB_CUDA(cudaMemcpyAsync(h->merged.p + o, f->pts->p, (size_t)f->n * sizeof(float4), cudaMemcpyDeviceToDevice, s)); o += f->n; }
-        const float4* cloud = h->merged.p;
-        if (m == 0 && ransac) {
-            LVB_TRY(h->merged2.ensure(n));
-            LVB_TRY(lidar_segment_ground_device_async(ctx, h->merged.p, n, ground_threshold, h->merged2.p, &md->P));
-            lvb::g_alloc_stream = ctx->stream;
-            cloud = h->merged2.p;
-        }
-        const unsigned char* cp = reinterpret_cast<const unsigned char*>(cloud);
-        ILAUNCH(h, icp_bbox_kernel, std::min(1024, inblk(n, 256)), 256, cp, 16, md);
-        ILAUNCH(h, icp_map_grid_kernel, 1, 1, md, cell_size[m]);
-        LVB_TRY(enqueue_hash(h, cp, n, 16, md, bound[m].cells, bound[m].coarse, false));
-        maps[m] = {h->nx_sorted.p, h->nx_cell_start.p, h->nx_coarse.p, cell_size[m], bound[m].qsort, false};
-    }
+    LVB_TRY(kf_build(hs, pl, cell_size, ground_threshold, u, &lvb_icp::nx, maps));
 
     // the registrations, each against the map frame just built
-    struct ScanState { int n, stride; const unsigned char* dev; std::shared_ptr<DevBuf<unsigned char>> arena; } saved[2];
-    for (int m = 0; m < 2; ++m) saved[m] = {hs[m]->scan_n, hs[m]->scan_stride, hs[m]->scan_dev, hs[m]->kf_arena};
+    ScanState saved[2];
+    for (int m = 0; m < 2; ++m) saved[m].save(hs[m]);
     lvb_icp::Segment fresh[2];
-    int rc = kf_register(hs, build, maps, u, ns, stride, p, true, fresh);
+    int rc = kf_register(hs, pl.build, maps, u, ns, stride, p);
+    if (rc == LVB_OK) rc = kf_to_world(hs, u, ns, stride, true, fresh);
     if (rc == LVB_OK) rc = icheck("map_build_optimize_keyframe");
     // the one read-back: solver states, pose, rpyxyz, both map descriptors (grid, point count, failure), the stored clouds' boxes
     if (rc == LVB_OK && cudaMemcpyAsync(u.hb, u.blk, sizeof(KfBlock), cudaMemcpyDeviceToHost, s) != cudaSuccess) rc = lvb::cuda_fail(cudaGetLastError(), "read-back", __FILE__, __LINE__);
     if (rc == LVB_OK) rc = host_sync(ctx, s);
     if (rc == LVB_OK) ctx->stage_busy = false;
-    for (int m = 0; m < 2 && rc == LVB_OK; ++m) if (build[m]) rc = grid_error(u.hb->map[m], fn, m ? "surf " : "ground ");
+    for (int m = 0; m < 2 && rc == LVB_OK; ++m) if (pl.build[m]) rc = grid_error(u.hb->map[m], fn, m ? "surf " : "ground ");
     if (rc != LVB_OK) {        // nothing was committed: the resident clouds and the map frames are as they were
         delete fresh[0].pts; delete fresh[1].pts;
-        for (int m = 0; m < 2; ++m) { hs[m]->scan_n = saved[m].n; hs[m]->scan_stride = saved[m].stride; hs[m]->scan_dev = saved[m].dev; hs[m]->kf_arena = saved[m].arena; }
+        for (int m = 0; m < 2; ++m) saved[m].restore(hs[m]);
         return rc;
     }
     const double el = std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
     for (int m = 0; m < 2; ++m) {
         lvb_icp* h = hs[m];
         const MapDesc& md = u.hb->map[m];
-        const bool built = build[m] && md.P > 0;
+        const bool built = pl.build[m] && md.P > 0;
         if (built) {           // the new map frame replaces the one before, as lvb_icp_map_build would
-            swap_buf(h->map_sorted, h->nx_sorted); swap_buf(h->cell_start, h->nx_cell_start); swap_buf(h->coarse, h->nx_coarse);
+            swap_buf(h->map_sorted, h->nx.sorted); swap_buf(h->cell_start, h->nx.cell_start); swap_buf(h->coarse, h->nx.coarse);
             h->map = md; h->cell_size = cell_size[m]; h->have_map = true;
         }
         bbox_store(fresh[m], u.hb->out_bbox[m]);
@@ -1337,6 +1397,66 @@ int lvb_icp_map_build_optimize_keyframe(lvb_icp* ground, lvb_icp* surf, const lo
         }
     }
     memcpy(pose, u.hb->pose, sizeof(u.hb->pose)); memcpy(rpyxyz, u.hb->rpyxyz, sizeof(u.hb->rpyxyz));
+    return LVB_OK;
+}
+
+// ---- Mapping::Relocate for one loop-closure candidate (mapping.cpp:251-300): BuildOldMapFrame (:78-112) into each handle's
+// relocation slot, then `rounds` rounds of both registrations without a prior, all on the device.  The same sizes are known on the host
+// as in lvb_icp_map_build_optimize_keyframe; one pinned upload, one read-back, one host synchronisation.  Nothing is stored and the
+// handles' map frames, resident clouds and map_append(NULL) scan stay as they were.
+int lvb_icp_map_relocate(lvb_icp* ground, lvb_icp* surf, const long long* keys, int n_keys, const float cell_size[2], double ground_threshold,
+                         const double map_pose[7], const double old_pose[7], const double relative_guess[7],
+                         const void* ground_pts, int n_ground, const void* surf_pts, int n_surf, int stride,
+                         const lvb_map_optimize_params* p, int rounds, double relative_o_c[7], double pose[7],
+                         lvb_solve_summary summary[2], double score[2], int n_map_points[2]) {
+    static const char* fn = "lvb_icp_map_relocate";
+    lvb_icp* hs[2] = {ground, surf};
+    const void* pts[2] = {ground_pts, surf_pts};
+    const int ns[2] = {n_ground, n_surf};
+    if (!ground || !surf || ground == surf || !keys || !cell_size || !map_pose || !old_pose || !relative_guess || !p || !relative_o_c || !pose) {
+        set_error("%s: null or bad argument", fn); return LVB_ERR_INVALID; }
+    if (n_keys < 1 || n_keys > 3) { set_error("%s: the old map frame has 1 to 3 keyframes, got %d", fn, n_keys); return LVB_ERR_INVALID; }
+    if (rounds < 1 || rounds > 16) { set_error("%s: rounds %d outside 1..16", fn, rounds); return LVB_ERR_INVALID; }
+    LVB_TRY(kf_check_args(hs, cell_size, pts, ns, stride, p, fn));
+    if (!(p->prior_weight < 0.0)) { set_error("%s: prior_weight must be < 0 (ScanToMapWith* with relocate = true add no prior)", fn); return LVB_ERR_INVALID; }
+    lvb_ctx* ctx = ground->ctx;
+    LVB_CUDA(cudaSetDevice(ctx->device)); lvb::g_alloc_stream = ctx->stream;
+    KfPlan pl;
+    LVB_TRY(kf_plan(hs, keys, n_keys, cell_size, ground_threshold > 0.0, fn, pl));
+    const auto t0 = std::chrono::steady_clock::now();
+    cudaStream_t s = ctx->stream;
+    lvb::timing_mark(s, "begin");
+    KfUpload u;
+    const double* reloc[2] = {old_pose, relative_guess};
+    LVB_TRY(kf_upload(ctx, hs, map_pose, old_pose /* replaced on the device by old_pose * relative_guess */, pl.seed, pts, ns, stride, u, reloc));
+    KfMap maps[2];
+    LVB_TRY(kf_build(hs, pl, cell_size, ground_threshold, u, &lvb_icp::reloc, maps));
+
+    ScanState saved[2];
+    for (int m = 0; m < 2; ++m) saved[m].save(hs[m]);
+    int rc = LVB_OK;
+    ILAUNCH(ground, icp_reloc_pose_kernel, 1, 1, u.blk, 0);
+    for (int r = 0; r < rounds && rc == LVB_OK; ++r) rc = kf_register(hs, pl.build, maps, u, ns, stride, p);
+    if (rc == LVB_OK) ILAUNCH(ground, icp_reloc_pose_kernel, 1, 1, u.blk, 1);
+    if (rc == LVB_OK) rc = icheck(fn);
+    // the one read-back: solver states, pose, relative_o_c, scores, both map descriptors (grid, point count, failure)
+    if (rc == LVB_OK && cudaMemcpyAsync(u.hb, u.blk, sizeof(KfBlock), cudaMemcpyDeviceToHost, s) != cudaSuccess) rc = lvb::cuda_fail(cudaGetLastError(), "read-back", __FILE__, __LINE__);
+    if (rc == LVB_OK) rc = host_sync(ctx, s);
+    if (rc == LVB_OK) ctx->stage_busy = false;
+    for (int m = 0; m < 2; ++m) saved[m].restore(hs[m]);
+    for (int m = 0; m < 2 && rc == LVB_OK; ++m) if (pl.build[m]) rc = grid_error(u.hb->map[m], fn, m ? "surf " : "ground ");
+    if (rc != LVB_OK) return rc;
+    const double el = std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
+    for (int m = 0; m < 2; ++m) {
+        const bool built = pl.build[m] && u.hb->map[m].P > 0;
+        if (n_map_points) n_map_points[m] = built ? u.hb->map[m].P : 0;
+        if (score) score[m] = u.hb->score[m];
+        if (summary) {
+            if (built) fill_summary(u.hb->st[m], p->prior_weight, el, &summary[m]);
+            else { memset(&summary[m], 0, sizeof(summary[m])); summary[m].termination_type = -1; }
+        }
+    }
+    memcpy(pose, u.hb->pose, sizeof(u.hb->pose)); memcpy(relative_o_c, u.hb->rel, sizeof(u.hb->rel));
     return LVB_OK;
 }
 

@@ -460,6 +460,12 @@ def se3_mul(a, b):
     return np.concatenate([q / np.linalg.norm(q), se3_apply(a, b[4:])])
 
 
+def se3_inv(a):
+    """Sophus SE3 inverse of a pose [qx qy qz qw tx ty tz]."""
+    q = np.array([-a[0], -a[1], -a[2], a[3]]) / np.linalg.norm(a[:4])
+    return np.concatenate([q, se3_inv_apply(a, np.zeros(3))])
+
+
 def make_lidar_scan(seed=SEED, num_scans=64, horizon_scan=1800, ang_res_y=0.427, ang_bottom=24.9, sensor_height=1.73,
                     sigma=0.01, dropout=0.02, n_boxes=14):
     """One revolution of a KITTI-like 64-beam spinning lidar (kitti.yaml:35-42) in the sensor frame (z up).
