@@ -61,6 +61,7 @@ struct BaDev {
     double *S, *rhs, *gcr, *diagH, *scal;      // inside the arena
     double *scale_c, *scale_l, *lam_c, *lam_l;
     LmState* st;
+    unsigned int* cta_done;             // last-CTA-done counters: [0] ba_schur_kernel, [1] ba_linearize_all_kernel<1> (zero between launches)
     int rank0, rank, world;
     int stage_poses;
     int imu_cta;                        // 1: one CTA per IMU factor (window-sized problems: latency), 0: one warp per factor (map scale)
@@ -124,6 +125,34 @@ __device__ __forceinline__ void block_add(double v, double* target, double* s_re
         if (lane == 0 && t != 0.0) atomicAdd(target, t);
     }
     __syncthreads();
+}
+
+// Last-CTA-done (as in lvb_p2p.cuh): every CTA of the grid arrives once, after its global writes; the CTA that arrives last sees
+// all of them and resets the counter for the next launch.  True in every thread of that CTA.
+__device__ __forceinline__ bool arrive_last(unsigned int* counter) {
+    __shared__ int s_last;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        __threadfence();
+        const int last = atomicAdd(counter, 1u) == gridDim.x - 1;
+        if (last) { *counter = 0u; __threadfence(); }
+        s_last = last;
+    }
+    __syncthreads();
+    return s_last != 0;
+}
+
+// The LM state as a block-wide copy in shared memory: every field loaded at once from L2 (the accumulators were written with
+// atomics), the decision then runs on shared memory instead of a chain of dependent L2 round trips, and the copy goes back whole.
+// Only for a CTA that no other thread of the grid can race with (the last one to arrive).
+static_assert(sizeof(LmState) % 8 == 0 && sizeof(LmState) / 8 <= TPB, "LmState is copied as 8-byte words, one per thread");
+__device__ __forceinline__ void lm_state_load(LmState* s, const LmState* g) {
+    if (threadIdx.x < sizeof(LmState) / 8) reinterpret_cast<unsigned long long*>(s)[threadIdx.x] = __ldcg(reinterpret_cast<const unsigned long long*>(g) + threadIdx.x);
+    __syncthreads();
+}
+__device__ __forceinline__ void lm_state_store(LmState* g, const LmState* s) {
+    __syncthreads();
+    if (threadIdx.x < sizeof(LmState) / 8) reinterpret_cast<unsigned long long*>(g)[threadIdx.x] = reinterpret_cast<const unsigned long long*>(s)[threadIdx.x];
 }
 
 // H(lower) += JA^T JB for two distinct blocks; offsets are global camera-system offsets (>= 0)
@@ -652,27 +681,47 @@ __device__ __forceinline__ void linearize_other_body(const BaDev& d, const Block
 template <int MODE>
 __global__ void __launch_bounds__(TPB) ba_linearize_other_kernel(BaDev d, BlockRanges R) { linearize_other_body<MODE>(d, R, blockIdx.x + R.b[3]); }
 
+// The LM decision of a single-GPU window pass, in the last CTA of the cost kernel (the candidate cost is complete).  What the
+// decision implies -- candidate -> x, clearing the accumulators -- is left to ba_post_wide_kernel over a whole grid: on the one CTA
+// it took longer than the kernel it would save (window of 10 keyframes: 10 us in this CTA, 20 keyframes: 24 us).
+__device__ __forceinline__ void decide_step_last_cta(const BaDev& d) {
+    __shared__ LmState s;
+    lm_state_load(&s, d.st);
+    if (threadIdx.x == 0) { lm_control_post(s); if (s.accept) s.x_cost = s.cand_cost_acc; }
+    lm_state_store(d.st, &s);
+}
+
 // Window-sized problems: ONE launch for all factor kinds.  The IMU blocks are a long single-warp dependency chain (~20 us) and the
 // visual blocks a short wide one; in one grid -- IMU and priors first so they start at once -- they overlap instead of running
 // back to back, and a launch is saved.  (At map scale the visual kernel's occupancy matters and the kernels stay separate.)
+// decide (MODE 1, single GPU): the kernel also closes the pass.  Every CTA clears its share of S and rhs, which the next pass's
+// ba_schur_kernel assembles into from zero whatever the decision; the last CTA to finish decides the step (decide_step_last_cta).
 template <int MODE>
-__global__ void __launch_bounds__(TPB) ba_linearize_all_kernel(BaDev d, BlockRanges R) {
+__global__ void __launch_bounds__(TPB) ba_linearize_all_kernel(BaDev d, BlockRanges R, int decide) {
+    if (MODE == 1 && d.st->done) return;            // uniform: only the last CTA below writes `done`
     const int n_other = R.b[6] - R.b[3];
     if ((int)blockIdx.x < n_other) linearize_other_body<MODE>(d, R, (int)blockIdx.x + R.b[3]);
     else linearize_visual_body<MODE>(d, R, (int)blockIdx.x - n_other);
+    if (MODE == 1 && decide) {
+        const size_t n = d.nS + (size_t)d.dimc;     // S, then rhs: adjacent in the arena
+        for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) d.S[i] = 0.0;
+        if (arrive_last(d.cta_done + 1)) decide_step_last_cta(d);
+    }
 }
 
 // ------------------------------------------------------------------ per-iteration system assembly
-__global__ void ba_zero_kernel(BaDev d) {
+// zero_S: the pass assembles S and rhs from zero (ba_schur_kernel with `assemble`); later passes get them cleared by the cost kernel
+__global__ void ba_zero_kernel(BaDev d, int zero_S) {
     const LmState* st = d.st;
     if (st->done || !st->need_linearize) return;
     const size_t nH = d.nS;
-    const size_t total = nH + d.dimc + 2 * (size_t)d.n_rho;
-    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
+    const size_t total = nH + d.dimc + 2 * (size_t)d.n_rho, nA = zero_S ? nH + d.dimc : 0;
+    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total + nA; i += (size_t)gridDim.x * blockDim.x) {
         if (i < nH) d.Hpp[i] = 0.0;
         else if (i < nH + d.dimc) d.gc[i - nH] = 0.0;
         else if (i < nH + d.dimc + d.n_rho) d.Hll[i - nH - d.dimc] = 0.0;
-        else d.gl[i - nH - d.dimc - d.n_rho] = 0.0;
+        else if (i < total) d.gl[i - nH - d.dimc - d.n_rho] = 0.0;
+        else d.S[i - total] = 0.0;              // S, then rhs
     }
 }
 
@@ -686,12 +735,9 @@ __device__ __forceinline__ void atomic_max_nonneg(unsigned long long* p, double 
 // (finalize() groups and pads them).  Lane l writes u_l = sqrt(1/h_l) [w_l | g_l] (its couplings merged by
 // pose slot) as a row of a shared-memory tile; the warp then forms the lower triangle of U^T U and subtracts
 // it from S / adds the last column to rhs with one red.global per entry:  S -= sum_l w_l^T w_l / h_l.
-__global__ void __launch_bounds__(TPB) ba_schur_kernel(BaDev d, int cols_max) {
+__device__ __forceinline__ void schur_warp(const BaDev& d, int cols_max, int w) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
-    if (d.st->done) return;
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    const int w = blockIdx.x * (TPB / 32) + warp;
-    if (w >= d.n_schur_warps) return;
     const int g = d.sw_group[w];
     const int ns = d.grp_ns[g];
     const int ncol = 6 * ns + 1;
@@ -787,6 +833,93 @@ __global__ void __launch_bounds__(TPB) ba_schur_kernel(BaDev d, int cols_max) {
         if (a == ncol - 1) { atomicAdd(&d.rhs[gb], v); continue; }
         const int ga = offs[a / 6] + a % 6;
         if (ga >= gb) atomicAdd(&d.S[SIDX(d, ga, gb)], -v); else atomicAdd(&d.S[SIDX(d, gb, ga)], -v);
+    }
+}
+
+__device__ __forceinline__ void warp_max_to_state(LmState* st, unsigned long long bits) {
+    for (int o = 16; o > 0; o >>= 1) { const unsigned long long v = __shfl_xor_sync(0xffffffffu, bits, o); bits = v > bits ? v : bits; }
+    if ((threadIdx.x & 31) == 0 && bits) atomicMax(&st->grad_max_bits, bits);
+}
+
+// One camera block of the single-GPU pass, read from Hpp and gc directly, every load issued before the first use: Jacobi scale
+// (first pass), damping, gcr, diagH, and the block's rows of the system -- S[diag] += H_kk + lambda_k and rhs += -g_k by red.add --
+// then the gradient max-norm ||x - Plus(x, -g)||_inf as ordered bits (0: nothing to report).  Same arithmetic as
+// ba_build_S_kernel<1> + prepare_camera_block, which the other passes use.
+__device__ __forceinline__ unsigned long long assemble_camera_block(const BaDev& d, int i) {
+    const LmState* st = d.st;
+    const bool is_pose = i < d.n_poses;
+    const int off = is_pose ? d.pose_off[i] : d.vec3_off[i - d.n_poses];
+    if (off < 0) return 0ull;
+    const int w = is_pose ? 6 : 3;
+    const int scale_valid = st->scale_valid, jacobi = st->jacobi, need_lin = st->need_linearize;
+    const double min_diag = st->min_diag, max_diag = st->max_diag, radius = st->radius;
+    double h[6], g[6], sc[6], x[7];
+#pragma unroll
+    for (int k = 0; k < 6; ++k) {
+        const bool in = k < w;
+        h[k] = in ? d.Hpp[SIDX(d, off + k, off + k)] : 0.0;
+        g[k] = in ? d.gc[off + k] : 0.0;
+        sc[k] = (in && scale_valid) ? d.scale_c[off + k] : 1.0;
+    }
+#pragma unroll
+    for (int k = 0; k < 7; ++k) x[k] = (is_pose && need_lin) ? d.poses[7 * i + k] : 0.0;
+#pragma unroll
+    for (int k = 0; k < 6; ++k) {
+        if (k >= w) break;
+        const int r = off + k;
+        const double s = scale_valid ? sc[k] : (jacobi ? 1.0 / (1.0 + sqrt(h[k])) : 1.0), s2 = s * s;
+        if (!scale_valid) d.scale_c[r] = s;
+        const double lam = fmin(fmax(s2 * h[k], min_diag), max_diag) / (radius * s2);
+        d.lam_c[r] = lam; d.diagH[r] = h[k]; d.gcr[r] = g[k];
+        atomicAdd(&d.S[SIDX(d, r, r)], h[k] + lam);
+        atomicAdd(&d.rhs[r], -g[k]);
+    }
+    if (!need_lin) return 0ull;
+    double gm = 0.0;
+    if (is_pose) {
+        double ng[6], out[7];
+        for (int k = 0; k < 6; ++k) ng[k] = -g[k];
+        pose_plus(x, ng, out);
+        for (int k = 0; k < 7; ++k) { const double df = fabs(x[k] - out[k]); gm = (df == df) ? fmax(gm, df) : INFINITY; }
+    } else for (int k = 0; k < 3; ++k) { const double df = fabs(g[k]); gm = (df == df) ? fmax(gm, df) : INFINITY; }
+    return (gm == gm) ? (unsigned long long)__double_as_longlong(fabs(gm)) : 0x7ff0000000000000ull;
+}
+
+// Single-GPU pass: S = lower(Hpp) + damping and rhs = -gc, added over the whole grid into the S / rhs the previous pass (or
+// ba_zero_kernel) cleared.  The adds commute with the Schur warps' `S -= U^T U` and `rhs += sum u g` atomics: no ordering between
+// the two and no grid barrier.  Dense storage (the only one on this path): one warp per row of the strict lower triangle.
+__device__ __forceinline__ void assemble_system(const BaDev& d) {
+    const int gid = blockIdx.x * blockDim.x + threadIdx.x, nthr = gridDim.x * blockDim.x, lane = threadIdx.x & 31;
+    if (gid < 16) d.scal[gid] = 0.0;
+    unsigned long long gbits = 0ull;
+    for (int i = gid; i < d.n_poses + d.n_vec3; i += nthr) gbits = max(gbits, assemble_camera_block(d, i));
+    warp_max_to_state(d.st, gbits);
+    for (int r = gid >> 5; r < d.dimc; r += nthr >> 5) {
+        const double* src = d.Hpp + SIDX(d, r, 0);
+        double* dst = d.S + SIDX(d, r, 0);
+        for (int j0 = lane; j0 < r; j0 += 4 * 32) {
+            double v[4];
+#pragma unroll
+            for (int u = 0; u < 4; ++u) v[u] = (j0 + 32 * u < r) ? __ldg(src + j0 + 32 * u) : 0.0;
+#pragma unroll
+            for (int u = 0; u < 4; ++u) if (v[u] != 0.0) atomicAdd(dst + j0 + 32 * u, v[u]);
+        }
+    }
+}
+
+// assemble (single GPU): S and rhs arrive as zeros; the kernel adds the rest of the system (assemble_system) next to the
+// elimination, and the last CTA to finish -- every gradient contribution and the cost are final then -- runs the LM pre-check
+// (lm_control_pre), so the Cholesky that follows only reads `done`.
+__global__ void __launch_bounds__(TPB) ba_schur_kernel(BaDev d, int cols_max, int assemble) {
+    if (d.st->done) return;                         // uniform: only the last CTA below writes `done`
+    if (assemble) assemble_system(d);
+    const int w = blockIdx.x * (TPB / 32) + (threadIdx.x >> 5);
+    if (w < d.n_schur_warps) schur_warp(d, cols_max, w);
+    if (assemble && arrive_last(d.cta_done)) {
+        __shared__ LmState s;
+        lm_state_load(&s, d.st);
+        if (threadIdx.x == 0) lm_control_pre(s);
+        lm_state_store(d.st, &s);
     }
 }
 
@@ -909,12 +1042,9 @@ __device__ __forceinline__ unsigned long long prepare_camera_block(const BaDev& 
     }
     return 0ull;
 }
-__device__ __forceinline__ void warp_max_to_state(LmState* st, unsigned long long bits) {
-    for (int o = 16; o > 0; o >>= 1) { const unsigned long long v = __shfl_xor_sync(0xffffffffu, bits, o); bits = v > bits ? v : bits; }
-    if ((threadIdx.x & 31) == 0 && bits) atomicMax(&st->grad_max_bits, bits);
-}
 
 // S <- lower(Hpp), rhs <- -gc, gcr <- gc, diagH <- diag(Hpp), scalars <- 0.
+// Not launched for the single-GPU window, whose Schur kernel assembles S itself (assemble_system).
 // FUSE_DAMP (single GPU): the camera blocks' Jacobi scale, LM damping and gradient max-norm (prepare_camera_block) ride along: the
 // bulk copy skips the diagonal and the thread that owns a block fills that block's rows (diagonal of S, rhs, gcr, diagH) and damps
 // them itself, so there is no ordering hazard -- the Schur kernel's `S -= ...` atomics that follow commute with the damping.
@@ -1091,8 +1221,8 @@ __global__ void __launch_bounds__(1024) ba_post_kernel(BaDev d, int decide_only)
     }
 }
 
-// Large problems (banded storage): the same accept + clear spread over the whole grid.  `accept` may be stale when the
-// solve finished in an earlier pass; the copy is idempotent then (the candidate has not been rewritten).
+// Large problems (banded storage) and the single-GPU window pass: the same accept + clear spread over the whole grid.  `accept` may
+// be stale when the solve finished in an earlier pass; the copy is idempotent then (the candidate has not been rewritten).
 __global__ void ba_post_wide_kernel(BaDev d) {
     const LmState* st = d.st;
     const size_t gid = (size_t)blockIdx.x * blockDim.x + threadIdx.x, stride = (size_t)gridDim.x * blockDim.x;
@@ -1162,6 +1292,7 @@ struct lvb_ba {
     DevBuf<double> Hpp, gc, Hll, gl, tf_w, arena, scale_c, scale_l, lam_c, lam_l;
     DevBuf<double> eval_r, eval_J;
     DevBuf<LmState> st;
+    DevBuf<unsigned int> cta_done;
     BaDev dev;
     BlockRanges ranges;
     size_t pose_smem = 0, imu_smem = 0;
@@ -1450,6 +1581,7 @@ int lvb_ba_finalize(lvb_ba* ba) {
     LVB_TRY(ba->scale_c.ensure(P.dimc)); LVB_TRY(ba->lam_c.ensure(P.dimc));
     LVB_TRY(ba->scale_l.ensure(std::max(1, nr))); LVB_TRY(ba->lam_l.ensure(std::max(1, nr)));
     LVB_TRY(ba->st.ensure(1));
+    if (!ba->cta_done.p) { LVB_TRY(ba->cta_done.ensure(2)); LVB_TRY(ba->cta_done.zero(s)); }     // each kernel leaves its counter at zero
 
     PROF("sync + alloc");
     BaDev& d = ba->dev;
@@ -1465,7 +1597,7 @@ int lvb_ba_finalize(lvb_ba* ba) {
     d.Hpp = ba->Hpp.p; d.gc = ba->gc.p; d.Hll = ba->Hll.p; d.gl = ba->gl.p; d.tf_w = ba->tf_w.p;
     d.S = ba->arena.p; d.rhs = d.S + nH; d.gcr = d.rhs + P.dimc; d.diagH = d.gcr + P.dimc; d.scal = d.diagH + P.dimc;
     d.scale_c = ba->scale_c.p; d.scale_l = ba->scale_l.p; d.lam_c = ba->lam_c.p; d.lam_l = ba->lam_l.p;
-    d.st = ba->st.p;
+    d.st = ba->st.p; d.cta_done = ba->cta_done.p;
     d.rank = ctx->rank; d.world = ctx->world; d.rank0 = (ctx->rank == 0) ? 1 : 0;
     d.stage_poses = (np <= MAX_STAGE_POSES) ? (ctx->use_tma ? 2 : 1) : 0;
     d.cams.c0 = make_cam(ba->cam); d.cams.c1 = make_cam(ba->cam + 11);
@@ -1593,6 +1725,17 @@ static bool merged_linearize(lvb_ba* ba) {
     return !off && ba->plan.srow == ba->plan.dimc && ba->plan.soff == 0 && ba->ranges.b[3] > 0 && ba->ranges.b[6] > ba->ranges.b[3];      // dense layout = window-sized
 }
 
+// accept + clear spread over a whole grid (ba_post_wide_kernel): the arrays are too large for one CTA
+static bool wide_post(const lvb_ba* ba) {
+    const BaDev& d = ba->dev;
+    return d.nS > ((size_t)1 << 20) || (size_t)d.n_poses * 7 + (size_t)d.n_vec3 * 3 + d.n_rho > ((size_t)1 << 17);
+}
+
+// The single-GPU window pass (six kernels): S is assembled inside the Schur kernel, whose last CTA runs the LM pre-check, and the
+// step is decided in the last CTA of the cost kernel.  Sharded problems need the all-reduce between those stages, and map-scale
+// ones keep their own kernels (zeroing a banded S each pass would cost more than the copy it replaces).
+static bool fused_pass(lvb_ba* ba) { return ba->ctx->world == 1 && merged_linearize(ba) && !wide_post(ba); }
+
 static bool use_side_branch(lvb_ba* ba) {
     // not inside a captured graph: replaying a graph with parallel branches was measured to be erratic (0.19 - 0.9 ms per
     // pass on the same build), a linear graph is stable
@@ -1610,7 +1753,8 @@ template <int MODE> static int launch_linearize(lvb_ba* ba) {
     lvb_ctx* ctx = ba->ctx;
     const bool one_grid = merged_linearize(ba);
     const bool fork = !one_grid && use_side_branch(ba);
-    if (one_grid) LAUNCH_AS(ba->ctx, kName[MODE][0], ba_linearize_all_kernel<MODE>, ba->ranges.b[6], TPB, std::max(ba->lin_smem, ba->imu_smem), d, ba->ranges);
+    const int decide = (MODE == 1 && fused_pass(ba)) ? 1 : 0;
+    if (one_grid) LAUNCH_AS(ba->ctx, kName[MODE][0], ba_linearize_all_kernel<MODE>, ba->ranges.b[6], TPB, std::max(ba->lin_smem, ba->imu_smem), d, ba->ranges, decide);
     else {
     if (fork) { LVB_CUDA(cudaEventRecord(ctx->ev_fork, ctx->stream)); LVB_CUDA(cudaStreamWaitEvent(ctx->side, ctx->ev_fork, 0)); }
     LAUNCH_AS(ba->ctx, kName[MODE][1], ba_linearize_kernel<MODE>, ba->ranges.b[3], TPB, ba->lin_smem, d, ba->ranges);
@@ -1623,19 +1767,26 @@ template <int MODE> static int launch_linearize(lvb_ba* ba) {
 }
 }  // extern "C++"
 
-// one pass = one LM iteration attempt (all decisions on the device), 10 launches (the two linearise kernels and the two
-// cost kernels run as parallel branches on a second stream):
-//   linearize (visual) | linearize (IMU + priors) | build S | Schur | camera damping | Cholesky (+ LM pre-check)
-//   | back-substitution + candidate | cost (visual) | cost (IMU + priors) | LM decision + accept + clear
+// one pass = one LM iteration attempt (all decisions on the device).  The single-GPU window (fused_pass) is six launches:
+//   linearize (all factor kinds) | Schur (+ S = lower(Hpp) + damping, rhs, LM pre-check in the last CTA) | Cholesky
+//   | back-substitution + candidate | cost (+ clear S / rhs, LM decision in the last CTA) | accept + clear (whole grid)
+// Every other problem keeps up to 10 (the two linearise kernels and the two cost kernels run as parallel branches on a second
+// stream at map scale):
+//   linearize (visual) | linearize (IMU + priors) | build S | Schur | [all-reduce] | camera damping | Cholesky (+ LM pre-check)
+//   | back-substitution + candidate | cost (visual) | cost (IMU + priors) | [all-reduce] | LM decision + accept + clear
 static int launch_linearize_and_reduce(lvb_ba* ba, bool standalone) {
     BaDev& d = ba->dev;
     lvb_ctx* ctx = ba->ctx;
     const size_t nH = d.nS;
+    const bool fused = fused_pass(ba);
     LVB_TRY(launch_linearize<0>(ba));
     const bool fuse_damp = ctx->world == 1;
-    if (fuse_damp) LAUNCH(ba->ctx, ba_build_S_kernel<1>, std::min(1024, nblk(nH, 256)), 256, 0, d);
-    else LAUNCH(ba->ctx, ba_build_S_kernel<0>, std::min(1024, nblk(nH, 256)), 256, 0, d);
-    LAUNCH(ba->ctx, ba_schur_kernel, nblk(d.n_schur_warps, TPB / 32), TPB, ba->schur_smem, d, std::max(1, ba->plan.schur_cols_max));
+    if (!fused) {
+        if (fuse_damp) LAUNCH(ba->ctx, ba_build_S_kernel<1>, std::min(1024, nblk(nH, 256)), 256, 0, d);
+        else LAUNCH(ba->ctx, ba_build_S_kernel<0>, std::min(1024, nblk(nH, 256)), 256, 0, d);
+    }
+    // the fused pass launches the Schur kernel even without landmarks: it assembles S
+    LAUNCH(ba->ctx, ba_schur_kernel, std::max(fused ? 1 : 0, nblk(d.n_schur_warps, TPB / 32)), TPB, ba->schur_smem, d, std::max(1, ba->plan.schur_cols_max), fused ? 1 : 0);
     if (d.tc_mode) LAUNCH(ba->ctx, ba_schur_tc_kernel, ba->n_tc_chunks / TC_CHUNKS, 128, (size_t)TC_CHUNKS * TC_CHUNK_BYTES, d, ba->n_tc_chunks);
     const size_t n_arena = nH + 3 * (size_t)d.dimc + 16;
     P2PArgs pa;
@@ -1649,18 +1800,24 @@ static int launch_linearize_and_reduce(lvb_ba* ba, bool standalone) {
     }
     // (fusing this into the Cholesky prologue was measured: it perturbs that kernel's register allocation and is slower)
     if (!fuse_damp && !fused_comm) LAUNCH(ba->ctx, ba_prepare_camera_kernel, nblk(d.n_poses + d.n_vec3, 128), 128, 0, d);
-    if (standalone) LAUNCH(ba->ctx, lm_control_pre_kernel, 1, 1, 0, d.st);
+    if (standalone && !fused) LAUNCH(ba->ctx, lm_control_pre_kernel, 1, 1, 0, d.st);
     return check_launch("linearize");
 }
 
 static int launch_step(lvb_ba* ba) {
     BaDev& d = ba->dev;
     lvb_ctx* ctx = ba->ctx;
-    LVB_TRY(ba->solver.launch(ctx, d.S, d.rhs, d.dimc, d.srow, d.soff, ba->plan.band, d.st));
+    const bool fused = fused_pass(ba);
+    LVB_TRY(ba->solver.launch(ctx, d.S, d.rhs, d.dimc, d.srow, d.soff, ba->plan.band, d.st, fused));
     LAUNCH(ba->ctx, ba_update_kernel, nblk((size_t)d.n_poses + d.n_vec3 + d.n_rho, TPB), TPB, 0, d);
     LVB_TRY(launch_linearize<1>(ba));
+    if (fused) {      // the decision is taken; accept + clear over a grid sized to the larger of the two jobs
+        const size_t work = std::max(d.nS / 2, (size_t)d.n_poses * 7 + (size_t)d.n_vec3 * 3 + d.n_rho);
+        LAUNCH(ba->ctx, ba_post_wide_kernel, std::min(4 * ba->ctx->sm_count, nblk(work, 256)), 256, 0, d);
+        return check_launch("step");
+    }
     if (ctx->world > 1) LVB_TRY(comm_allreduce_sum_f64(ctx, &d.st->cand_cost_acc, 5));
-    const bool wide = d.nS > ((size_t)1 << 20) || (size_t)d.n_poses * 7 + (size_t)d.n_vec3 * 3 + d.n_rho > ((size_t)1 << 17);
+    const bool wide = wide_post(ba);
     LAUNCH(ba->ctx, ba_post_kernel, 1, wide ? 32 : 1024, 0, d, wide ? 1 : 0);
     if (wide) LAUNCH(ba->ctx, ba_post_wide_kernel, 4 * ba->ctx->sm_count, 256, 0, d);
     return check_launch("step");
@@ -1668,8 +1825,9 @@ static int launch_step(lvb_ba* ba) {
 
 static int launch_clear(lvb_ba* ba) {
     BaDev& d = ba->dev;
-    const size_t nH = d.nS;
-    LAUNCH(ba->ctx, ba_zero_kernel, std::min(1024, nblk(nH + d.dimc + 2 * (size_t)d.n_rho, 256)), 256, 0, d);
+    const bool zero_S = fused_pass(ba);
+    const size_t n = d.nS + d.dimc + 2 * (size_t)d.n_rho + (zero_S ? d.nS + d.dimc : 0);
+    LAUNCH(ba->ctx, ba_zero_kernel, std::min(1024, nblk(n, 256)), 256, 0, d, zero_S ? 1 : 0);
     return check_launch("clear");
 }
 

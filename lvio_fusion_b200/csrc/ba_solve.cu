@@ -41,12 +41,16 @@ __device__ long long g_chol_dbg[8];
 // envelope into shared memory once (chol_resident_columns, ba_plan.h) while warp 0 factors diagonal block 0 from global memory;
 // the panel of step k is then block column k itself, the rhs a shared vector, and only x goes back to global memory.  Nothing reads
 // the factor after the solve (S is rebuilt from Hpp on every pass), so the two storages compute the same x with the same arithmetic.
+//
+// run_pre: thread 0 runs the LM pre-check first.  The single-GPU window pass runs it in the last CTA of its Schur kernel instead;
+// then nothing precedes warp 0's loads of diagonal block 0, and every warp only checks `done` (issued next to those loads).
 template <bool kResident>
 __global__ void __launch_bounds__(CHOL_T) ba_cholesky_kernel(double* __restrict__ S, double* __restrict__ rhs, int n, long long srow, long long soff,
-                                                                  LmState* st, const int* __restrict__ env_rmax) {
-    if (threadIdx.x == 0) lm_control_pre(*st);
-    __syncthreads();
-    if (st->done) return;
+                                                                  LmState* st, const int* __restrict__ env_rmax, int run_pre) {
+    if (run_pre) {
+        if (threadIdx.x == 0) lm_control_pre(*st);
+        __syncthreads();
+    }
     extern __shared__ __align__(16) double sm[];
     __shared__ int fail;
     __shared__ int boff[CHOL_RES_STEPS];
@@ -68,8 +72,11 @@ __global__ void __launch_bounds__(CHOL_T) ba_cholesky_kernel(double* __restrict_
         double a[32];
 #pragma unroll
         for (int j = 0; j < 32; ++j) a[j] = (lane < b0 && j <= lane) ? *G.at(lane, j) : ((j == lane) ? 1.0 : 0.0);
+        if (st->done) return;                       // uniform over the CTA, like the check of the other warps
         const int bad = chol_diag32_pair(a, lane, sm, sm + 32 * 34);
         if (bad && lane == 0) fail = 1;
+    } else if (st->done) {
+        return;
     } else if constexpr (kResident) {
         // ---- load: the rhs and the envelope, all of S the solve touches (upper triangles of the diagonal blocks and columns past n
         // as zeros); batches of 8 independent loads per thread
@@ -292,11 +299,12 @@ int ReducedSolver::upload(lvb_ctx* ctx, const SolverPlan& sp, const std::vector<
     return LVB_OK;
 }
 
-int ReducedSolver::launch(lvb_ctx* ctx, double* S, double* rhs, int n, long long srow, long long soff, int band, LmState* st) const {
+int ReducedSolver::launch(lvb_ctx* ctx, double* S, double* rhs, int n, long long srow, long long soff, int band, LmState* st, bool pre_done) const {
     const SolverPlan& sp = plan;
+    const int run_pre = pre_done ? 0 : 1;
     if (sp.tree_levels > 0) {
         // multifrontal tree: leaves (all SMs) -> ... -> root, then the back-substitution root -> leaves; 2 (levels + 1) launches
-        LAUNCH(ctx, lm_control_pre_kernel, 1, 1, 0, st);
+        if (run_pre) LAUNCH(ctx, lm_control_pre_kernel, 1, 1, 0, st);
         const int n_fronts = sp.level_first[sp.tree_levels - 1] + sp.level_count[sp.tree_levels - 1];
         ba_front_init_kernel<<<dim3(16, n_fronts), 256, 0, ctx->stream>>>(fronts.p, n_fronts, S, rhs, pool.p, srow, soff, band, st);
         ctx->launches++; timing_mark(ctx->stream, "ba_front_init_kernel");
@@ -310,16 +318,16 @@ int ReducedSolver::launch(lvb_ctx* ctx, double* S, double* rhs, int n, long long
             const int bs = std::min(32, n - kb);
             const int m = rmax[kb >> 5] - (kb + bs) + 2;
             const int ntile = (m + 31) / 32, total = m > 1 ? ntile * (ntile + 1) / 2 : 0;
-            LAUNCH(ctx, ba_wide_diag_kernel, 1, 32, 0, S, n, srow, soff, kb, invd.p, st, kb == 0 ? 1 : 0);
+            LAUNCH(ctx, ba_wide_diag_kernel, 1, 32, 0, S, n, srow, soff, kb, invd.p, st, kb == 0 ? run_pre : 0);
             LAUNCH(ctx, ba_wide_panel_kernel, (m + 127) / 128, 128, 0, S, rhs, n, srow, soff, kb, invd.p, st, rmax_d.p);
             LAUNCH(ctx, ba_wide_update_kernel, (total + WIDE_WARPS - 1) / WIDE_WARPS, WIDE_WARPS * 32, (size_t)WIDE_WARPS * 2 * 32 * 34 * 8, S, rhs, n, srow, soff, kb, st, rmax_d.p);
         }
         for (int kb = ((n - 1) / 32) * 32; kb >= 0; kb -= 32)
             LAUNCH(ctx, ba_wide_backward_kernel, 1, 256, 0, S, rhs, n, srow, soff, kb, invd.p, st, rmax_d.p);
     } else if (sp.resident) {
-        LAUNCH_AS(ctx, "ba_cholesky_kernel", ba_cholesky_kernel<true>, 1, CHOL_T, sp.resident_smem, S, rhs, n, srow, soff, st, rmax_d.p);
+        LAUNCH_AS(ctx, "ba_cholesky_kernel", ba_cholesky_kernel<true>, 1, CHOL_T, sp.resident_smem, S, rhs, n, srow, soff, st, rmax_d.p, run_pre);
     } else {
-        LAUNCH_AS(ctx, "ba_cholesky_kernel", ba_cholesky_kernel<false>, 1, CHOL_T, sp.chol_smem, S, rhs, n, srow, soff, st, rmax_d.p);
+        LAUNCH_AS(ctx, "ba_cholesky_kernel", ba_cholesky_kernel<false>, 1, CHOL_T, sp.chol_smem, S, rhs, n, srow, soff, st, rmax_d.p, run_pre);
     }
     return LVB_OK;
 }

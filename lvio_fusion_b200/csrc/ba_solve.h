@@ -16,9 +16,10 @@ struct ReducedSolver {
     DevBuf<Front> fronts; DevBuf<double> pool;      // separator tree: the fronts and their border arrays
     // n unknowns; allocates on the context's stream and sets the solver kernels' shared-memory limits on first use
     int upload(lvb_ctx* ctx, const SolverPlan& sp, const std::vector<int>& env_rmax, int n);
-    // rhs <- S^-1 rhs for S (n x n, element (i, j) at i * srow + j + soff, half bandwidth `band` for the tree), after lm_control_pre;
+    // rhs <- S^-1 rhs for S (n x n, element (i, j) at i * srow + j + soff, half bandwidth `band` for the tree), after lm_control_pre
+    // (run by the solver's first kernel unless pre_done: an earlier kernel of the pass ran it);
     // a non-positive pivot sets st->solve_fail, a finished solve (st->done) makes every kernel return at once
-    int launch(lvb_ctx* ctx, double* S, double* rhs, int n, long long srow, long long soff, int band, LmState* st) const;
+    int launch(lvb_ctx* ctx, double* S, double* rhs, int n, long long srow, long long soff, int band, LmState* st, bool pre_done = false) const;
 };
 
 // The plan-shaping A/B switches LVB_NO_TREE and LVB_TREE_SEP_BAND, read once per process.
