@@ -51,7 +51,7 @@ struct BaDev {
     const int *lm_start, *lm_fac;
     const int *tf_slot;                 // 2 planes: slot of pose_1 / pose_2 inside the landmark's Schur group (-1: constant pose)
     const int *sw_group, *sw_lm, *grp_ns, *grp_off;   // Schur warps: group id, 32 landmark ids (-1 pad); per group: #slots, offsets
-    int n_schur_warps, warp_syrk;
+    int n_schur_warps;
     int tc_mode;                        // 1: Schur contraction on the tensor cores (wgmma, split bf16), FP64 rhs only here
     unsigned short* tc_u;               // packed U^T: [chunk of 16 landmarks][3 splits][128 x 16 bf16 K-major core-matrix tile]
     const int* tc_cdim;                 // camera offset -> compact pose dimension (0..127) or -1
@@ -277,6 +277,65 @@ __global__ void __launch_bounds__(TPB) ba_eval_two_camera_kernel(BaDev d, double
     if (J_out) { J_out[2 * f] = o.Jrho[0]; J_out[2 * f + 1] = o.Jrho[1]; }
 }
 
+// An IMU factor is worked on by a thread group of NT threads: one warp (NT = 32) or one 128-thread CTA (window-sized problems).
+template <int NT> __device__ __forceinline__ void group_sync() { if (NT == 32) __syncwarp(); else __syncthreads(); }
+
+// Whitening by the square-root information U (upper triangular): s_r[16..30] = U r, s_Jw = U J (ambient, 15 x 32).
+template <int NT>
+__device__ __forceinline__ void imu_whiten(const double* U, const double* s_raw, double* s_Jw, double* s_r, bool with_jac) {
+    const int t = NT == 32 ? threadIdx.x & 31 : threadIdx.x;
+    if (t < 15) { double s = 0; for (int k = 0; k < 15; ++k) s += U[15 * t + k] * s_r[k]; s_r[16 + t] = s; }
+    if (with_jac) for (int e = t; e < 480; e += NT) {
+        const int i = e >> 5, j = e & 31;
+        double s = 0; for (int k = i; k < 15; ++k) s += U[15 * i + k] * s_raw[32 * k + j];
+        s_Jw[e] = s;
+    }
+    group_sync<NT>();
+}
+
+// The linearised IMU factor into the system, once the whitened residual and Jacobian are in s_r / s_Jw and every thread of the
+// group has read the whitened residual: the tangent Jacobian Jt[15][30] scaled by the robust weight sr goes into s_raw (cols:
+// pose_i 6 | v ba bg 9 | pose_j 6 | v ba bg 9), the residual is scaled likewise, s_gidx gets the 30 global camera-system indices
+// (-1: constant block), then gc += Jt^T r and lower(Hpp) += Jt^T Jt.  In a CTA, warp 0 forms the tangent rows while warp 1
+// builds the index table.
+template <int NT>
+__device__ __forceinline__ void imu_accumulate(const BaDev& d, const int* ix, int n, int f, const double* P, double sr, const double* s_Jw, double* s_raw, double* s_r, int* s_gidx) {
+    const int t = NT == 32 ? threadIdx.x & 31 : threadIdx.x;
+    if (t < 15) {
+        const double* a = s_Jw + 32 * t;
+        double* row = s_raw + 30 * t;
+        double t6[6];
+        ambient_row_to_tangent(P + 7 * ix[f], a, t6);
+        for (int k = 0; k < 6; ++k) row[k] = t6[k] * sr;
+        for (int k = 0; k < 9; ++k) row[6 + k] = a[7 + k] * sr;
+        ambient_row_to_tangent(P + 7 * ix[4 * n + f], a + 16, t6);
+        for (int k = 0; k < 6; ++k) row[15 + k] = t6[k] * sr;
+        for (int k = 0; k < 9; ++k) row[21 + k] = a[23 + k] * sr;
+        s_r[16 + t] *= sr;
+    }
+    const int l = NT == 32 ? t : t - 32;
+    if (l >= 0 && l < 30) {
+        int blk, loc;
+        if (l < 6) { blk = 0; loc = l; } else if (l < 15) { blk = 1 + (l - 6) / 3; loc = (l - 6) % 3; }
+        else if (l < 21) { blk = 4; loc = l - 15; } else { blk = 5 + (l - 21) / 3; loc = (l - 21) % 3; }
+        const int id = ix[(size_t)blk * n + f];
+        const int off = id < 0 ? -1 : ((blk == 0 || blk == 4) ? d.pose_off[id] : d.vec3_off[id]);
+        s_gidx[l] = off < 0 ? -1 : off + loc;
+    }
+    group_sync<NT>();
+    if (t < 30 && s_gidx[t] >= 0) {
+        double g = 0; for (int i = 0; i < 15; ++i) g += s_raw[30 * i + t] * s_r[16 + i];
+        atomicAdd(&d.gc[s_gidx[t]], g);
+    }
+    for (int e = t; e < 465; e += NT) {
+        const int a = c_tri_a[e], b = c_tri_b[e];
+        const int ga = s_gidx[a], gb = s_gidx[b];
+        if (ga < 0 || gb < 0) continue;
+        double h = 0; for (int i = 0; i < 15; ++i) h += s_raw[30 * i + a] * s_raw[30 * i + b];
+        if (ga >= gb) atomicAdd(&d.Hpp[SIDX(d, ga, gb)], h); else atomicAdd(&d.Hpp[SIDX(d, gb, ga)], h);
+    }
+}
+
 // IMU: one warp per factor.  Fills s_r (whitened residual, 15) and s_Jw (whitened ambient Jacobian 15x32).
 __device__ void imu_warp_eval(const BaDev& d, int f, const double* P, const double* V, double* s_raw /*480*/, double* s_Jw /*480*/, double* s_r /*32: raw 0..14, whitened 16..30*/, bool with_jac = true) {
     const int lane = threadIdx.x & 31;
@@ -295,14 +354,7 @@ __device__ void imu_warp_eval(const BaDev& d, int f, const double* P, const doub
         else if (with_jac && !(lane >= 6 && c[287] != 0.0)) imu_raw_jacobian_block(k, lane, Ti, Vi, Bgi, Tj, Vj, s_raw);
     }
     __syncwarp();
-    const double* U = c + 62;
-    if (lane < 15) { double s = 0; for (int k = 0; k < 15; ++k) s += U[15 * lane + k] * s_r[k]; s_r[16 + lane] = s; }
-    if (with_jac) for (int e = lane; e < 480; e += 32) {
-        const int i = e >> 5, j = e & 31;
-        double s = 0; for (int k = i; k < 15; ++k) s += U[15 * i + k] * s_raw[32 * k + j];     // U is upper triangular
-        s_Jw[e] = s;
-    }
-    __syncwarp();
+    imu_whiten<32>(c + 62, s_raw, s_Jw, s_r, with_jac);
 }
 
 __global__ void __launch_bounds__(TPB) ba_eval_imu_kernel(BaDev d, double* __restrict__ r_out, double* __restrict__ J_out) {
@@ -336,7 +388,7 @@ __global__ void ba_eval_prior_kernel(BaDev d, int kind, double* __restrict__ r_o
 // Warp-level SYRK: the 32 blocks of a warp share their pose key (finalize() sorts and pads), so the warp
 // writes its Jacobian rows [2 x ncol per lane] to shared memory, each lane then owns a few entries of the
 // lower triangle of A^T A (A = [J_1 | J_2 | r] or [J | r]) and issues ONE red.global per entry instead of 32.
-__device__ __forceinline__ void warp_syrk_flush(const BaDev& d, const double* A /*64 x SYRK_LD*/, int ncol, int off1, int off2) {
+__device__ __forceinline__ void syrk_flush(const BaDev& d, const double* A /*64 x SYRK_LD*/, int ncol, int off1, int off2) {
     const int lane = threadIdx.x & 31;
     const int nent = ncol * (ncol + 1) / 2;
     for (int e = lane; e < nent; e += 32) {
@@ -354,6 +406,29 @@ __device__ __forceinline__ void warp_syrk_flush(const BaDev& d, const double* A 
         if (ga >= gb) atomicAdd(&d.Hpp[SIDX(d, ga, gb)], v); else atomicAdd(&d.Hpp[SIDX(d, gb, ga)], v);
     }
 }
+// The SYRK loop of one warp: while lanes with `take` remain, the first one's key (key1, key2) and camera offsets lead, the lanes
+// holding that key write their two rows (rows(row0, row1), NCOL entries each), the others zeros, and the warp flushes A^T A.
+// TWO_POSES: 13 columns [J_1 | J_2 | r], and key2 / off2 are exchanged too; one pose: 7 columns [J | r], key2 / off2 constants.
+template <bool TWO_POSES, class Rows>
+__device__ __forceinline__ void syrk_loop(const BaDev& d, double* A, bool take, int key1, int key2, int off1, int off2, Rows rows) {
+    constexpr int NCOL = TWO_POSES ? 13 : 7;
+    const int lane = threadIdx.x & 31;
+    unsigned todo = __ballot_sync(0xffffffffu, take);
+    while (todo) {
+        const int leader = __ffs(todo) - 1;
+        const int k1 = __shfl_sync(0xffffffffu, key1, leader), o1 = __shfl_sync(0xffffffffu, off1, leader);
+        const int k2 = TWO_POSES ? __shfl_sync(0xffffffffu, key2, leader) : key2;
+        const int o2 = TWO_POSES ? __shfl_sync(0xffffffffu, off2, leader) : off2;
+        const bool mine = take && key1 == k1 && key2 == k2;
+        double* row0 = A + (2 * lane) * SYRK_LD; double* row1 = row0 + SYRK_LD;
+        if (mine) rows(row0, row1);
+        else for (int k = 0; k < NCOL; ++k) { row0[k] = 0.0; row1[k] = 0.0; }
+        __syncwarp();
+        syrk_flush(d, A, NCOL, o1, o2);
+        __syncwarp();
+        todo &= ~__ballot_sync(0xffffffffu, mine);
+    }
+}
 
 template <int MODE>
 __device__ __forceinline__ void linearize_visual_body(const BaDev& d, const BlockRanges& R, const int b) {
@@ -366,7 +441,7 @@ __device__ __forceinline__ void linearize_visual_body(const BaDev& d, const Bloc
     const double* Psrc = MODE == 0 ? d.poses : d.c_poses;
     const double* Rho = MODE == 0 ? d.rho : d.c_rho;
     double* cost_target = MODE == 0 ? &d.st->cost_acc : &d.st->cand_cost_acc;
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int warp = threadIdx.x >> 5;
     double cost = 0.0;
     const size_t pose_bytes = d.stage_poses ? (((size_t)d.n_poses * 56 + 16 + 15) & ~(size_t)15) : 0;
     double* A = reinterpret_cast<double*>(smem_raw + pose_bytes) + (size_t)warp * SYRK_ROWS * SYRK_LD;
@@ -411,24 +486,11 @@ __device__ __forceinline__ void linearize_visual_body(const BaDev& d, const Bloc
         }
         if (MODE == 0) {
             // blocks are sorted by (pose_1, pose_2): a warp holds one key (padded layout) or a few key segments
-            unsigned todo = d.warp_syrk ? __ballot_sync(0xffffffffu, valid && i1 != i2) : 0u;
-            const bool direct = valid && (!d.warp_syrk || i1 == i2);
-            while (todo) {
-                const int leader = __ffs(todo) - 1;
-                const int k1 = __shfl_sync(0xffffffffu, i1, leader), k2 = __shfl_sync(0xffffffffu, i2, leader);
-                const int o1 = __shfl_sync(0xffffffffu, off1, leader), o2 = __shfl_sync(0xffffffffu, off2, leader);
-                const bool mine = valid && i1 == k1 && i2 == k2;
-                double* row0 = A + (2 * lane) * SYRK_LD; double* row1 = row0 + SYRK_LD;
-                if (mine) {
-                    for (int k = 0; k < 6; ++k) { row0[k] = o.J1[k]; row1[k] = o.J1[6 + k]; row0[6 + k] = o.J2[k]; row1[6 + k] = o.J2[6 + k]; }
-                    row0[12] = o.r[0]; row1[12] = o.r[1];
-                } else for (int k = 0; k < 13; ++k) { row0[k] = 0.0; row1[k] = 0.0; }
-                __syncwarp();
-                warp_syrk_flush(d, A, 13, o1, o2);
-                __syncwarp();
-                todo &= ~__ballot_sync(0xffffffffu, mine);
-            }
-            if (direct) {
+            syrk_loop<true>(d, A, valid && i1 != i2, i1, i2, off1, off2, [&](double* row0, double* row1) {
+                for (int k = 0; k < 6; ++k) { row0[k] = o.J1[k]; row1[k] = o.J1[6 + k]; row0[6 + k] = o.J2[k]; row1[6 + k] = o.J2[6 + k]; }
+                row0[12] = o.r[0]; row1[12] = o.r[1];
+            });
+            if (valid && i1 == i2) {
                 if (off1 >= 0) add_diag(d.Hpp, d.gc, d, off1, o.J1, 6, 2, o.r);
                 if (off2 >= 0) add_diag(d.Hpp, d.gc, d, off2, o.J2, 6, 2, o.r);
                 if (off1 >= 0 && off2 >= 0) add_cross(d.Hpp, d, off1, o.J1, 6, off2, o.J2, 6, 2);
@@ -450,22 +512,10 @@ __device__ __forceinline__ void linearize_visual_body(const BaDev& d, const Bloc
             if (MODE == 0) { off = d.pose_off[ip]; o.r[0] *= sr; o.r[1] *= sr; for (int k = 0; k < 12; ++k) o.J[k] *= sr; }
         }
         if (MODE == 0) {
-            unsigned todo = d.warp_syrk ? __ballot_sync(0xffffffffu, valid) : 0u;
-            while (todo) {
-                const int leader = __ffs(todo) - 1;
-                const int k1 = __shfl_sync(0xffffffffu, ip, leader), o1 = __shfl_sync(0xffffffffu, off, leader);
-                const bool mine = valid && ip == k1;
-                double* row0 = A + (2 * lane) * SYRK_LD; double* row1 = row0 + SYRK_LD;
-                if (mine) {
-                    for (int k = 0; k < 6; ++k) { row0[k] = o.J[k]; row1[k] = o.J[6 + k]; }
-                    row0[6] = o.r[0]; row1[6] = o.r[1];
-                } else for (int k = 0; k < 7; ++k) { row0[k] = 0.0; row1[k] = 0.0; }
-                __syncwarp();
-                warp_syrk_flush(d, A, 7, o1, -1);
-                __syncwarp();
-                todo &= ~__ballot_sync(0xffffffffu, mine);
-            }
-            if (!d.warp_syrk && valid && off >= 0) add_diag(d.Hpp, d.gc, d, off, o.J, 6, 2, o.r);
+            syrk_loop<false>(d, A, valid, ip, 0, off, -1, [&](double* row0, double* row1) {
+                for (int k = 0; k < 6; ++k) { row0[k] = o.J[k]; row1[k] = o.J[6 + k]; }
+                row0[6] = o.r[0]; row1[6] = o.r[1];
+            });
         }
     } else {                     // ---- a3 TwoCameraReprojectionError
         const int n = d.n[2];
@@ -539,54 +589,15 @@ __device__ __forceinline__ void linearize_other_body(const BaDev& d, const Block
             }
         }
         __syncthreads();
-        const double* U = s_c + 62;
-        if (tid < 15) { double sacc = 0; for (int k = 0; k < 15; ++k) sacc += U[15 * tid + k] * s_r[k]; s_r[16 + tid] = sacc; }
-        if (MODE == 0) for (int e = tid; e < 480; e += TPB) {
-            const int i = e >> 5, j = e & 31;
-            double sacc = 0; for (int k = i; k < 15; ++k) sacc += U[15 * i + k] * s_raw[32 * k + j];     // U is upper triangular
-            s_Jw[e] = sacc;
-        }
-        __syncthreads();
+        imu_whiten<TPB>(s_c + 62, s_raw, s_Jw, s_r, MODE == 0);
         double s = 0.0;
         for (int i = 0; i < 15; ++i) s += s_r[16 + i] * s_r[16 + i];
         double rho_v, sr;
         huber(d.huber[3], s, &rho_v, &sr);
         if (tid == 0) cost = 0.5 * rho_v;
         if (MODE == 0) {
-            // tangent Jacobian Jt[15][30] into s_raw (cols: pose_i 6 | v ba bg 9 | pose_j 6 | v ba bg 9)
             __syncthreads();                                      // every thread has read the whitened residual
-            if (tid < 15) {
-                const double* a = s_Jw + 32 * tid;
-                double* t = s_raw + 30 * tid;
-                double t6[6];
-                ambient_row_to_tangent(Psrc + 7 * ix[f], a, t6);
-                for (int k = 0; k < 6; ++k) t[k] = t6[k] * sr;
-                for (int k = 0; k < 9; ++k) t[6 + k] = a[7 + k] * sr;
-                ambient_row_to_tangent(Psrc + 7 * ix[4 * n + f], a + 16, t6);
-                for (int k = 0; k < 6; ++k) t[15 + k] = t6[k] * sr;
-                for (int k = 0; k < 9; ++k) t[21 + k] = a[23 + k] * sr;
-                s_r[16 + tid] *= sr;
-            } else if (tid >= 32 && tid < 62) {
-                const int l = tid - 32;
-                int blk, loc;
-                if (l < 6) { blk = 0; loc = l; } else if (l < 15) { blk = 1 + (l - 6) / 3; loc = (l - 6) % 3; }
-                else if (l < 21) { blk = 4; loc = l - 15; } else { blk = 5 + (l - 21) / 3; loc = (l - 21) % 3; }
-                const int id = ix[(size_t)blk * n + f];
-                const int off = id < 0 ? -1 : ((blk == 0 || blk == 4) ? d.pose_off[id] : d.vec3_off[id]);
-                s_gidx[l] = off < 0 ? -1 : off + loc;
-            }
-            __syncthreads();
-            if (tid < 30 && s_gidx[tid] >= 0) {
-                double g = 0; for (int i = 0; i < 15; ++i) g += s_raw[30 * i + tid] * s_r[16 + i];
-                atomicAdd(&d.gc[s_gidx[tid]], g);
-            }
-            for (int e = tid; e < 465; e += TPB) {
-                const int a = c_tri_a[e], bb = c_tri_b[e];
-                const int ga = s_gidx[a], gb = s_gidx[bb];
-                if (ga < 0 || gb < 0) continue;
-                double h = 0; for (int i = 0; i < 15; ++i) h += s_raw[30 * i + a] * s_raw[30 * i + bb];
-                if (ga >= gb) atomicAdd(&d.Hpp[SIDX(d, ga, gb)], h); else atomicAdd(&d.Hpp[SIDX(d, gb, ga)], h);
-            }
+            imu_accumulate<TPB>(d, ix, n, f, Psrc, sr, s_Jw, s_raw, s_r, s_gidx);
         }
     } else if (b < R.b[4]) {   // ---- IMU, map scale: one warp per factor, four factors per CTA (throughput: thousands of factors)
         double* s_raw = reinterpret_cast<double*>(smem_raw);     // 4 x 480
@@ -604,42 +615,7 @@ __device__ __forceinline__ void linearize_other_body(const BaDev& d, const Block
             double rho_v, sr;
             huber(d.huber[3], s, &rho_v, &sr);
             if (lane == 0) cost = 0.5 * rho_v;
-            if (MODE == 0) {
-                const int* ix = d.fi[3];
-                // tangent Jacobian Jt[15][30] into `raw` (cols: pose_i 6 | v ba bg 9 | pose_j 6 | v ba bg 9)
-                if (lane < 15) {
-                    const double* a = Jw + 32 * lane;
-                    double* t = raw + 30 * lane;
-                    double t6[6];
-                    ambient_row_to_tangent(Psrc + 7 * ix[f], a, t6);
-                    for (int k = 0; k < 6; ++k) t[k] = t6[k] * sr;
-                    for (int k = 0; k < 9; ++k) t[6 + k] = a[7 + k] * sr;
-                    ambient_row_to_tangent(Psrc + 7 * ix[4 * n + f], a + 16, t6);
-                    for (int k = 0; k < 6; ++k) t[15 + k] = t6[k] * sr;
-                    for (int k = 0; k < 9; ++k) t[21 + k] = a[23 + k] * sr;
-                    rr[16 + lane] *= sr;
-                }
-                if (lane < 30) {
-                    int blk, loc;
-                    if (lane < 6) { blk = 0; loc = lane; } else if (lane < 15) { blk = 1 + (lane - 6) / 3; loc = (lane - 6) % 3; }
-                    else if (lane < 21) { blk = 4; loc = lane - 15; } else { blk = 5 + (lane - 21) / 3; loc = (lane - 21) % 3; }
-                    const int id = ix[(size_t)blk * n + f];
-                    const int off = id < 0 ? -1 : ((blk == 0 || blk == 4) ? d.pose_off[id] : d.vec3_off[id]);
-                    gidx[lane] = off < 0 ? -1 : off + loc;
-                }
-                __syncwarp();
-                if (lane < 30 && gidx[lane] >= 0) {
-                    double g = 0; for (int i = 0; i < 15; ++i) g += raw[30 * i + lane] * rr[16 + i];
-                    atomicAdd(&d.gc[gidx[lane]], g);
-                }
-                for (int e = lane; e < 465; e += 32) {
-                    const int a = c_tri_a[e], bb = c_tri_b[e];
-                    const int ga = gidx[a], gb = gidx[bb];
-                    if (ga < 0 || gb < 0) continue;
-                    double h = 0; for (int i = 0; i < 15; ++i) h += raw[30 * i + a] * raw[30 * i + bb];
-                    if (ga >= gb) atomicAdd(&d.Hpp[SIDX(d, ga, gb)], h); else atomicAdd(&d.Hpp[SIDX(d, gb, ga)], h);
-                }
-            }
+            if (MODE == 0) imu_accumulate<32>(d, d.fi[3], n, f, Psrc, sr, Jw, raw, rr, gidx);     // each lane has read only its own residual entry
         }
     } else {   // ---- PoseGraphError / PoseError priors: one thread per block
         const int kind = b < R.b[5] ? 4 : 5;
@@ -731,6 +707,23 @@ __device__ __forceinline__ void atomic_max_nonneg(unsigned long long* p, double 
 }
 
 
+// Four factors of a landmark's track at once, every load issued before the first use: factor id -> pose slots -> 96-byte coupling
+// record is a chain of dependent round trips, and one factor at a time made the Schur kernel L2-latency bound (35 long-scoreboard
+// stall cycles per issue at map scale).  f[u] = lm_fac[eb + u], -1 past e1; slots() issues the caller's index loads (unconditional,
+// at max(f, 0): no branches between them); w[u] is factor f[u]'s record (factor 0's when f[u] < 0).
+template <class Slots>
+__device__ __forceinline__ void gather_couplings(const BaDev& d, int eb, int e1, int (&f)[4], double2 (&w)[4][6], Slots slots) {
+#pragma unroll
+    for (int u = 0; u < 4; ++u) f[u] = (eb + u < e1) ? d.lm_fac[eb + u] : -1;
+    slots();
+#pragma unroll
+    for (int u = 0; u < 4; ++u) {
+        const double2* src = reinterpret_cast<const double2*>(d.tf_w + (size_t)max(f[u], 0) * 12);
+#pragma unroll
+        for (int k = 0; k < 6; ++k) w[u][k] = src[k];
+    }
+}
+
 // K5: eliminate the inverse depths.  One warp per 32 landmarks that share their set of pose offsets
 // (finalize() groups and pads them).  Lane l writes u_l = sqrt(1/h_l) [w_l | g_l] (its couplings merged by
 // pose slot) as a row of a shared-memory tile; the warp then forms the lower triangle of U^T U and subtracts
@@ -758,23 +751,14 @@ __device__ __forceinline__ void schur_warp(const BaDev& d, int cols_max, int w) 
         const double hl = h + lam;
         if (hl > 0.0 && ns > 0) {
             const int n = d.n[0];
-            // gather the landmark's coupling records four factors at a time: all index loads of a batch are issued before the first
-            // use (factor id -> slots -> 96-byte record is a chain of three dependent round trips; one factor at a time made this
-            // kernel L2-latency bound, 35 long-scoreboard stall cycles per issue at map scale)
             const int e1 = d.lm_start[l + 1];
-            for (int eb = d.lm_start[l]; eb < e1; eb += 4) {
+            for (int eb = d.lm_start[l]; eb < e1; eb += 4) {      // the landmark's coupling records, merged by pose slot
                 int f[4], s0[4], s1[4];
-#pragma unroll
-                for (int u = 0; u < 4; ++u) f[u] = (eb + u < e1) ? d.lm_fac[eb + u] : -1;
-#pragma unroll
-                for (int u = 0; u < 4; ++u) { const int fc = max(f[u], 0); s0[u] = d.tf_slot[fc]; s1[u] = d.tf_slot[(size_t)n + fc]; }      // unconditional (clamped) loads: no branches between them
                 double2 w[4][6];
+                gather_couplings(d, eb, e1, f, w, [&] {
 #pragma unroll
-                for (int u = 0; u < 4; ++u) {
-                    const double2* src = reinterpret_cast<const double2*>(d.tf_w + (size_t)max(f[u], 0) * 12);
-#pragma unroll
-                    for (int k = 0; k < 6; ++k) w[u][k] = src[k];
-                }
+                    for (int u = 0; u < 4; ++u) { const int fc = max(f[u], 0); s0[u] = d.tf_slot[fc]; s1[u] = d.tf_slot[(size_t)n + fc]; }
+                });
 #pragma unroll
                 for (int u = 0; u < 4; ++u) {
                     if (f[u] < 0) continue;
@@ -841,47 +825,63 @@ __device__ __forceinline__ void warp_max_to_state(LmState* st, unsigned long lon
     if ((threadIdx.x & 31) == 0 && bits) atomicMax(&st->grad_max_bits, bits);
 }
 
-// One camera block of the single-GPU pass, read from Hpp and gc directly, every load issued before the first use: Jacobi scale
-// (first pass), damping, gcr, diagH, and the block's rows of the system -- S[diag] += H_kk + lambda_k and rhs += -g_k by red.add --
-// then the gradient max-norm ||x - Plus(x, -g)||_inf as ordered bits (0: nothing to report).  Same arithmetic as
-// ba_build_S_kernel<1> + prepare_camera_block, which the other passes use.
-__device__ __forceinline__ unsigned long long assemble_camera_block(const BaDev& d, int i) {
-    const LmState* st = d.st;
+// Row r of a camera block: its Hessian diagonal, gradient and (once valid) Jacobi scale; zeros and a scale of one when !in
+__device__ __forceinline__ void camera_row_load(const BaDev& d, bool reduced, int r, bool in, int scale_valid, double& h, double& g, double& sc) {
+    h = in ? (reduced ? d.diagH[r] : d.Hpp[SIDX(d, r, r)]) : 0.0;
+    g = in ? (reduced ? d.gcr : d.gc)[r] : 0.0;
+    sc = (in && scale_valid) ? d.scale_c[r] : 1.0;
+}
+
+// The LM step of camera block i (a pose, or a vec3 at i - n_poses), from the Hessian diagonal h_k and the gradient g_k of its rows r
+// (Hpp's diagonal and gc, or with `reduced` the all-reduced diagH and gcr): the Jacobi scale (written on the first pass), the
+// damping lambda_k = clamp(s^2 h_k, min_diag, max_diag) / (radius s^2), then damp(r, h_k, g_k, lambda_k) -- the caller's rows of
+// the system.  Returns the gradient max-norm ||x - Plus(x, -g)||_inf as ordered bits (0: nothing to report); the caller reduces it
+// over the warp and issues ONE atomicMax.
+// LOAD_FIRST (the window pass, where this is on the critical path) issues every load -- the LM state's fields, the block's h, g,
+// scale and x -- before the first use.  Otherwise each row is loaded as it is used, and the state's fields, x and g are read again
+// where needed (the stores to scale_c / lam_c may alias the state): holding them would raise the wider kernels' register counts.
+template <bool LOAD_FIRST, class Damp>
+__device__ __forceinline__ unsigned long long camera_block_step(const BaDev& d, int i, bool reduced, Damp damp) {
+    LmState held;
+    if (LOAD_FIRST) {
+        const LmState* src = d.st;
+        held.scale_valid = src->scale_valid; held.jacobi = src->jacobi; held.need_linearize = src->need_linearize;
+        held.min_diag = src->min_diag; held.max_diag = src->max_diag; held.radius = src->radius;
+    }
+    const LmState* st = LOAD_FIRST ? &held : d.st;
     const bool is_pose = i < d.n_poses;
     const int off = is_pose ? d.pose_off[i] : d.vec3_off[i - d.n_poses];
     if (off < 0) return 0ull;
     const int w = is_pose ? 6 : 3;
-    const int scale_valid = st->scale_valid, jacobi = st->jacobi, need_lin = st->need_linearize;
-    const double min_diag = st->min_diag, max_diag = st->max_diag, radius = st->radius;
+    const double* grad = reduced ? d.gcr : d.gc;
     double h[6], g[6], sc[6], x[7];
+    if (LOAD_FIRST) {
 #pragma unroll
-    for (int k = 0; k < 6; ++k) {
-        const bool in = k < w;
-        h[k] = in ? d.Hpp[SIDX(d, off + k, off + k)] : 0.0;
-        g[k] = in ? d.gc[off + k] : 0.0;
-        sc[k] = (in && scale_valid) ? d.scale_c[off + k] : 1.0;
+        for (int k = 0; k < 6; ++k) camera_row_load(d, reduced, off + k, k < w, st->scale_valid, h[k], g[k], sc[k]);
+#pragma unroll
+        for (int k = 0; k < 7; ++k) x[k] = (is_pose && st->need_linearize) ? d.poses[7 * i + k] : 0.0;
     }
-#pragma unroll
-    for (int k = 0; k < 7; ++k) x[k] = (is_pose && need_lin) ? d.poses[7 * i + k] : 0.0;
 #pragma unroll
     for (int k = 0; k < 6; ++k) {
         if (k >= w) break;
+        if (!LOAD_FIRST) camera_row_load(d, reduced, off + k, true, st->scale_valid, h[k], g[k], sc[k]);
         const int r = off + k;
-        const double s = scale_valid ? sc[k] : (jacobi ? 1.0 / (1.0 + sqrt(h[k])) : 1.0), s2 = s * s;
-        if (!scale_valid) d.scale_c[r] = s;
-        const double lam = fmin(fmax(s2 * h[k], min_diag), max_diag) / (radius * s2);
-        d.lam_c[r] = lam; d.diagH[r] = h[k]; d.gcr[r] = g[k];
-        atomicAdd(&d.S[SIDX(d, r, r)], h[k] + lam);
-        atomicAdd(&d.rhs[r], -g[k]);
+        const double s = st->scale_valid ? sc[k] : (st->jacobi ? 1.0 / (1.0 + sqrt(h[k])) : 1.0), s2 = s * s;
+        if (!st->scale_valid) d.scale_c[r] = s;
+        const double lam = fmin(fmax(s2 * h[k], st->min_diag), st->max_diag) / (st->radius * s2);
+        d.lam_c[r] = lam;
+        damp(r, h[k], g[k], lam);
     }
-    if (!need_lin) return 0ull;
+    if (!st->need_linearize) return 0ull;
+    const double* xp = LOAD_FIRST ? x : d.poses + 7 * i;
+    const double* gp = LOAD_FIRST ? g : grad + off;
     double gm = 0.0;
     if (is_pose) {
         double ng[6], out[7];
-        for (int k = 0; k < 6; ++k) ng[k] = -g[k];
-        pose_plus(x, ng, out);
-        for (int k = 0; k < 7; ++k) { const double df = fabs(x[k] - out[k]); gm = (df == df) ? fmax(gm, df) : INFINITY; }
-    } else for (int k = 0; k < 3; ++k) { const double df = fabs(g[k]); gm = (df == df) ? fmax(gm, df) : INFINITY; }
+        for (int k = 0; k < 6; ++k) ng[k] = -gp[k];
+        pose_plus(xp, ng, out);
+        for (int k = 0; k < 7; ++k) { const double df = fabs(xp[k] - out[k]); gm = (df == df) ? fmax(gm, df) : INFINITY; }
+    } else for (int k = 0; k < 3; ++k) { const double df = fabs(gp[k]); gm = (df == df) ? fmax(gm, df) : INFINITY; }
     return (gm == gm) ? (unsigned long long)__double_as_longlong(fabs(gm)) : 0x7ff0000000000000ull;
 }
 
@@ -892,7 +892,12 @@ __device__ __forceinline__ void assemble_system(const BaDev& d) {
     const int gid = blockIdx.x * blockDim.x + threadIdx.x, nthr = gridDim.x * blockDim.x, lane = threadIdx.x & 31;
     if (gid < 16) d.scal[gid] = 0.0;
     unsigned long long gbits = 0ull;
-    for (int i = gid; i < d.n_poses + d.n_vec3; i += nthr) gbits = max(gbits, assemble_camera_block(d, i));
+    for (int i = gid; i < d.n_poses + d.n_vec3; i += nthr)       // the block's rows: S[diag] += H_kk + lambda_k, rhs += -g_k
+        gbits = max(gbits, camera_block_step<true>(d, i, false, [&](int r, double h, double g, double lam) {
+            d.diagH[r] = h; d.gcr[r] = g;
+            atomicAdd(&d.S[SIDX(d, r, r)], h + lam);
+            atomicAdd(&d.rhs[r], -g);
+        }));
     warp_max_to_state(d.st, gbits);
     for (int r = gid >> 5; r < d.dimc; r += nthr >> 5) {
         const double* src = d.Hpp + SIDX(d, r, 0);
@@ -1004,48 +1009,27 @@ __global__ void ba_pack_scalars_kernel(BaDev d) {
     d.scal[0] = st->need_linearize ? st->cost_acc : 0.0;
     d.scal[1 + d.rank] = __longlong_as_double((long long)st->grad_max_bits);
 }
+// Cost and the max over the ranks of the gradient norm from the all-reduced scalars (read past L1: other CTAs or peers summed them)
+__device__ __forceinline__ void unpack_scalars(const BaDev& d, LmState* st, int need_lin) {
+    if (need_lin) st->cost_acc = __ldcg(d.scal);
+    double m = 0.0;
+    for (int r = 0; r < d.world; ++r) m = fmax(m, __ldcg(d.scal + 1 + r));
+    st->grad_max_bits = (unsigned long long)__double_as_longlong(m);
+}
 __global__ void ba_unpack_scalars_kernel(BaDev d) {
     LmState* st = d.st;
     if (st->done) return;
-    if (st->need_linearize) st->cost_acc = d.scal[0];
-    double m = 0.0;
-    for (int r = 0; r < d.world; ++r) m = fmax(m, d.scal[1 + r]);
-    st->grad_max_bits = (unsigned long long)__double_as_longlong(m);
+    unpack_scalars(d, st, st->need_linearize);
 }
 
-// camera blocks: Jacobi scale, damping added to diag(S), gradient max-norm ||x - Plus(x,-g)||_inf
-// returns the block's gradient max-norm as ordered bits (0: nothing to report); the caller reduces over the warp and issues ONE atomicMax
-__device__ __forceinline__ unsigned long long prepare_camera_block(const BaDev& d, int i) {
-    LmState* st = d.st;
-    const bool is_pose = i < d.n_poses;
-    const int off = is_pose ? d.pose_off[i] : d.vec3_off[i - d.n_poses];
-    if (off < 0) return 0ull;
-    const int w = is_pose ? 6 : 3;
-    for (int k = 0; k < w; ++k) {
-        const double h = d.diagH[off + k];
-        if (!st->scale_valid) d.scale_c[off + k] = st->jacobi ? 1.0 / (1.0 + sqrt(h)) : 1.0;
-        const double s = d.scale_c[off + k], s2 = s * s;
-        const double lam = fmin(fmax(s2 * h, st->min_diag), st->max_diag) / (st->radius * s2);
-        d.lam_c[off + k] = lam;
-        d.S[SIDX(d, off + k, off + k)] += lam;
-    }
-    if (st->need_linearize) {
-        double gm = 0.0;
-        if (is_pose) {
-            double ng[6], out[7];
-            for (int k = 0; k < 6; ++k) ng[k] = -d.gcr[off + k];
-            const double* x = d.poses + 7 * i;
-            pose_plus(x, ng, out);
-            for (int k = 0; k < 7; ++k) { const double df = fabs(x[k] - out[k]); gm = (df == df) ? fmax(gm, df) : INFINITY; }
-        } else for (int k = 0; k < 3; ++k) { const double df = fabs(d.gcr[off + k]); gm = (df == df) ? fmax(gm, df) : INFINITY; }
-        return (gm == gm) ? (unsigned long long)__double_as_longlong(fabs(gm)) : 0x7ff0000000000000ull;
-    }
-    return 0ull;
+// Sharded problems: the damping of camera block i once diagH and gcr hold the global sums, S[diag] += lambda_k
+__device__ __forceinline__ unsigned long long damp_reduced_camera_block(const BaDev& d, int i) {
+    return camera_block_step<false>(d, i, true, [&](int r, double, double, double lam) { d.S[SIDX(d, r, r)] += lam; });
 }
 
 // S <- lower(Hpp), rhs <- -gc, gcr <- gc, diagH <- diag(Hpp), scalars <- 0.
 // Not launched for the single-GPU window, whose Schur kernel assembles S itself (assemble_system).
-// FUSE_DAMP (single GPU): the camera blocks' Jacobi scale, LM damping and gradient max-norm (prepare_camera_block) ride along: the
+// FUSE_DAMP (single GPU): the camera blocks' Jacobi scale, LM damping and gradient max-norm (camera_block_step) ride along: the
 // bulk copy skips the diagonal and the thread that owns a block fills that block's rows (diagonal of S, rhs, gcr, diagH) and damps
 // them itself, so there is no ordering hazard -- the Schur kernel's `S -= ...` atomics that follow commute with the damping.
 // Sharded problems damp after the all-reduce instead (the diagonal must be the global one) and keep ba_prepare_camera_kernel.
@@ -1063,18 +1047,10 @@ __global__ void ba_build_S_kernel(BaDev d) {
         for (size_t r = gid; r < (size_t)d.dimc; r += stride) { d.diagH[r] = d.Hpp[SIDX(d, r, r)]; d.rhs[r] = -d.gc[r]; d.gcr[r] = d.gc[r]; }
     } else {
         unsigned long long gbits = 0ull;
-        for (size_t i = gid; i < (size_t)(d.n_poses + d.n_vec3); i += stride) {
-            const bool is_pose = i < (size_t)d.n_poses;
-            const int off = is_pose ? d.pose_off[i] : d.vec3_off[i - d.n_poses];
-            if (off < 0) continue;
-            const int w = is_pose ? 6 : 3;
-            for (int k = 0; k < w; ++k) {
-                const int r = off + k;
-                const double h = d.Hpp[SIDX(d, r, r)];
-                d.diagH[r] = h; d.rhs[r] = -d.gc[r]; d.gcr[r] = d.gc[r]; d.S[SIDX(d, r, r)] = h;
-            }
-            gbits = max(gbits, prepare_camera_block(d, (int)i));
-        }
+        for (size_t i = gid; i < (size_t)(d.n_poses + d.n_vec3); i += stride)
+            gbits = max(gbits, camera_block_step<false>(d, (int)i, false, [&](int r, double h, double g, double lam) {
+                d.diagH[r] = h; d.rhs[r] = -g; d.gcr[r] = g; d.S[SIDX(d, r, r)] = h + lam;
+            }));
         warp_max_to_state(d.st, gbits);
     }
 }
@@ -1082,7 +1058,7 @@ __global__ void ba_build_S_kernel(BaDev d) {
 __global__ void ba_prepare_camera_kernel(BaDev d) {
     if (d.st->done) return;
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    warp_max_to_state(d.st, (i < d.n_poses + d.n_vec3) ? prepare_camera_block(d, i) : 0ull);
+    warp_max_to_state(d.st, (i < d.n_poses + d.n_vec3) ? damp_reduced_camera_block(d, i) : 0ull);
 }
 
 // Sharded problems, window size: the exchange of the reduced system and everything that only exists because of it, in ONE kernel
@@ -1105,15 +1081,10 @@ __global__ void __launch_bounds__(256) ba_allreduce_fused_kernel(P2PArgs a, BaDe
     }, &last, &epoch);
     if (!alive || !last) return;
     if (active) {
-        if (threadIdx.x == 0) {
-            if (need_lin) st->cost_acc = __ldcg(d.scal);
-            double m = 0.0;
-            for (int r = 0; r < d.world; ++r) m = fmax(m, __ldcg(d.scal + 1 + r));
-            st->grad_max_bits = (unsigned long long)__double_as_longlong(m);
-        }
+        if (threadIdx.x == 0) unpack_scalars(d, st, need_lin);
         __syncthreads();
         unsigned long long gbits = 0ull;
-        for (int i = threadIdx.x; i < d.n_poses + d.n_vec3; i += blockDim.x) gbits = max(gbits, prepare_camera_block(d, i));
+        for (int i = threadIdx.x; i < d.n_poses + d.n_vec3; i += blockDim.x) gbits = max(gbits, damp_reduced_camera_block(d, i));
         warp_max_to_state(st, gbits);
         __syncthreads();
     }
@@ -1156,21 +1127,15 @@ __global__ void __launch_bounds__(TPB) ba_update_kernel(BaDev d) {
             const int n = d.n[0];
             const int* ix = d.fi[0];
             double s = d.gl[l];
-            for (int eb = e0; eb < e1; eb += 4) {      // four factors at a time, loads before uses (see ba_schur_kernel)
+            for (int eb = e0; eb < e1; eb += 4) {
                 int f[4], o0[4], o1[4];
-#pragma unroll
-                for (int u = 0; u < 4; ++u) f[u] = (eb + u < e1) ? d.lm_fac[eb + u] : -1;
-#pragma unroll
-                for (int u = 0; u < 4; ++u) { const int fc = max(f[u], 0); o0[u] = ix[(size_t)n + fc]; o1[u] = ix[(size_t)2 * n + fc]; }      // unconditional (clamped) loads
-#pragma unroll
-                for (int u = 0; u < 4; ++u) { o0[u] = d.pose_off[o0[u]]; o1[u] = d.pose_off[o1[u]]; }
                 double2 w[4][6];
+                gather_couplings(d, eb, e1, f, w, [&] {
 #pragma unroll
-                for (int u = 0; u < 4; ++u) {
-                    const double2* src = reinterpret_cast<const double2*>(d.tf_w + (size_t)max(f[u], 0) * 12);
+                    for (int u = 0; u < 4; ++u) { const int fc = max(f[u], 0); o0[u] = ix[(size_t)n + fc]; o1[u] = ix[(size_t)2 * n + fc]; }
 #pragma unroll
-                    for (int k = 0; k < 6; ++k) w[u][k] = src[k];
-                }
+                    for (int u = 0; u < 4; ++u) { o0[u] = d.pose_off[o0[u]]; o1[u] = d.pose_off[o1[u]]; }
+                });
 #pragma unroll
                 for (int u = 0; u < 4; ++u) {
                     if (f[u] < 0) continue;
@@ -1190,6 +1155,27 @@ __global__ void __launch_bounds__(TPB) ba_update_kernel(BaDev d) {
     block_add(xn, &st->x_norm2, s_red);
 }
 
+// What an LM decision implies: candidate -> x when `accept`, the accumulators of the next linearisation cleared when `clear`.
+// The calling threads take elements first, first + stride, ...
+__device__ __forceinline__ void accept_and_clear(const BaDev& d, bool accept, bool clear, size_t first, size_t stride) {
+    if (accept) {
+        const size_t np = (size_t)d.n_poses * 7, nv = (size_t)d.n_vec3 * 3, nr = d.n_rho;
+        for (size_t i = first; i < np + nv + nr; i += stride) {
+            if (i < np) d.poses[i] = d.c_poses[i];
+            else if (i < np + nv) d.vec3[i - np] = d.c_vec3[i - np];
+            else d.rho[i - np - nv] = d.c_rho[i - np - nv];
+        }
+    }
+    if (clear) {
+        const size_t nH = d.nS;
+        double2* H2 = reinterpret_cast<double2*>(d.Hpp);
+        for (size_t i = first; i < nH / 2; i += stride) H2[i] = make_double2(0.0, 0.0);
+        if ((nH & 1) && first == 0) d.Hpp[nH - 1] = 0.0;
+        for (size_t i = first; i < (size_t)d.dimc; i += stride) d.gc[i] = 0.0;
+        for (size_t i = first; i < (size_t)d.n_rho; i += stride) { d.Hll[i] = 0.0; d.gl[i] = 0.0; }
+    }
+}
+
 // One CTA closes the iteration: LM decision (thread 0), then -- if the step was accepted -- candidate -> x and the
 // accumulators of the next linearisation are cleared (problems on the dense-solver path are small: < 1 MB).
 __global__ void __launch_bounds__(1024) ba_post_kernel(BaDev d, int decide_only) {
@@ -1203,45 +1189,14 @@ __global__ void __launch_bounds__(1024) ba_post_kernel(BaDev d, int decide_only)
     }
     __syncthreads();
     if (decide_only) return;
-    if (s_accept) {
-        const size_t np = (size_t)d.n_poses * 7, nv = (size_t)d.n_vec3 * 3, nr = d.n_rho;
-        for (size_t i = threadIdx.x; i < np + nv + nr; i += blockDim.x) {
-            if (i < np) d.poses[i] = d.c_poses[i];
-            else if (i < np + nv) d.vec3[i - np] = d.c_vec3[i - np];
-            else d.rho[i - np - nv] = d.c_rho[i - np - nv];
-        }
-    }
-    if (s_zero) {
-        const size_t nH = d.nS;
-        double2* H2 = reinterpret_cast<double2*>(d.Hpp);
-        for (size_t i = threadIdx.x; i < nH / 2; i += blockDim.x) H2[i] = make_double2(0.0, 0.0);
-        if ((nH & 1) && threadIdx.x == 0) d.Hpp[nH - 1] = 0.0;
-        for (size_t i = threadIdx.x; i < (size_t)d.dimc; i += blockDim.x) d.gc[i] = 0.0;
-        for (size_t i = threadIdx.x; i < (size_t)d.n_rho; i += blockDim.x) { d.Hll[i] = 0.0; d.gl[i] = 0.0; }
-    }
+    accept_and_clear(d, s_accept, s_zero, threadIdx.x, blockDim.x);
 }
 
 // Large problems (banded storage) and the single-GPU window pass: the same accept + clear spread over the whole grid.  `accept` may
 // be stale when the solve finished in an earlier pass; the copy is idempotent then (the candidate has not been rewritten).
 __global__ void ba_post_wide_kernel(BaDev d) {
     const LmState* st = d.st;
-    const size_t gid = (size_t)blockIdx.x * blockDim.x + threadIdx.x, stride = (size_t)gridDim.x * blockDim.x;
-    if (st->accept) {
-        const size_t np = (size_t)d.n_poses * 7, nv = (size_t)d.n_vec3 * 3, nr = d.n_rho;
-        for (size_t i = gid; i < np + nv + nr; i += stride) {
-            if (i < np) d.poses[i] = d.c_poses[i];
-            else if (i < np + nv) d.vec3[i - np] = d.c_vec3[i - np];
-            else d.rho[i - np - nv] = d.c_rho[i - np - nv];
-        }
-    }
-    if (!st->done && st->need_linearize) {
-        const size_t nH = d.nS;
-        double2* H2 = reinterpret_cast<double2*>(d.Hpp);
-        for (size_t i = gid; i < nH / 2; i += stride) H2[i] = make_double2(0.0, 0.0);
-        if ((nH & 1) && gid == 0) d.Hpp[nH - 1] = 0.0;
-        for (size_t i = gid; i < (size_t)d.dimc; i += stride) d.gc[i] = 0.0;
-        for (size_t i = gid; i < (size_t)d.n_rho; i += stride) { d.Hll[i] = 0.0; d.gl[i] = 0.0; }
-    }
+    accept_and_clear(d, st->accept, !st->done && st->need_linearize, (size_t)blockIdx.x * blockDim.x + threadIdx.x, (size_t)gridDim.x * blockDim.x);
 }
 
 __global__ void ba_reproj_error_kernel(BaDev d, int n, const double* __restrict__ ob_pw, const int* __restrict__ pose_idx, double* __restrict__ err) {
@@ -1592,7 +1547,7 @@ int lvb_ba_finalize(lvb_ba* ba) {
     for (int k = 0; k < 6; ++k) { d.n[k] = P.nd[k]; d.fc[k] = ba->fc[k].p; d.fi[k] = ba->fi[k].p; d.huber[k] = ba->huber[k]; }
     d.lm_start = ba->lm_start.p; d.lm_fac = ba->lm_fac.p;
     d.tf_slot = ba->tf_slot.p; d.sw_group = ba->sw_group.p; d.sw_lm = ba->sw_lm.p; d.grp_ns = ba->grp_ns.p; d.grp_off = ba->grp_off.p;
-    d.n_schur_warps = P.n_schur_warps; d.warp_syrk = 1;
+    d.n_schur_warps = P.n_schur_warps;
     d.tc_mode = 0; d.tc_u = ba->tc_u.p; d.tc_cdim = ba->tc_cdim.p; d.tc_off = ba->tc_off.p; d.tc_ndim = 6 * npf;
     d.Hpp = ba->Hpp.p; d.gc = ba->gc.p; d.Hll = ba->Hll.p; d.gl = ba->gl.p; d.tf_w = ba->tf_w.p;
     d.S = ba->arena.p; d.rhs = d.S + nH; d.gcr = d.rhs + P.dimc; d.diagH = d.gcr + P.dimc; d.scal = d.diagH + P.dimc;
