@@ -318,6 +318,23 @@ LVB_API int lvb_icp_map_relocate(lvb_icp* ground, lvb_icp* surf, const long long
                                  const void* ground_pts, int n_ground, const void* surf_pts, int n_surf, int stride_bytes,
                                  const lvb_map_optimize_params* p, int rounds, double relative_o_c[7] /* out */, double pose[7] /* out */,
                                  lvb_solve_summary summary[2], double score[2], int n_map_points[2]);
+/* Mapping::ToWorld for n_keys resident keyframes at once (src/mapping.cpp:206-229; called by Mapping::ToWorld(start) after a
+ * GNSS or loop correction, backend.cpp:71-91, relocator.cpp:236-244): the world cloud under keys[i] becomes the float32 SE3
+ * transform of that keyframe's robot-frame cloud (kept on the device since it was stored) by poses[i].cast<float>().
+ *   Each re-anchored cloud is bit for bit what lvb_icp_map_evict(key) + lvb_icp_map_append(key, robot cloud, poses[i]) stores, whichever
+ *   entry point stored it first: the result depends on the robot-frame cloud and poses[i] only, so repeated calls accumulate no error
+ *   and re-anchoring at the pose a cloud was stored with changes nothing.
+ *   ground / surf: one may be NULL; every key must be resident on every handle given; the two must belong to one context.
+ *   keys may come in any order; poses: n_keys x 7 doubles, [qx qy qz qw tx ty tz].
+ * One pinned upload, one kernel over every point of every listed cloud, one host synchronisation, whatever n_keys is; n_keys == 0
+ * launches and waits for nothing.  The bounding boxes of the new clouds are recorded, so the next lvb_icp_map_build_optimize_keyframe
+ * or lvb_icp_map_relocate that merges them pays no extra synchronisation for them.
+ * The world clouds are overwritten in place; nothing else changes: the handles' map frames (copies made by their builds), the
+ * relocation slots, the scan lvb_icp_map_append(NULL) refers to and every cloud not listed stay as they were.  Nothing is exchanged
+ * between ranks: the call is not collective on a sharded context.
+ * Errors, all before any state changes: LVB_ERR_INVALID for an unknown or duplicated key, NULL keys / poses with n_keys > 0,
+ * n_keys < 0, both handles NULL or equal, handles of different contexts. */
+LVB_API int lvb_icp_map_to_world(lvb_icp* ground, lvb_icp* surf, const long long* keys, int n_keys, const double* poses /* n_keys x 7 */);
 
 /* ---- lidar feature pipeline, the producer of the scan-to-map inputs (SURVEY 8(f).2).
  * Stands behind FeatureAssociation::Process (association.cpp:88-268: Preprocess, AdjustDistortion, CalculateSmoothness,

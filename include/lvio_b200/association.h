@@ -16,6 +16,8 @@
 #include <cmath>
 #include <type_traits>
 #include <unordered_map>
+#include <unordered_set>
+#include <vector>
 #include "ceres_shim.h"
 
 // Inside the reference tree the class of the same name already exists (it also owns the feature extraction):
@@ -75,14 +77,42 @@ public:
         Handles& h = handles_of_thread()[this];
         if (!ensure_handles(h)) return false;
         resident_ = &h;
-        const int stride = (int)sizeof(assoc_detail::cloud_data(ground_robot, 0)[0]);
-        lvb_icp_map_evict(h.ground, key); lvb_icp_map_evict(h.surf, key);            // re-registering a keyframe (ToWorld(start)) replaces its clouds
-        return lvb_icp_map_append(h.ground, key, assoc_detail::cloud_data(ground_robot, 0), (int)ground_robot.size(), stride, pose7) == LVB_OK &&
-               lvb_icp_map_append(h.surf, key, assoc_detail::cloud_data(surf_robot, 0), (int)surf_robot.size(), stride, pose7) == LVB_OK;
+        return store_keyframe(h, key, ground_robot, surf_robot, pose7);
     }
     bool EvictKeyframe(long long key) {
         Handles& h = handles_of_thread()[this];
-        return ensure_handles(h) && lvb_icp_map_evict(h.ground, key) == LVB_OK && lvb_icp_map_evict(h.surf, key) == LVB_OK;
+        if (!ensure_handles(h)) return false;
+        if (key < 0) h.keys.clear(); else h.keys.erase(key);
+        return lvb_icp_map_evict(h.ground, key) == LVB_OK && lvb_icp_map_evict(h.surf, key) == LVB_OK;
+    }
+
+    // Mapping::ToWorld(double start) (mapping.cpp:222-229) and Relocator::CorrectLoop's ToWorld loop over the keyframes since old_time
+    // (relocator.cpp:236-244), after a GNSS or loop correction moved their poses: keys[i] / frames[i], n of them, in any order.  The
+    // keyframes this class has stored are re-anchored at frame->pose with ONE device call (lvb_icp_map_to_world: their robot-frame
+    // clouds stay on the device, one host synchronisation for all of them); a lidar keyframe it has not stored (ToWorld(start) also
+    // writes the window's keyframes) goes through AppendKeyframe; a frame without feature_lidar is skipped -- the reference stores
+    // empty clouds for it, which no map frame ever merges.  A key listed twice is re-anchored once.  Like RelocateKeyframe this runs on
+    // the handles that keep the resident clouds, from whichever thread calls it, and the caller holds backend_->mutex
+    // (INTEGRATION.md 3a).  false: a library call failed (lvb_last_error()).
+    template <class FramePtr>
+    bool ToWorldKeyframes(const long long* keys, const FramePtr* frames, int n) {
+        Handles& h = resident_ ? *resident_ : handles_of_thread()[this];
+        if (!ensure_handles(h)) return false;
+        std::vector<long long> moved;
+        std::vector<double> poses;
+        std::unordered_set<long long> seen;
+        bool ok = true;
+        for (int i = 0; i < n; ++i) {
+            const FramePtr& f = frames[i];
+            if (!f->feature_lidar || !seen.insert(keys[i]).second) continue;
+            if (h.keys.count(keys[i])) {
+                moved.push_back(keys[i]);
+                poses.insert(poses.end(), f->pose.data(), f->pose.data() + 7);
+            } else if (!store_keyframe(h, keys[i], f->feature_lidar->points_ground, f->feature_lidar->points_surf, f->pose.data())) {
+                ok = false;
+            }
+        }
+        return lvb_icp_map_to_world(h.ground, h.surf, moved.data(), (int)moved.size(), poses.data()) == LVB_OK && ok;
     }
     bool BuildMapFrame(const long long* keys, int n_keys, double ground_ransac_threshold) {
         Handles& h = handles_of_thread()[this];
@@ -139,10 +169,12 @@ public:
         }
         // ToWorld of a side that was not registered: the call above stores only the clouds of the handles it was given
         const double* pose = frame->pose.data();
+        h.keys.erase(key);                           // until both sides hold the keyframe's clouds again
         if (!reg_g && !(lvb_icp_map_evict(h.ground, key) == LVB_OK &&
                         lvb_icp_map_append(h.ground, key, assoc_detail::cloud_data(g, 0), (int)g.size(), stride, pose) == LVB_OK)) return false;
         if (!reg_s && !(lvb_icp_map_evict(h.surf, key) == LVB_OK &&
                         lvb_icp_map_append(h.surf, key, assoc_detail::cloud_data(s, 0), (int)s.size(), stride, pose) == LVB_OK)) return false;
+        h.keys.insert(key);
         return true;
     }
 
@@ -172,6 +204,7 @@ public:
             return false;
         h.ground_map = n_map[0] > 0; h.surf_map = n_map[1] > 0;
         h.resident = h.ground_map && h.surf_map;
+        h.keys.insert(key);
         resident_ = &h;
         return true;
     }
@@ -243,8 +276,24 @@ private:
     // lvb_icp handles (voxel hash + scratch on one context's stream) are single-threaded and the context is per host thread
     // (ceres_shim.h): Mapping::Optimize and Relocator::RelocateByPoints reach the same object from two threads without a lock
     // (mapping.cpp:155-177, relocator.cpp:188-206), so every thread gets its own pair.
-    // resident: both map frames built (ScanToMapWith* use them); ground_map / surf_map: that side's map frame is the last BuildMapFrame's
-    struct Handles { lvb_icp* ground = nullptr; lvb_icp* surf = nullptr; bool resident = false, ground_map = false, surf_map = false; };
+    // resident: both map frames built (ScanToMapWith* use them); ground_map / surf_map: that side's map frame is the last BuildMapFrame's;
+    // keys: the keyframes whose clouds both handles hold (ToWorldKeyframes re-anchors those on the device)
+    struct Handles {
+        lvb_icp* ground = nullptr; lvb_icp* surf = nullptr; bool resident = false, ground_map = false, surf_map = false;
+        std::unordered_set<long long> keys;
+    };
+    // ToWorld of one keyframe into h: its two robot-frame clouds replace whatever h held under `key`
+    template <class Cloud>
+    static bool store_keyframe(Handles& h, long long key, const Cloud& ground_robot, const Cloud& surf_robot, const double* pose7) {
+        const int stride = (int)sizeof(assoc_detail::cloud_data(ground_robot, 0)[0]);
+        h.keys.erase(key);
+        lvb_icp_map_evict(h.ground, key); lvb_icp_map_evict(h.surf, key);            // re-registering a keyframe (ToWorld(start)) replaces its clouds
+        if (lvb_icp_map_append(h.ground, key, assoc_detail::cloud_data(ground_robot, 0), (int)ground_robot.size(), stride, pose7) != LVB_OK ||
+            lvb_icp_map_append(h.surf, key, assoc_detail::cloud_data(surf_robot, 0), (int)surf_robot.size(), stride, pose7) != LVB_OK)
+            return false;
+        h.keys.insert(key);
+        return true;
+    }
     static bool ensure_handles(Handles& h) {
         lvb::Runtime& rt = lvb::Runtime::get();
         if (!rt.ensure()) return false;

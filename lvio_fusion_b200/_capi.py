@@ -140,6 +140,7 @@ _LVB_ONLY = {
     "icp_map_relocate": (C.c_int, [VP, VP, C.POINTER(C.c_longlong), C.c_int, c_float_p, C.c_double, c_double_p, c_double_p, c_double_p,
                                    VP, C.c_int, VP, C.c_int, C.c_int, C.POINTER(MapOptimizeParams), C.c_int, c_double_p, c_double_p,
                                    C.POINTER(SolveSummary), c_double_p, c_int_p]),
+    "icp_map_to_world": (C.c_int, [VP, VP, C.POINTER(C.c_longlong), C.c_int, c_double_p]),
     "sync_count": (C.c_longlong, [VP]),
     "debug_timing": (C.c_int, [C.c_int]),
     "debug_cholesky_clocks": (C.c_int, [C.POINTER(C.c_longlong), C.c_int]),

@@ -441,6 +441,28 @@ def relocate(ground, surf, keys, cell_sizes, ground_threshold, map_pose, old_pos
     return rel, p, (s[0], s[1]), (float(score[0]), float(score[1])), (int(nm[0]), int(nm[1]))
 
 
+def map_to_world(ground, surf, keys, poses):
+    """Mapping::ToWorld for several resident keyframes at once (mapping.cpp:206-229; Mapping::ToWorld(start) after a GNSS or loop
+    correction) in one device call with one host synchronisation (CUDA library only): the world cloud under keys[i] on `ground` and
+    `surf` (FeatureAssociation handles of one context; one may be None) becomes the float32 transform of that keyframe's robot-frame
+    cloud, kept on the device since it was stored, by poses[i] (n x 7, [qx qy qz qw tx ty tz]).  Bit for bit what map_evict +
+    map_append of the robot-frame cloud at poses[i] stores.  The map frames and every cloud not listed stay as they are."""
+    if ground is None and surf is None:
+        raise ValueError("map_to_world: at least one of ground / surf is needed")
+    if ground is surf:
+        raise ValueError("map_to_world: ground and surf must be two different handles")
+    api = (ground or surf).api
+    keys = [int(x) for x in keys]
+    p = np.ascontiguousarray(poses, dtype=np.float64)
+    if p.size != 7 * len(keys) or (len(keys) and p.shape[-1] != 7):
+        raise ValueError("map_to_world: %d keys need %d x 7 poses, got shape %s" % (len(keys), len(keys), p.shape))
+    if len(set(keys)) != len(keys):
+        raise ValueError("map_to_world: a key is listed twice")
+    k = (C.c_longlong * max(1, len(keys)))(*keys)
+    api.check(api.icp_map_to_world(ground.h if ground else None, surf.h if surf else None, k, len(keys), _dp(p.reshape(-1))),
+              "icp_map_to_world")
+
+
 def _fp(a):
     return None if a is None else a.ctypes.data_as(_capi.c_float_p)
 

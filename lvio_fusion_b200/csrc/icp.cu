@@ -18,6 +18,7 @@
 #include <memory>
 #include <stdlib.h>
 #include <string.h>
+#include <unordered_map>
 #include <vector>
 #include "lvb_internal.cuh"
 #include "lvb_math.cuh"
@@ -158,20 +159,62 @@ __global__ void icp_transform_cloud_kernel(const unsigned char* __restrict__ in,
 }
 
 // Mapping::ToWorld (mapping.cpp:205-220) into the resident store: records of any stride -> packed (x, y, z, intensity) in the world
-// frame; with bbox, also the bounding box of the stored cloud into bbox[6] (icp_bbox_kernel's min / max: equal to what it finds on `out`)
-__global__ void icp_to_world_kernel(const unsigned char* __restrict__ in, float4* __restrict__ out, int n, int stride, const float* __restrict__ tf7, int* bbox) {
+// frame, and the same records untransformed into `robot` (lvb_icp_map_to_world re-anchors from them); with bbox, also the bounding
+// box of the stored cloud into bbox[6] (icp_bbox_kernel's min / max: equal to what it finds on `out`)
+__global__ void icp_to_world_kernel(const unsigned char* __restrict__ in, float4* __restrict__ out, float4* __restrict__ robot, int n, int stride,
+                                    const float* __restrict__ tf7, int* bbox) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     float mn[3] = {FLT_MAX, FLT_MAX, FLT_MAX}, mx[3] = {-FLT_MAX, -FLT_MAX, -FLT_MAX};
     if (i < n) {
         float tf[7];
         for (int k = 0; k < 7; ++k) tf[k] = tf7[k];
         const float* src = reinterpret_cast<const float*>(in + (size_t)i * stride);
+        const float w = stride >= 16 ? src[3] : 0.0f;
         const float3 q = transform_f32(tf, make_float3(src[0], src[1], src[2]));
-        out[i] = make_float4(q.x, q.y, q.z, stride >= 16 ? src[3] : 0.0f);
+        out[i] = make_float4(q.x, q.y, q.z, w);
+        if (robot) robot[i] = make_float4(src[0], src[1], src[2], w);
         mn[0] = fminf(mn[0], q.x); mn[1] = fminf(mn[1], q.y); mn[2] = fminf(mn[2], q.z);
         mx[0] = fmaxf(mx[0], q.x); mx[1] = fmaxf(mx[1], q.y); mx[2] = fmaxf(mx[2], q.z);
     }
     if (bbox) bbox_merge(mn, mx, bbox);
+}
+
+// Mapping::ToWorld(start) (mapping.cpp:222-229) on resident clouds: one entry per (handle, keyframe) re-anchored by lvb_icp_map_to_world
+struct TwSeg {
+    const float4* robot;         // the keyframe's robot-frame records, as icp_to_world_kernel stored them
+    float4* world;               // its world cloud, overwritten in place
+    float tf[7];                 // the new pose.cast<float>()
+    int n;
+};
+enum { TW_TPB = 256, TW_PER = 4 };      // threads per block, points per thread: a block re-anchors 1 024 points of one cloud
+// Every point of every listed cloud: block b belongs to the last entry whose first block is <= b (first[]: the exclusive prefix of
+// ceil(n / 1024) over the entries; an empty cloud owns no block).  The transform is icp_to_world_kernel's, so the result is what
+// lvb_icp_map_append of the same records stores, bit for bit; the box of each cloud goes to boxes[6 * entry] (icp_bbox_kernel's values).
+__global__ void __launch_bounds__(TW_TPB) icp_map_to_world_kernel(const TwSeg* __restrict__ segs, const int* __restrict__ first, int n_segs,
+                                                                  int* __restrict__ boxes) {
+    const int b = blockIdx.x;
+    int lo = 0, hi = n_segs - 1;
+    while (lo < hi) { const int mid = (lo + hi + 1) >> 1; if (__ldg(&first[mid]) <= b) lo = mid; else hi = mid - 1; }
+    const TwSeg& sg = segs[lo];
+    float tf[7];
+    for (int k = 0; k < 7; ++k) tf[k] = sg.tf[k];
+    const int n = sg.n;
+    const float4* __restrict__ in = sg.robot;
+    float4* __restrict__ out = sg.world;
+    const int base = (b - __ldg(&first[lo])) * (TW_TPB * TW_PER) + threadIdx.x;
+    float mn[3] = {FLT_MAX, FLT_MAX, FLT_MAX}, mx[3] = {-FLT_MAX, -FLT_MAX, -FLT_MAX};
+#pragma unroll
+    for (int j = 0; j < TW_PER; ++j) {
+        const int i = base + j * TW_TPB;
+        if (i < n) {
+            const float4 r = __ldg(&in[i]);
+            const float3 q = transform_f32(tf, make_float3(r.x, r.y, r.z));
+            out[i] = make_float4(q.x, q.y, q.z, r.w);
+            mn[0] = fminf(mn[0], q.x); mn[1] = fminf(mn[1], q.y); mn[2] = fminf(mn[2], q.z);
+            mx[0] = fmaxf(mx[0], q.x); mx[1] = fmaxf(mx[1], q.y); mx[2] = fmaxf(mx[2], q.z);
+        }
+    }
+    bbox_merge(mn, mx, boxes + 6 * (size_t)lo);
 }
 
 struct Best3 { float d[3]; int i[3]; int p[3]; };   // d2, original index, position in the sorted array
@@ -647,9 +690,13 @@ struct lvb_icp {
     DevBuf<IcpState> st;
     DevBuf<int> q_key, q_counts, q_start, q_fill, q_sums, q_total, q_order;
     // device-resident world clouds per keyframe (Mapping::pointclouds_surf / _ground, mapping.cpp:208-219) and the merged map frame
-    // lo / hi: the cloud's bounding box (icp_bbox_kernel's), recorded by lvb_icp_map_build_optimize_keyframe for the clouds it stores
-    // and computed by it once for the others (has_bbox false)
-    struct Segment { long long key; DevBuf<float4>* pts = nullptr; int n; bool has_bbox = false; float lo[3], hi[3]; };
+    // robot: the same records in the robot frame (x, y, z, intensity), kept so that lvb_icp_map_to_world can re-anchor the cloud
+    // lo / hi: the cloud's bounding box (icp_bbox_kernel's), recorded by lvb_icp_map_build_optimize_keyframe and lvb_icp_map_to_world
+    // for the clouds they write and computed by the former once for the others (has_bbox false)
+    struct Segment {
+        long long key; DevBuf<float4>* pts = nullptr; DevBuf<float4>* robot = nullptr; int n; bool has_bbox = false; float lo[3], hi[3];
+        void release() { delete pts; delete robot; pts = robot = nullptr; }
+    };
     std::vector<Segment> segments;
     DevBuf<float4> merged, merged2;
     struct MapBufs { DevBuf<float4> sorted; DevBuf<int> cell_start, coarse; };      // a map frame's sorted cloud and voxel hash
@@ -660,7 +707,7 @@ struct lvb_icp {
     // the keyframe calls' upload: [KfBlock | ground scan | surf scan] in one allocation, held by both handles of the call
     // so that either one's scan stays valid for lvb_icp_map_append(NULL) until that handle uploads another scan
     std::shared_ptr<DevBuf<unsigned char>> kf_arena;
-    ~lvb_icp() { for (auto& sg : segments) delete sg.pts; }
+    ~lvb_icp() { for (auto& sg : segments) sg.release(); }
 };
 
 #define ILAUNCH(h, kernel, grid, block, ...)                                              \
@@ -855,15 +902,16 @@ int lvb_icp_map_append(lvb_icp* h, long long key, const void* robot_points, int 
         n = h->scan_n; stride = h->scan_stride; src = h->scan_dev;
     }
     for (auto& sg : h->segments) if (sg.key == key) { set_error("lvb_icp_map_append: key %lld exists", key); return LVB_ERR_INVALID; }
-    lvb_icp::Segment sg; sg.key = key; sg.n = n; sg.pts = new DevBuf<float4>();
+    lvb_icp::Segment sg; sg.key = key; sg.n = n; sg.pts = new DevBuf<float4>(); sg.robot = new DevBuf<float4>();
     int rc = sg.pts->ensure(std::max(1, n));
+    if (rc == LVB_OK) rc = sg.robot->ensure(std::max(1, n));
     DevBuf<float> d_tf;
     float tf[7]; for (int i = 0; i < 7; ++i) tf[i] = (float)pose[i];      // Twc.cast<float>() (mapping.cpp:195)
     if (rc == LVB_OK) rc = d_tf.upload(tf, 7, s);
-    if (rc != LVB_OK) { delete sg.pts; return rc; }
-    ILAUNCH(h, icp_to_world_kernel, inblk(n, 256), 256, src, sg.pts->p, n, stride, d_tf.p, (int*)nullptr);
+    if (rc != LVB_OK) { sg.release(); return rc; }
+    ILAUNCH(h, icp_to_world_kernel, inblk(n, 256), 256, src, sg.pts->p, sg.robot->p, n, stride, d_tf.p, (int*)nullptr);
     rc = icheck("map_append");
-    if (rc != LVB_OK) { delete sg.pts; return rc; }
+    if (rc != LVB_OK) { sg.release(); return rc; }
     LVB_TRY(host_sync(h->ctx, s));
     h->segments.push_back(sg);
     return LVB_OK;
@@ -874,7 +922,7 @@ int lvb_icp_map_evict(lvb_icp* h, long long key) {
     LVB_CUDA(cudaSetDevice(h->ctx->device)); lvb::g_alloc_stream = h->ctx->stream;
     size_t w = 0;
     for (size_t i = 0; i < h->segments.size(); ++i) {
-        if (key < 0 || h->segments[i].key == key) delete h->segments[i].pts; else h->segments[w++] = h->segments[i];
+        if (key < 0 || h->segments[i].key == key) h->segments[i].release(); else h->segments[w++] = h->segments[i];
     }
     h->segments.resize(w);
     return LVB_OK;
@@ -1111,15 +1159,17 @@ static int kf_register(lvb_icp* const hs[2], const bool run[2], const KfMap maps
 }
 
 // The end of Mapping::Optimize's loop body: ToWorld (:185, :205-220) of the scans of every handle given, transformed by the final
-// pose.cast<float>(), into fresh[] (not yet stored; with `boxes`, their bounding boxes into blk->out_bbox)
+// pose.cast<float>(), into fresh[] with their robot-frame records (not yet stored; with `boxes`, their bounding boxes into
+// blk->out_bbox)
 static int kf_to_world(lvb_icp* const hs[2], const KfUpload& u, const int ns[2], int stride, bool boxes, lvb_icp::Segment fresh[2]) {
     for (int m = 0; m < 2; ++m) {
         if (!hs[m]) continue;
-        fresh[m].key = -1; fresh[m].n = ns[m]; fresh[m].pts = new DevBuf<float4>();
-        const int rc = fresh[m].pts->ensure(std::max(1, ns[m]));
-        if (rc != LVB_OK) { delete fresh[0].pts; delete fresh[1].pts; fresh[0].pts = fresh[1].pts = nullptr; return rc; }
-        ILAUNCH(hs[m], icp_to_world_kernel, inblk(ns[m], 256), 256, u.arena->p + u.off[m], fresh[m].pts->p, ns[m], stride, u.blk->tf,
-                boxes ? u.blk->out_bbox[m] : nullptr);
+        fresh[m].key = -1; fresh[m].n = ns[m]; fresh[m].pts = new DevBuf<float4>(); fresh[m].robot = new DevBuf<float4>();
+        int rc = fresh[m].pts->ensure(std::max(1, ns[m]));
+        if (rc == LVB_OK) rc = fresh[m].robot->ensure(std::max(1, ns[m]));
+        if (rc != LVB_OK) { fresh[0].release(); fresh[1].release(); return rc; }
+        ILAUNCH(hs[m], icp_to_world_kernel, inblk(ns[m], 256), 256, u.arena->p + u.off[m], fresh[m].pts->p, fresh[m].robot->p, ns[m], stride,
+                u.blk->tf, boxes ? u.blk->out_bbox[m] : nullptr);
     }
     return LVB_OK;
 }
@@ -1127,7 +1177,7 @@ static int kf_to_world(lvb_icp* const hs[2], const KfUpload& u, const int ns[2],
 // replace the cloud under `key` with sg, or add it
 static void store_segment(lvb_icp* h, long long key, lvb_icp::Segment& sg) {
     sg.key = key;
-    for (auto& old : h->segments) if (old.key == key) { delete old.pts; old = sg; return; }
+    for (auto& old : h->segments) if (old.key == key) { old.release(); old = sg; return; }
     h->segments.push_back(sg);
 }
 
@@ -1172,7 +1222,7 @@ int lvb_icp_map_optimize_keyframe(lvb_icp* ground, lvb_icp* surf, const double m
     LVB_TRY(kf_register(hs, run, maps, u, ns, stride, p));
     LVB_TRY(kf_to_world(hs, u, ns, stride, false, fresh));
     int rc = icheck("map_optimize_keyframe");
-    if (rc != LVB_OK) { delete fresh[0].pts; delete fresh[1].pts; return rc; }
+    if (rc != LVB_OK) { fresh[0].release(); fresh[1].release(); return rc; }
     for (int m = 0; m < 2; ++m) if (hs[m]) store_segment(hs[m], key, fresh[m]);
     // the one read-back: both solver states, rpyxyz and the pose
     LVB_CUDA(cudaMemcpyAsync(u.hb, u.blk, sizeof(KfBlock), cudaMemcpyDeviceToHost, s));
@@ -1374,7 +1424,7 @@ int lvb_icp_map_build_optimize_keyframe(lvb_icp* ground, lvb_icp* surf, const lo
     if (rc == LVB_OK) ctx->stage_busy = false;
     for (int m = 0; m < 2 && rc == LVB_OK; ++m) if (pl.build[m]) rc = grid_error(u.hb->map[m], fn, m ? "surf " : "ground ");
     if (rc != LVB_OK) {        // nothing was committed: the resident clouds and the map frames are as they were
-        delete fresh[0].pts; delete fresh[1].pts;
+        fresh[0].release(); fresh[1].release();
         for (int m = 0; m < 2; ++m) saved[m].restore(hs[m]);
         return rc;
     }
@@ -1457,6 +1507,82 @@ int lvb_icp_map_relocate(lvb_icp* ground, lvb_icp* surf, const long long* keys, 
         }
     }
     memcpy(pose, u.hb->pose, sizeof(u.hb->pose)); memcpy(relative_o_c, u.hb->rel, sizeof(u.hb->rel));
+    return LVB_OK;
+}
+
+// ---- Mapping::ToWorld(start) after a GNSS or loop correction (mapping.cpp:222-229; backend.cpp:71-91, relocator.cpp:236-244): the
+// world clouds of n_keys resident keyframes on one or both handles re-made from their robot-frame records at new poses.  One pinned
+// upload of the table [TwSeg per (handle, key) | first block per entry | boxes], one kernel over every point, the boxes read back with
+// one copy, one host synchronisation.  Every check comes before the upload; the clouds are overwritten in place.
+int lvb_icp_map_to_world(lvb_icp* ground, lvb_icp* surf, const long long* keys, int n_keys, const double* poses) {
+    static const char* fn = "lvb_icp_map_to_world";
+    lvb_icp* hs[2] = {ground, surf};
+    if ((!ground && !surf) || ground == surf || n_keys < 0 || (n_keys > 0 && (!keys || !poses))) {
+        set_error("%s: null or bad argument", fn); return LVB_ERR_INVALID; }
+    if (ground && surf && ground->ctx != surf->ctx) { set_error("%s: the two handles belong to different contexts", fn); return LVB_ERR_INVALID; }
+    if (n_keys == 0) return LVB_OK;
+    {
+        std::vector<long long> sorted(keys, keys + n_keys);
+        std::sort(sorted.begin(), sorted.end());
+        const auto dup = std::adjacent_find(sorted.begin(), sorted.end());
+        if (dup != sorted.end()) { set_error("%s: key %lld is listed twice", fn, *dup); return LVB_ERR_INVALID; }
+    }
+    std::vector<lvb_icp::Segment*> segs;
+    std::vector<int> pose_of;                 // the row of `poses` each entry takes
+    for (int m = 0; m < 2; ++m) {
+        if (!hs[m]) continue;
+        std::unordered_map<long long, lvb_icp::Segment*> at;
+        for (auto& sg : hs[m]->segments) at[sg.key] = &sg;
+        for (int k = 0; k < n_keys; ++k) {
+            const auto it = at.find(keys[k]);
+            if (it == at.end()) { set_error("%s: key %lld is not resident on the %s handle", fn, keys[k], m ? "surf" : "ground"); return LVB_ERR_INVALID; }
+            segs.push_back(it->second); pose_of.push_back(k);
+        }
+    }
+    const size_t S = segs.size();
+    std::vector<int> first(S);
+    size_t blocks = 0;
+    for (size_t i = 0; i < S; ++i) {
+        first[i] = (int)blocks;
+        blocks += inblk(segs[i]->n, TW_TPB * TW_PER);
+        if (blocks > 0x7fffffffull) { set_error("%s: more than 2^31 blocks of %d points", fn, TW_TPB * TW_PER); return LVB_ERR_INVALID; }
+    }
+    int seed[6];
+    bbox_seed(seed);
+    if (blocks == 0) {         // every listed cloud is empty: nothing to write, and their boxes stay the empty seeds
+        for (auto* sg : segs) bbox_store(*sg, seed);
+        return LVB_OK;
+    }
+    lvb_ctx* ctx = (ground ? ground : surf)->ctx;
+    lvb_icp* h0 = ground ? ground : surf;
+    LVB_CUDA(cudaSetDevice(ctx->device)); lvb::g_alloc_stream = ctx->stream;
+    cudaStream_t s = ctx->stream;
+    const size_t off_first = (S * sizeof(TwSeg) + 255) & ~(size_t)255;
+    const size_t off_box = (off_first + S * sizeof(int) + 255) & ~(size_t)255;
+    const size_t all = off_box + S * 6 * sizeof(int);
+    LVB_TRY(lvb::stage_wait(ctx));
+    LVB_TRY(lvb::stage_grow(ctx, all, 0));
+    TwSeg* ht = reinterpret_cast<TwSeg*>(ctx->stage_h);
+    int* hbox = reinterpret_cast<int*>(ctx->stage_h + off_box);
+    for (size_t i = 0; i < S; ++i) {
+        ht[i].robot = segs[i]->robot->p; ht[i].world = segs[i]->pts->p; ht[i].n = segs[i]->n;
+        for (int k = 0; k < 7; ++k) ht[i].tf[k] = (float)poses[7 * (size_t)pose_of[i] + k];      // pose.cast<float>() (mapping.cpp:195)
+        memcpy(hbox + 6 * i, seed, sizeof(seed));
+    }
+    memcpy(ctx->stage_h + off_first, first.data(), S * sizeof(int));
+    DevBuf<unsigned char> d;
+    LVB_TRY(d.ensure(all));
+    LVB_CUDA(cudaMemcpyAsync(d.p, ctx->stage_h, all, cudaMemcpyHostToDevice, s));
+    LVB_TRY(lvb::stage_mark_busy(ctx, s));
+    int* dbox = reinterpret_cast<int*>(d.p + off_box);
+    lvb::timing_mark(s, "begin");        // with per-kernel timing on, the kernel's interval starts after the table's upload
+    ILAUNCH(h0, icp_map_to_world_kernel, (int)blocks, TW_TPB, reinterpret_cast<const TwSeg*>(d.p), reinterpret_cast<const int*>(d.p + off_first),
+            (int)S, dbox);
+    LVB_TRY(icheck(fn));
+    LVB_CUDA(cudaMemcpyAsync(hbox, dbox, S * 6 * sizeof(int), cudaMemcpyDeviceToHost, s));
+    LVB_TRY(host_sync(ctx, s));
+    ctx->stage_busy = false;
+    for (size_t i = 0; i < S; ++i) bbox_store(*segs[i], hbox + 6 * i);
     return LVB_OK;
 }
 
