@@ -18,8 +18,9 @@ bool tree_sep_band_switch() { static const bool on = getenv("LVB_TREE_SEP_BAND")
 
 namespace {
 
-// accumulated SM clocks per Cholesky phase: diag, panel, trailing, backward, total, calls; then the resident kernel's load phase
-// (warps 1..7, overlapping warp 0's first diagonal block) and its calls
+// accumulated SM clocks per Cholesky phase as thread 0 sees them: the diagonal-block factorisations (warp 0), the all-warp panel +
+// head block, warp 0's wait for the rest of each step, backward, total, calls; then the resident kernel's load phase (warps 1..7,
+// overlapping warp 0's first diagonal block) and its calls
 __device__ long long g_chol_dbg[8];
 
 // ------------------------------------------------------------------ single-CTA solve
@@ -27,14 +28,17 @@ __device__ long long g_chol_dbg[8];
 // the right-hand side carried along as an extra row (so the forward substitution is free), then a
 // blocked backward substitution.  Result: rhs <- S^-1 rhs.
 //
-// Schedule of one 32-column step k (look-ahead of depth one, the serial part on its own warp):
-//   warp 0     : panel solve of the 32 "head" rows (= the rows of diagonal block k + 1), one row per lane;  update of diagonal block
-//                k + 1 by these rows as one 32 x 32 register-tiled product, handed to the row-per-lane layout of the factorisation
-//                through shared memory (no trip through global memory);  factorisation of block k + 1 into the OTHER (Dt, invd) buffer
-//   warps 1..7 : the INVERSE of block k of L to the block's place in S (for the backward pass);  panel solve of the remaining rows +
-//                the rhs row;  named barrier (warp 0 only arrives, once its head rows are in shared memory);  trailing update of
-//                everything but diagonal block k + 1
-// so the pivot chain of block k + 1 overlaps the panel and the trailing update of step k instead of following them.
+// Schedule of one 32-column step k (look-ahead of depth one: only the factorisation of the next diagonal block is serial, and it
+// has a warp to itself):
+//   1. all warps : panel solve of every panel row, one row per thread: the 32 "head" rows (= the rows of diagonal block k + 1)
+//                  first, then the others, the rhs row last;  the last warp also stores the INVERSE of block k of L to the
+//                  block's place in S (for the backward pass)
+//   2. warps 0..2: update of the lower triangle of diagonal block k + 1 by the head rows, a 16 x 16 block per warp, staged in the
+//                  free (Dt, invd) buffer
+//   3. warp 0    : block k + 1 minus that update, factored into the free buffer
+//      warps 1..7: trailing update of everything but diagonal block k + 1
+// so the pivot chain of block k + 1 overlaps the trailing update of step k instead of following it.  The last step has no next
+// block and its trailing update is empty: it ends after the panel (the rhs row).
 //
 // The schedule runs on one of two storages of S.  kResident = false: S in global memory (in practice L2), each panel copied to the
 // shared buffer P.  kResident = true (the windows, whenever plan_reduced_solver finds that the envelope fits): warps 1..7 load the
@@ -64,8 +68,9 @@ __global__ void __launch_bounds__(CHOL_T) ba_cholesky_kernel(double* __restrict_
     const CholGlobal G{S, srow, soff};
     const auto W = [&] { if constexpr (kResident) return CholResident{R + ((n + 1) & ~1), boff}; else return G; }();   // chol_resident_rhs
     if (tid == 0) fail = 0;
-    long long t_diag = 0, t_panel = 0, t_trail = 0, t0 = clock64(), tA;
-    const long long t_begin = t0;
+    // 32-bit SM clocks (a call is far shorter than a wrap): 64-bit timers would be spilled out of the loop-carried registers
+    unsigned t_fact = 0, t_panel = 0, t_wait = 0, t0 = clock(), tA;
+    const unsigned t_begin = t0;
     // ---- diagonal block 0: warp 0, one row per lane in registers (lvb_chol.cuh), from global memory in both storages
     if (warp == 0) {
         const int b0 = min(32, n);
@@ -75,6 +80,7 @@ __global__ void __launch_bounds__(CHOL_T) ba_cholesky_kernel(double* __restrict_
         if (st->done) return;                       // uniform over the CTA, like the check of the other warps
         const int bad = chol_diag32_pair(a, lane, sm, sm + 32 * 34);
         if (bad && lane == 0) fail = 1;
+        tA = clock(); t_fact += tA - t0; t0 = tA;
     } else if (st->done) {
         return;
     } else if constexpr (kResident) {
@@ -96,10 +102,10 @@ __global__ void __launch_bounds__(CHOL_T) ba_cholesky_kernel(double* __restrict_
             }
             o += cnt / 32 * 34;
         }
-        if (t1 == 0) t_load = clock64() - t0;
+        if (t1 == 0) t_load = (unsigned)clock() - t0;
     }
     __syncthreads();
-    tA = clock64(); t_diag += tA - t0; t0 = tA;
+    tA = clock(); t_wait += tA - t0; t0 = tA;
     for (int kb = 0; kb < n; kb += 32) {
         const int bs = min(32, n - kb), kn = kb + 32;
         const int hb = max(0, min(32, n - kn));                    // rows of the next diagonal block ("head" rows of the panel)
@@ -112,71 +118,75 @@ __global__ void __launch_bounds__(CHOL_T) ba_cholesky_kernel(double* __restrict_
         // panel row rr < m - 1 at P + rr * 34, the rhs row at Prhs (resident: the panel is block column k below its diagonal block)
         double* const P = kResident ? W.at(kb + bs, kb) : part;
         double* const Prhs = kResident ? R + kb : P + (m - 1) * 34;
-        if (warp == 0 && hb > 0) {
-            double x[32], a[32];
+        // the INVERSE of block kb of L goes to the block's place in S: the backward pass then applies a diagonal block as 32 independent
+        // FMAs per lane instead of a 32-step substitution chain.  Column c of L^-1 is the panel solve of the unit row e_c; one warp
+        // (the last one, which has the fewest panel rows) does it while the others are in the panel.
+        if (warp == nw - 1) {
+            double e[32];
 #pragma unroll
-            for (int j = 0; j < 32; ++j) x[j] = (lane < mh && j < bs) ? W.at(kn + lane, kb)[j] : 0.0;
+            for (int j = 0; j < 32; ++j) e[j] = (j == lane) ? 1.0 : 0.0;
+            chol_panel_row(e, Dt, invd);
+#pragma unroll
+            for (int j = 0; j < 32; ++j) if (j >= lane && j < bs) W.at(kb + j, kb)[lane] = e[j];
+        }
+        // ---- panel, one row per thread:  x L^T = a, right-looking, no divisions.  Rows 0 .. mh - 1 are the head rows.
+        for (int rr = tid; rr < m; rr += nt) {
+            const bool is_rhs = (rr == m - 1);
+            double* src = is_rhs ? (R + kb) : W.at(kb + bs + rr, kb);
+            double a[32];
+#pragma unroll
+            for (int j = 0; j < 32; ++j) a[j] = (j < bs) ? src[j] : 0.0;
+            chol_panel_row(a, Dt, invd);
+#pragma unroll
+            for (int j = 0; j < 32; ++j) { if (!kResident) P[rr * 34 + j] = a[j]; if (j < bs) src[j] = a[j]; }
+        }
+        __syncthreads();
+        if (hb == 0) {                         // the last step: nothing right of the block (env_rmax <= n - 1, so m == 1)
+            tA = clock(); t_panel += tA - t0; t0 = tA;
+            break;
+        }
+        // ---- head block: diagonal block kn -= (head rows)(head rows)^T on its lower triangle, staged in the free diagonal-block
+        // buffer for warp 0's row-per-lane layout.  Warps 0..2 each form one of the 16 x 16 blocks (0, 0), (16, 0), (16, 16), lane
+        // (ry, cx) a 2 x 4 micro-tile (chol_tile_product: each entry summed as the trailing update sums it).  The block (0, 16) lies
+        // above the diagonal, which chol_diag32_pair never lets into the lower triangle, so it is not formed: this phase is bound by
+        // the product's shared-memory loads, not by its DFMAs.  Head rows outside the envelope are structurally zero and have no
+        // panel row.
+        if (mh > 0 && warp < 3) {
+            const int R0 = warp ? 16 : 0, C0 = warp == 2 ? 16 : 0, ry = lane >> 2, cx = lane & 3;
+            double acc[2][4] = {};
+            const double2* rp[2]; const double2* cp[4];
+#pragma unroll
+            for (int i = 0; i < 2; ++i) rp[i] = reinterpret_cast<const double2*>(P + (size_t)min(R0 + ry + 8 * i, mh - 1) * 34);
+#pragma unroll
+            for (int j = 0; j < 4; ++j) cp[j] = reinterpret_cast<const double2*>(P + (size_t)min(C0 + cx + 4 * j, mh - 1) * 34);
+            chol_tile_product(acc, rp, cp);
+#pragma unroll
+            for (int i = 0; i < 2; ++i)
+#pragma unroll
+                for (int j = 0; j < 4; ++j) {
+                    const int r = R0 + ry + 8 * i, c = C0 + cx + 4 * j;
+                    Dn[r * 34 + c] = (r < mh && c < mh) ? acc[i][j] : 0.0;
+                }
+        }
+        __syncthreads();
+        tA = clock(); t_panel += tA - t0; t0 = tA;
+        if (warp == 0) {
+            // ---- factorisation of block kn into the free buffer (loading the block earlier, to overlap the head block, spills)
+            double a[32];
 #pragma unroll
             for (int j = 0; j < 32; ++j) a[j] = (lane < hb && j <= lane) ? W.at(kn + lane, kn)[j] : ((j == lane) ? 1.0 : 0.0);
-            chol_panel_row(x, Dt, invd);
-#pragma unroll
-            for (int j = 0; j < 32; ++j) if (lane < mh) { P[lane * 34 + j] = x[j]; if (!kResident && j < bs) W.at(kn + lane, kb)[j] = x[j]; }
-            __syncwarp();
-            asm volatile("bar.arrive 1, %0;" :: "r"(nt) : "memory");
-            tA = clock64(); t_panel += tA - t0; t0 = tA;
-            // diagonal block kn -= (head rows)(head rows)^T: computed as a 32 x 32 tile in the 4 x 8 register micro-tile layout of the
-            // trailing update (12 LDS.128 per 64 DFMA; the row-per-lane layout would need one LDS.128 per 2 DFMA and is bound by the
-            // shared-memory return path), then passed through the free diagonal-block buffer to the row-per-lane layout of the
-            // factorisation.  Head rows outside the envelope are structurally zero and have no panel row.
             if (mh > 0) {
-                const int ry = lane >> 2, cx = lane & 3;
-                double acc[4][8] = {};
-                const double2* rp[4]; const double2* cp[8];
-#pragma unroll
-                for (int i = 0; i < 4; ++i) rp[i] = reinterpret_cast<const double2*>(P + (size_t)min(ry + 8 * i, mh - 1) * 34);
-#pragma unroll
-                for (int j = 0; j < 8; ++j) cp[j] = reinterpret_cast<const double2*>(P + (size_t)min(cx + 4 * j, mh - 1) * 34);
-                chol_tile_product(acc, rp, cp);
-#pragma unroll
-                for (int i = 0; i < 4; ++i)
-#pragma unroll
-                    for (int j = 0; j < 8; ++j) Dn[(ry + 8 * i) * 34 + cx + 4 * j] = (ry + 8 * i < mh && cx + 4 * j < mh) ? acc[i][j] : 0.0;
-                __syncwarp();
 #pragma unroll
                 for (int j = 0; j < 32; ++j) a[j] -= Dn[lane * 34 + j];
                 __syncwarp();
             }
             const int bad = chol_diag32_pair(a, lane, Dn, Dn + 32 * 34);
             if (bad && lane == 0) fail = 1;
-            tA = clock64(); t_diag += tA - t0; t0 = tA;
+            tA = clock(); t_fact += tA - t0; t0 = tA;
         } else {
-            const int wid = hb > 0 ? warp - 1 : warp, nwk = hb > 0 ? nw - 1 : nw;       // the warps doing this part
-            const int t2 = wid * 32 + lane, nt2 = nwk * 32;
-            // the INVERSE of block kb of L goes to the block's place in S: the backward pass then applies a diagonal block as 32 independent
-            // FMAs per lane instead of a 32-step substitution chain.  Column c of L^-1 is the panel solve of the unit row e_c; one warp
-            // (the last one, which has the fewest panel rows) does it while the others are in the panel.
-            if (wid == nwk - 1) {
-                double e[32];
-#pragma unroll
-                for (int j = 0; j < 32; ++j) e[j] = (j == lane) ? 1.0 : 0.0;
-                chol_panel_row(e, Dt, invd);
-#pragma unroll
-                for (int j = 0; j < 32; ++j) if (j >= lane && j < bs) W.at(kb + j, kb)[lane] = e[j];
-            }
-            // ---- panel, the rows warp 0 does not take:  x L^T = a, right-looking, no divisions
-            for (int rr = mh + t2; rr < m; rr += nt2) {
-                const bool is_rhs = (rr == m - 1);
-                double* src = is_rhs ? (R + kb) : W.at(kb + bs + rr, kb);
-                double a[32];
-    #pragma unroll
-                for (int j = 0; j < 32; ++j) a[j] = (j < bs) ? src[j] : 0.0;
-                chol_panel_row(a, Dt, invd);
-    #pragma unroll
-                for (int j = 0; j < 32; ++j) { if (!kResident) P[rr * 34 + j] = a[j]; if (j < bs) src[j] = a[j]; }
-            }
-            asm volatile("bar.sync 1, %0;" :: "r"(nt) : "memory");
-            // ---- trailing update A22 -= P P^T on the lower triangle: one warp per 32x32 tile, each lane a 4x8 register micro-tile
-            // (chol_tile_product).  The head rows of tile (0, 0) -- diagonal block kn -- are warp 0's.
+            // ---- trailing update A22 -= P P^T on the lower triangle but diagonal block kn: one warp per 32x32 tile, each lane a 4x8
+            // register micro-tile (chol_tile_product)
+            const int wid = warp - 1, nwk = nw - 1;
             const int ntile = (m + 31) >> 5;
             const int total = (m > 1) ? ntile * (ntile + 1) / 2 : 0;
             for (int t = wid; t < total; t += nwk) {
@@ -216,7 +226,7 @@ __global__ void __launch_bounds__(CHOL_T) ba_cholesky_kernel(double* __restrict_
             }
         }
         __syncthreads();
-        tA = clock64(); t_trail += tA - t0; t0 = tA;
+        tA = clock(); t_wait += tA - t0; t0 = tA;
     }
     // ---- backward substitution  L^T x = y  (y is in rhs), left-looking per 32-column block:
     //   x_k = D_k^-T (y_k - sum_{r below} L[r][k-block]^T x_r),  D_k^-1 stored in place of D_k by the factorisation
@@ -264,7 +274,7 @@ __global__ void __launch_bounds__(CHOL_T) ba_cholesky_kernel(double* __restrict_
     if (kResident) for (int i = tid; i < n; i += nt) rhs[i] = R[i];
     if (tid == 0 && fail) st->solve_fail = 1;
     if (tid == 0) {
-        tA = clock64(); g_chol_dbg[0] += t_diag; g_chol_dbg[1] += t_panel; g_chol_dbg[2] += t_trail; g_chol_dbg[3] += tA - t0; g_chol_dbg[4] += tA - t_begin; g_chol_dbg[5] += 1;
+        tA = clock(); g_chol_dbg[0] += t_fact; g_chol_dbg[1] += t_panel; g_chol_dbg[2] += t_wait; g_chol_dbg[3] += tA - t0; g_chol_dbg[4] += tA - t_begin; g_chol_dbg[5] += 1;
         if (kResident) { g_chol_dbg[6] += t_load; g_chol_dbg[7] += 1; }
     }
 }

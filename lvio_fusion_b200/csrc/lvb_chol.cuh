@@ -116,23 +116,25 @@ __device__ __forceinline__ void chol_tile_index(const int t, int& ti, int& tj) {
     tj = t - ti * (ti + 1) / 2;
 }
 
-// One lane's 4 x 8 register micro-tile of a 32 x 32 tile of P P^T: acc[i][j] += (row rp[i]) . (row cp[j]) over 32 columns, rows read
-// as double2.  The callers give lane the rows ry + 8 i and the columns cx + 4 j (ry = lane / 4, cx = lane % 4): consecutive lanes
+// One lane's RI x CJ register micro-tile of a tile of P P^T: acc[i][j] += (row rp[i]) . (row cp[j]) over 32 columns, rows read
+// as double2, every entry accumulated in the same order (k = 0..15, .x then .y) whatever the micro-tile's shape.  The trailing
+// updates use 4 x 8 and give lane the rows ry + 8 i and the columns cx + 4 j (ry = lane / 4, cx = lane % 4): consecutive lanes
 // touch consecutive panel rows, so the LDS.128 operand loads are bank-conflict free and every loaded value feeds 4 or 8 DFMAs.
 // The callers zero acc before they set up rp and cp: zeroing it here instead makes the compiler schedule ba_front_factor_kernel
 // differently.
-__device__ __forceinline__ void chol_tile_product(double (&acc)[4][8], const double2* const (&rp)[4], const double2* const (&cp)[8]) {
+template <int RI, int CJ>
+__device__ __forceinline__ void chol_tile_product(double (&acc)[RI][CJ], const double2* const (&rp)[RI], const double2* const (&cp)[CJ]) {
 #pragma unroll 2
     for (int k = 0; k < 16; ++k) {
-        double2 rv[4], cv[8];
+        double2 rv[RI], cv[CJ];
 #pragma unroll
-        for (int i = 0; i < 4; ++i) rv[i] = rp[i][k];
+        for (int i = 0; i < RI; ++i) rv[i] = rp[i][k];
 #pragma unroll
-        for (int j = 0; j < 8; ++j) cv[j] = cp[j][k];
+        for (int j = 0; j < CJ; ++j) cv[j] = cp[j][k];
 #pragma unroll
-        for (int i = 0; i < 4; ++i)
+        for (int i = 0; i < RI; ++i)
 #pragma unroll
-            for (int j = 0; j < 8; ++j) { acc[i][j] += rv[i].x * cv[j].x; acc[i][j] += rv[i].y * cv[j].y; }
+            for (int j = 0; j < CJ; ++j) { acc[i][j] += rv[i].x * cv[j].x; acc[i][j] += rv[i].y * cv[j].y; }
     }
 }
 
