@@ -292,6 +292,53 @@ LVB_API int lvb_icp_map_build_optimize_keyframe(lvb_icp* ground, lvb_icp* surf, 
                                                 const void* ground_pts, int n_ground, const void* surf_pts, int n_surf, int stride_bytes,
                                                 const lvb_map_optimize_params* p, double pose[7] /* in: frame->pose, out: optimised */,
                                                 double rpyxyz[6] /* out */, lvb_solve_summary summary[2], int n_map_points[2]);
+/* Mapping::Optimize(active_kfs) (mapping.cpp:139-191) for the n_kf lidar keyframes of a backend pass, in time order, in one call with
+ * one host synchronisation: for k = 0 .. n_kf-1, on the device,
+ *   incoming pose  pose_k = T_{k-1} * ( ... (T_0 * pose)), pose as the caller holds it: the PoseGraph::ForwardUpdate(T_j, t_j + eps)
+ *                  of every earlier keyframe of the call, in order (pose_graph.cpp:245-252)
+ *   map frame      map_keys (0 to 3, merge order: get_lidar_frames(0, t_k, 3)), each a cloud resident on both handles before the call or
+ *                  the key of an earlier keyframe of the call (then the clouds this call stored for it); built as
+ *                  lvb_icp_map_build_optimize_keyframe builds it.  map_pose: that of the newest map key -- the optimised pose of that
+ *                  keyframe when it is in the call, the record's map_pose otherwise.
+ *   registrations  as lvb_icp_map_build_optimize_keyframe: both sides, the pose hand-off, a side with an empty merged cloud or whose
+ *                  SegmentGround keeps no point is not registered, no map keys register nothing
+ *   transform      T_k = pose_k(optimised) * pose_k(incoming)^-1 (mapping.cpp:181-182)
+ *   ToWorld        both clouds stored under `key`, replacing what it held; later keyframes of the call merge them from there.
+ * Every SE3 product and inverse rounds each double operation on its own: lvio_fusion_b200/se3.py restates them bit for bit, and
+ * replaying ForwardUpdate(transform, t_k + eps) with Sophus on the host moves the frames after each keyframe as the reference does.
+ * The records are read (inputs) and written (outputs, only when the call succeeds).  Each record's weight[2] and prior_weight are that
+ * keyframe's (ScanToMapWith* take them from each frame: the lidar weights and features_left.size() * weights.visual, association.cpp:
+ * 318-323, 376-381) and replace p's; the rest of p, cell_size[2], ground_threshold and stride_bytes are
+ * lvb_icp_map_build_optimize_keyframe's and apply to every keyframe.  Each summary's total_time_in_seconds is the whole call's.  Keys of the call are distinct.  The launch sequence depends
+ * only on the sizes and the options.  n_kf == 1 is lvb_icp_map_build_optimize_keyframe, bit for bit, with the same launches and
+ * synchronisations; n_kf == 0 launches and waits for nothing.
+ * Afterwards each handle is as the step-by-step loop leaves it: its map frame is the newest one built with points, map_append(NULL)
+ * refers to the last keyframe's scan.  A map frame that merges clouds of the call is sized from their robot-frame boxes at the
+ * incoming poses the caller gave, widened by 1 m; a cloud that ends up outside makes that grid coarser (the 3-NN stays exact), and
+ * only a grid that does not fit at ring 1 fails (LVB_ERR_UNSUPPORTED).
+ * Errors, all before any state changes: as lvb_icp_map_build_optimize_keyframe (time limit set, sharded context, handles of different
+ * contexts, bad cell size or gate), and LVB_ERR_INVALID for a map key that is neither resident nor an earlier keyframe of the call, a
+ * key listed twice, a key among its own map keys, or n_map_keys outside 0..3.  Failures found on the device in any keyframe (no finite
+ * bounding box, grid overflow) are reported after the synchronisation and commit nothing: every resident cloud, map frame and the
+ * map_append(NULL) scan stay as they were. */
+typedef struct lvb_map_keyframe {
+    long long key;                          /* in: the keyframe's time key */
+    long long map_keys[3];                  /* in: its map frame's keys, merge order */
+    int n_map_keys;                         /* in: 0 to 3 */
+    int n_ground, n_surf;                   /* in: robot-frame cloud sizes */
+    const void* ground_pts;                 /* in: n_ground records of stride_bytes */
+    const void* surf_pts;                   /* in: n_surf records */
+    double map_pose[7];                     /* in: the newest map key's pose (unused when it is a keyframe of the call) */
+    double pose[7];                         /* in: frame->pose; out: optimised */
+    double weight[2];                       /* in: ground, surf registration weight of this keyframe */
+    double prior_weight;                    /* in: this keyframe's prior weight (< 0: no prior) */
+    double transform[7];                    /* out: T_k */
+    double rpyxyz[6];                       /* out */
+    lvb_solve_summary summary[2];           /* out: ground, surf; termination_type -1 when not registered */
+    int n_map_points[2];                    /* out: each map frame's size (0 = not built) */
+} lvb_map_keyframe;
+LVB_API int lvb_icp_map_optimize_keyframes(lvb_icp* ground, lvb_icp* surf, lvb_map_keyframe* kfs, int n_kf, const float cell_size[2],
+                                           double ground_threshold, int stride_bytes, const lvb_map_optimize_params* p);
 /* Mapping::Relocate for one loop-closure candidate (mapping.cpp:78-112, 251-300), with one host synchronisation:
  *   pose = old_pose * relative_guess                                 (clone_frame->pose, :256)
  *   BuildOldMapFrame: the map frame of keys / n_keys (1 to 3: the lidar keyframe before the old one, the old one if it has lidar, the
@@ -372,6 +419,9 @@ LVB_API int lvb_lidar_extract_features(lvb_ctx* ctx, const lvb_lidar_config* cfg
 LVB_API int lvb_debug_timing(int enable);
 /* as lvb_debug_timing(0), but writes "kernel_name microseconds" lines (launch order) into out instead of printing them */
 LVB_API int lvb_debug_timing_report(char* out, int cap);
+/* the voxel grid of the handle's current map frame: grid[0] = ring (voxels per search radius: 4, 2 or 1), grid[1..3] = voxels per
+ * axis.  LVB_ERR_STATE without a map frame. */
+LVB_API int lvb_debug_icp_map_grid(lvb_icp* icp, int grid[4]);
 /* the reduced-system solver alone (parity test of the multifrontal tree, ba_tree.cuh): S x = b for an SPD band matrix stored as
  * n rows of band + 1 entries (row i = columns i - band .. i), true half bandwidth <= band - 31; use_tree 0 forces the single-CTA
  * envelope kernel (or, when its panel does not fit in shared memory, the per-phase grids of ba_wide.cuh); *levels_out = tree levels

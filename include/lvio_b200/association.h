@@ -209,6 +209,55 @@ public:
         return true;
     }
 
+    // Mapping::Optimize(active_kfs) (mapping.cpp:139-191) for its n lidar keyframes, in time order, in ONE device call with one host
+    // synchronisation (lvb_icp_map_optimize_keyframes): frames[k] is keyframe keys[k]; its map frame is map_keys[3 k .. 3 k +
+    // n_map_keys[k]) (get_lidar_frames(0, t_k, 3), merge order), resident or keys of earlier frames of the call; map_poses7[7 k]: the
+    // newest map key's pose when it is resident.  frame->pose goes in as the caller holds it -- before the earlier keyframes'
+    // ForwardUpdates, which the device chains -- and comes back optimised, also copied to poses7 (n x 7).  transforms7 (n x 7): T_k =
+    // new_k * old_k^-1, in order; the caller replays PoseGraph::ForwardUpdate(T_k, t_k + epsilon) and then writes poses7 back to the
+    // frames of the call (INTEGRATION.md 3a).  Each keyframe registers with its own MapOptimizeParams weights and prior weight, as
+    // ScanToMapWith* would.  summary: 2 per keyframe or NULL.  false: the call failed and changed nothing (the
+    // per-keyframe OptimizeKeyframe loop is the fallback; lvb_last_error() says why).
+    template <class FramePtr>
+    bool OptimizeKeyframes(const FramePtr* frames, const long long* keys, const long long* map_keys, const int* n_map_keys, const double* map_poses7,
+                           int n, double ground_ransac_threshold, double* poses7, double* transforms7, lvb_solve_summary* summary = nullptr) {
+        Handles& h = handles_of_thread()[this];
+        if (!ensure_handles(h)) return false;
+        if (n <= 0) return true;
+        std::vector<lvb_map_keyframe> recs(n);
+        int stride = 0;
+        for (int k = 0; k < n; ++k) {
+            const auto& g = frames[k]->feature_lidar->points_ground;
+            const auto& s = frames[k]->feature_lidar->points_surf;
+            stride = (int)sizeof(assoc_detail::cloud_data(g, 0)[0]);
+            lvb_map_keyframe& r = recs[k];
+            std::memset(&r, 0, sizeof(r));
+            r.key = keys[k]; r.n_map_keys = n_map_keys[k];
+            for (int i = 0; i < n_map_keys[k] && i < 3; ++i) r.map_keys[i] = map_keys[3 * k + i];
+            r.ground_pts = assoc_detail::cloud_data(g, 0); r.n_ground = (int)g.size();
+            r.surf_pts = assoc_detail::cloud_data(s, 0); r.n_surf = (int)s.size();
+            std::memcpy(r.map_pose, map_poses7 + 7 * k, sizeof(r.map_pose)); std::memcpy(r.pose, frames[k]->pose.data(), sizeof(r.pose));
+            const lvb_map_optimize_params pk = MapOptimizeParams(frames[k]);      // each keyframe's own weights and prior weight
+            r.weight[0] = pk.weight[0]; r.weight[1] = pk.weight[1]; r.prior_weight = pk.prior_weight;
+        }
+        const lvb_map_optimize_params p = MapOptimizeParams(frames[0]);          // the options, gates and losses every keyframe shares
+        const float cells[2] = {cell_of(resolution_ * resolution_ * 100), cell_of(resolution_ * resolution_ * 25)};
+        if (lvb_icp_map_optimize_keyframes(h.ground, h.surf, recs.data(), n, cells, ground_ransac_threshold, stride, &p) != LVB_OK) return false;
+        for (int k = 0; k < n; ++k) {
+            const lvb_map_keyframe& r = recs[k];
+            std::memcpy(frames[k]->pose.data(), r.pose, sizeof(r.pose));
+            if (poses7) std::memcpy(poses7 + 7 * k, r.pose, sizeof(r.pose));
+            if (transforms7) std::memcpy(transforms7 + 7 * k, r.transform, sizeof(r.transform));
+            if (summary) { summary[2 * k] = r.summary[0]; summary[2 * k + 1] = r.summary[1]; }
+            h.keys.insert(keys[k]);
+        }
+        // as OptimizeKeyframe(frame, keys, ...) leaves them after the last keyframe: that keyframe's map frames
+        h.ground_map = recs[n - 1].n_map_points[0] > 0; h.surf_map = recs[n - 1].n_map_points[1] > 0;
+        h.resident = h.ground_map && h.surf_map;
+        resident_ = &h;
+        return true;
+    }
+
     // Mapping::Relocate for one loop-closure candidate (mapping.cpp:78-112, 251-300) in ONE device call with one host synchronisation
     // (lvb_icp_map_relocate): BuildOldMapFrame of `keys` (1 to 3 resident keyframes in time order: the lidar keyframe before the old
     // one, the old one if it has lidar, the one after it; map_pose7 = the earliest one's pose) with BuildMapFrame's cell sizes and

@@ -76,6 +76,27 @@ class MapOptimizeParams(C.Structure):
     ]
 
 
+class MapKeyframe(C.Structure):
+    """lvb_map_keyframe (include/lvio_b200.h): one keyframe of lvb_icp_map_optimize_keyframes, inputs and outputs."""
+    _fields_ = [
+        ("key", C.c_longlong),
+        ("map_keys", C.c_longlong * 3),
+        ("n_map_keys", C.c_int),
+        ("n_ground", C.c_int),
+        ("n_surf", C.c_int),
+        ("ground_pts", C.c_void_p),
+        ("surf_pts", C.c_void_p),
+        ("map_pose", C.c_double * 7),
+        ("pose", C.c_double * 7),
+        ("weight", C.c_double * 2),
+        ("prior_weight", C.c_double),
+        ("transform", C.c_double * 7),
+        ("rpyxyz", C.c_double * 6),
+        ("summary", SolveSummary * 2),
+        ("n_map_points", C.c_int * 2),
+    ]
+
+
 VP = C.c_void_p
 _SIGS = {
     "version": (C.c_int, []),
@@ -141,10 +162,13 @@ _LVB_ONLY = {
                                    VP, C.c_int, VP, C.c_int, C.c_int, C.POINTER(MapOptimizeParams), C.c_int, c_double_p, c_double_p,
                                    C.POINTER(SolveSummary), c_double_p, c_int_p]),
     "icp_map_to_world": (C.c_int, [VP, VP, C.POINTER(C.c_longlong), C.c_int, c_double_p]),
+    "icp_map_optimize_keyframes": (C.c_int, [VP, VP, C.POINTER(MapKeyframe), C.c_int, c_float_p, C.c_double, C.c_int,
+                                             C.POINTER(MapOptimizeParams)]),
     "sync_count": (C.c_longlong, [VP]),
     "debug_timing": (C.c_int, [C.c_int]),
     "debug_cholesky_clocks": (C.c_int, [C.POINTER(C.c_longlong), C.c_int]),
     "debug_timing_report": (C.c_int, [C.c_char_p, C.c_int]),
+    "debug_icp_map_grid": (C.c_int, [VP, c_int_p]),
     "debug_band_solve": (C.c_int, [VP, C.c_int, C.c_int, c_double_p, c_double_p, c_double_p, C.c_int, c_int_p]),
 }
 

@@ -415,6 +415,67 @@ def build_and_optimize_keyframe(ground, surf, keys, cell_sizes, ground_threshold
     return p, e, (s[0], s[1]), (int(nm[0]), int(nm[1]))
 
 
+def build_and_optimize_keyframes(ground, surf, keyframes, cell_sizes, ground_threshold, weight, prior_weight, huber_a, dist_thr,
+                                 options=None, **kw):
+    """Mapping::Optimize(active_kfs) (mapping.cpp:139-191) for a chain of lidar keyframes in one device call with one host
+    synchronisation (CUDA library only).  keyframes: in time order, each (key, map_keys, map_pose, pose, ground_points, surf_points):
+    map_keys (0 to 3, merge order) are resident keys or keys of earlier keyframes of the chain; map_pose is used when the newest map
+    key is resident; pose is the incoming pose as the caller holds it, before the earlier keyframes' ForwardUpdates (the device chains
+    them, se3.forward_update restates it).  weight ((ground, surf)) and prior_weight are each keyframe's own, as ScanToMapWith* take
+    them from each frame: one value for all keyframes, or one per keyframe (n x 2 and n).  The other arguments are
+    build_and_optimize_keyframe's and apply to every keyframe.
+    Returns one (pose, transform, rpyxyz, (ground summary, surf summary), (ground map points, surf map points)) per keyframe, with
+    transform = optimised pose * incoming pose^-1, the T of PoseGraph::ForwardUpdate(T, t_k + epsilon)."""
+    fn = "build_and_optimize_keyframes"
+    if ground is None or surf is None:
+        raise ValueError("%s: both the ground and the surf handle are needed" % fn)
+    if ground is surf:
+        raise ValueError("%s: ground and surf must be two different handles" % fn)
+    n_kf = len(keyframes)
+    w = np.asarray(weight, dtype=np.float64)
+    pw = np.asarray(prior_weight, dtype=np.float64)
+    if w.shape not in ((2,), (n_kf, 2)) or pw.shape not in ((), (n_kf,)):
+        raise ValueError("%s: weight is (ground, surf) or one pair per keyframe, prior_weight one value or one per keyframe; got %s and %s for %d "
+                         "keyframes" % (fn, w.shape, pw.shape, n_kf))
+    w, pw = np.broadcast_to(w, (n_kf, 2)), np.broadcast_to(pw, (n_kf,))
+    recs = (_capi.MapKeyframe * max(1, n_kf))()
+    keep, strides, seen = [], set(), []
+    api, prm = ground.api, None
+    for k, (key, map_keys, map_pose, pose, gp, sp) in enumerate(keyframes):
+        key, map_keys = int(key), [int(x) for x in map_keys]
+        if len(map_keys) > 3:
+            raise ValueError("%s: keyframe %d has %d map keys (at most 3)" % (fn, k, len(map_keys)))
+        if key in seen:
+            raise ValueError("%s: key %d is listed twice" % (fn, key))
+        if key in map_keys:
+            raise ValueError("%s: key %d is its own map key" % (fn, key))
+        mp, p = _f64(map_pose).reshape(-1), _f64(pose).reshape(-1)
+        if mp.size != 7 or p.size != 7:
+            raise ValueError("%s: keyframe %d: map_pose and pose are 7 doubles [qx qy qz qw tx ty tz]" % (fn, k))
+        api, pts, vp, n, stride, prm = _keyframe_args(fn, ground, surf, gp, sp, w[k], pw[k], huber_a, dist_thr, options, kw)
+        strides.add(stride)
+        seen.append(key)
+        keep.append(pts)
+        r = recs[k]
+        r.key, r.n_map_keys = key, len(map_keys)
+        for i, x in enumerate(map_keys):
+            r.map_keys[i] = x
+        r.n_ground, r.n_surf, r.ground_pts, r.surf_pts = n[0], n[1], vp[0], vp[1]
+        for i in range(7):
+            r.map_pose[i], r.pose[i] = float(mp[i]), float(p[i])
+        r.weight[0], r.weight[1], r.prior_weight = float(w[k][0]), float(w[k][1]), float(pw[k])
+    if len(strides) > 1:
+        raise ValueError("%s: every cloud must have the same record stride, got %s" % (fn, sorted(strides)))
+    if prm is None:
+        _, _, _, _, _, prm = _keyframe_args(fn, ground, surf, np.zeros((0, 4), np.float32), np.zeros((0, 4), np.float32), (1.0, 1.0),
+                                            -1.0, huber_a, dist_thr, options, kw)
+    cs = np.asarray(cell_sizes, dtype=np.float32).reshape(2).copy()
+    api.check(api.icp_map_optimize_keyframes(ground.h, surf.h, recs, len(keyframes), cs.ctypes.data_as(_capi.c_float_p), float(ground_threshold),
+                                             strides.pop() if strides else 16, C.byref(prm)), "icp_map_optimize_keyframes")
+    return [(np.array(r.pose[:]), np.array(r.transform[:]), np.array(r.rpyxyz[:]), (r.summary[0], r.summary[1]),
+             (int(r.n_map_points[0]), int(r.n_map_points[1]))) for r in recs[:len(keyframes)]]
+
+
 def relocate(ground, surf, keys, cell_sizes, ground_threshold, map_pose, old_pose, relative_guess, ground_points, surf_points,
              weight, huber_a, dist_thr, rounds=4, options=None, **kw):
     """Mapping::Relocate for one loop-closure candidate (mapping.cpp:78-112, 251-300) in one device call with one host

@@ -19,6 +19,7 @@
 #include <stdlib.h>
 #include <string.h>
 #include <unordered_map>
+#include <unordered_set>
 #include <vector>
 #include "lvb_internal.cuh"
 #include "lvb_math.cuh"
@@ -352,10 +353,20 @@ __global__ void __launch_bounds__(ITPB) icp_associate_kernel(IcpDev d) {
     d.nrm[i] = n.x; d.nrm[d.K + i] = n.y; d.nrm[2 * (size_t)d.K + i] = n.z;
 }
 
+// What a map frame's grid may use: voxels, coarse blocks and query-sort counters.  kGridLimits is what every map frame gets whose
+// buffers are sized from exact boxes (2^26 voxels, coarse blocks unbounded, 8 M counters); lvb_icp_map_optimize_keyframes passes the
+// capacities it allocated for a map frame whose box the host could only estimate.
+struct GridCap { double cells, coarse, qsort; };
+__device__ __forceinline__ bool grid_fits(double dx, double dy, double dz, const GridCap& cap) {
+    const double cb = __dmul_rn(__dmul_rn(floor(__dmul_rn(__dadd_rn(dx, 3.0), 0.25)), floor(__dmul_rn(__dadd_rn(dy, 3.0), 0.25))),
+                                floor(__dmul_rn(__dadd_rn(dz, 3.0), 0.25)));
+    return __dmul_rn(__dmul_rn(dx, dy), dz) <= cap.cells && cb <= cap.coarse;
+}
+
 // The voxel grid of a map frame and the key granularity of its queries' visiting order, on one thread, from the bounding box in
 // m->bbox.  Every float / double operation is rounded on its own (no contraction), so the grid does not depend on how this file is
 // compiled.  An empty or failed map frame gets a one-voxel grid and P = 0, which every kernel treats as "nothing to do".
-__global__ void icp_map_grid_kernel(MapDesc* m, float cell_size) {
+__global__ void icp_map_grid_kernel(MapDesc* m, float cell_size, GridCap cap) {
     Grid g;
     int P = m->P, err = 0;
     double dx = 1, dy = 1, dz = 1;
@@ -368,16 +379,16 @@ __global__ void icp_map_grid_kernel(MapDesc* m, float cell_size) {
         else {
             // The voxel edge is (radius * 1.0001) / ring: the hair of slack guarantees that float rounding of the voxel coordinate
             // never separates two points closer than the radius by more than `ring` voxels.  ring = 4 unless the bounding box would
-            // need more than MAX_CELLS voxels.
+            // need more voxels (or coarse blocks) than `cap` allows; every ring finds the same exact 3-NN.
             int ring = 4;
             for (;; ring >>= 1) {
                 g.cell = __fdiv_rn(__fmul_rn(cell_size, 1.0001f), (float)ring); g.inv_cell = __fdiv_rn(1.0f, g.cell);
                 dx = __dadd_rn(floor(__dmul_rn((double)wx, (double)g.inv_cell)), 1.0);
                 dy = __dadd_rn(floor(__dmul_rn((double)wy, (double)g.inv_cell)), 1.0);
                 dz = __dadd_rn(floor(__dmul_rn((double)wz, (double)g.inv_cell)), 1.0);
-                if (__dmul_rn(__dmul_rn(dx, dy), dz) <= (double)MAX_CELLS || ring == 1) break;
+                if (grid_fits(dx, dy, dz, cap) || ring == 1) break;
             }
-            if (__dmul_rn(__dmul_rn(dx, dy), dz) > (double)MAX_CELLS) err = 2;
+            if (!grid_fits(dx, dy, dz, cap)) err = 2;
             g.ring = ring;
         }
     }
@@ -392,9 +403,9 @@ __global__ void icp_map_grid_kernel(MapDesc* m, float cell_size) {
     m->ncb = g.cbx * g.cby * g.cbz;
     // key granularity of the query visiting order: blocks of 2 x 2 x 2 voxels (measured on configs[2], association kernel: 4 x 4 x 4
     // blocks 0.51 ms, 2 x 2 x 2 0.44 ms, single voxels 0.50 ms plus a slower sort) -- coarser only when the grid would need more
-    // than 8 M counters
+    // than cap.qsort (8 M) counters
     int shift = 1;
-    while (__dmul_rn(__dmul_rn((double)((g.gx >> shift) + 1), (double)((g.gy >> shift) + 1)), (double)((g.gz >> shift) + 1)) > 8.0e6) ++shift;
+    while (__dmul_rn(__dmul_rn((double)((g.gx >> shift) + 1), (double)((g.gy >> shift) + 1)), (double)((g.gz >> shift) + 1)) > cap.qsort) ++shift;
     const int rnd = (1 << shift) - 1;
     m->shift = shift;
     m->cgx = (g.gx + rnd) >> shift; m->cgy = (g.gy + rnd) >> shift; m->cgz = (g.gz + rnd) >> shift;
@@ -639,12 +650,37 @@ __device__ __forceinline__ void kf_seed(KfBlock* b, int seed, const KfSeed& p) {
     for (int k = 0; k < 3; ++k) { s.x[k] = b->rpyxyz[c_free[seed][k]]; s.cand[k] = s.x[k]; s.prior_target[k] = s.x[k]; }
     s.prior_w = p.prior_w; s.huber_a = p.huber_a[seed]; s.weight = p.weight[seed];
 }
+// lvb_icp_map_optimize_keyframes: what ties keyframe k of the call to the earlier ones.  The blocks and links of a call lie in two
+// arrays, link k beside block k.
+struct KfLink {
+    double T[7];                 // new_k * old_k^-1 (mapping.cpp:181-182), rewritten by every pose kernel of keyframe k
+    double old[7];               // old_k: the incoming pose after the earlier keyframes' ForwardUpdates
+    MapDesc kept[2];             // the map frame the keyframe's build slot holds after icp_map_keep_kernel
+    int k;                       // the keyframe's index in the call
+    int map_from;                // the keyframe of the call whose optimised pose is the map pose (the newest map key), or -1
+};
+// Before keyframe k's registrations: PoseGraph::ForwardUpdate(T_j, t_j + epsilon) of every earlier keyframe j, in order
+// (pose_graph.cpp:245-252: pose = T_j * pose), and the map pose of an in-call newest map key
+__device__ void kf_chain_in(KfBlock* b, KfLink* l) {
+    const KfLink* l0 = l - l->k;
+    for (int j = 0; j < l->k; ++j) {
+        double t[7];
+        kf_se3_mul(l0[j].T, b->pose, t);
+        for (int i = 0; i < 7; ++i) b->pose[i] = t[i];
+    }
+    if (l->map_from >= 0) { const KfBlock* src = b - (l->k - l->map_from); for (int i = 0; i < 7; ++i) b->map_pose[i] = src->pose[i]; }
+    for (int i = 0; i < 7; ++i) l->old[i] = b->pose[i];
+}
+
 // A registration whose map frame is empty (map[m].P == 0: SegmentGround kept no point in the in-call build) is not solved -- its LM
 // passes return at once -- and leaves rpyxyz and the pose as they were, as BuildMapFrame's failure on that side does in the
-// step-by-step path.
-__global__ void icp_kf_pose_kernel(KfBlock* b, int from, int seed, KfSeed p) {
+// step-by-step path.  link (lvb_icp_map_optimize_keyframes only): the incoming pose is chained before the first step, and the
+// keyframe's transform is formed after each.
+__global__ void icp_kf_pose_kernel(KfBlock* b, int from, int seed, KfSeed p, KfLink* link) {
+    if (link && from < 0) kf_chain_in(b, link);
     if (from < 0 || b->map[from].P > 0) kf_pose_update(b, from);
     for (int k = 0; k < 7; ++k) b->tf[k] = __double2float_rn(b->pose[k]);
+    if (link) { double inv[7]; kf_se3_inv(link->old, inv); kf_se3_mul(b->pose, inv, link->T); }
     if (seed < 0) return;
     kf_seed(b, seed, p);
     if (b->map[seed].P == 0) b->st[seed].lm.done = 1;
@@ -666,6 +702,22 @@ __global__ void icp_reloc_pose_kernel(KfBlock* b, int stage) {
                           ? ds(fmin(__ddiv_rn(n, 10.0), m ? 30.0 : 20.0), __ddiv_rn(dm(2.0, b->st[m].lm.x_cost), n))
                           : __longlong_as_double(0x7ff8000000000000LL);
     }
+}
+
+// lvb_icp_map_optimize_keyframes builds the map frames of one side into two slots in turn.  After a build into `dst` whose map frame
+// came out empty (SegmentGround kept no point, or it failed), the slot takes over the previous build's map frame from `src` (whose
+// descriptor is *prev), so that every slot holds the newest map frame with points: the one the step-by-step loop leaves the handle
+// with, as a failed lvb_icp_map_build keeps the map frame before it.  *kept: the descriptor of what dst holds afterwards.
+__global__ void icp_map_keep_kernel(const MapDesc* built, const MapDesc* prev, MapDesc* kept, const float4* src_sorted, const int* src_start,
+                                    const int* src_coarse, float4* dst_sorted, int* dst_start, int* dst_coarse) {
+    const bool take = built->P == 0 && prev->P > 0;
+    if (blockIdx.x == 0 && threadIdx.x == 0) *kept = take ? *prev : *built;
+    if (!take) return;
+    const int P = prev->P, nc = prev->ncell + 1, nb = prev->ncb;
+    const int t0 = blockIdx.x * blockDim.x + threadIdx.x, step = gridDim.x * blockDim.x;
+    for (int i = t0; i < P; i += step) dst_sorted[i] = src_sorted[i];
+    for (int i = t0; i < nc; i += step) dst_start[i] = src_start[i];
+    for (int i = t0; i < nb; i += step) dst_coarse[i] = src_coarse[i];
 }
 
 }  // namespace
@@ -702,6 +754,7 @@ struct lvb_icp {
     struct MapBufs { DevBuf<float4> sorted; DevBuf<int> cell_start, coarse; };      // a map frame's sorted cloud and voxel hash
     MapBufs nx;          // every build writes its map frame here; it is swapped in only when the build succeeded
     MapBufs reloc;       // lvb_icp_map_relocate's old map frame: reused by every relocation, never swapped in
+    MapBufs chain;       // lvb_icp_map_optimize_keyframes builds its map frames into nx and this slot in turn
     int scan_n = 0, scan_stride = 0;          // the scan of the last upload_scan (reusable by lvb_icp_map_append)
     const unsigned char* scan_dev = nullptr;  // where that scan lies: scan_raw, or this handle's part of kf_arena
     // the keyframe calls' upload: [KfBlock | ground scan | surf scan] in one allocation, held by both handles of the call
@@ -735,6 +788,7 @@ static MapDesc desc_seed(int P) {
     bbox_seed(m.bbox);
     return m;
 }
+static const GridCap kGridLimits = {(double)MAX_CELLS, (double)INFINITY, 8.0e6};
 // the failure icp_map_grid_kernel reported in a map frame's descriptor
 static int grid_error(const MapDesc& m, const char* fn, const char* side) {
     if (m.err == 1) { set_error("%s: map cloud has no finite bounding box", fn); return LVB_ERR_INVALID; }
@@ -850,7 +904,7 @@ static int build_map(lvb_icp* h, const unsigned char* d_points, int n, int strid
     cudaStream_t s = ctx->stream;
     MapDesc* md = &h->frame.p->map;
     ILAUNCH(h, icp_bbox_kernel, std::min(1024, inblk(n, 256)), 256, d_points, stride, md);
-    ILAUNCH(h, icp_map_grid_kernel, 1, 1, md, cell_size);
+    ILAUNCH(h, icp_map_grid_kernel, 1, 1, md, cell_size, kGridLimits);
     LVB_TRY(icheck("map grid"));
     MapDesc m;
     LVB_CUDA(cudaMemcpyAsync(&m, md, sizeof(m), cudaMemcpyDeviceToHost, s));
@@ -1095,6 +1149,7 @@ struct KfUpload {
     KfBlock* blk;                                     // its KfBlock (device)
     KfBlock* hb;                                      // the pinned staging area: the upload, then the read-back
     size_t off[2];                                    // where the scans lie in the arena
+    KfLink* link = nullptr;                           // its KfLink (device; lvb_icp_map_optimize_keyframes only)
 };
 
 // One copy from the pinned staging area: the poses (with `reloc`, lvb_icp_map_relocate's old_pose and relative guess), the two map
@@ -1139,7 +1194,7 @@ static int kf_register(lvb_icp* const hs[2], const bool run[2], const KfMap maps
     seed.o = p->options; seed.prior_w = p->prior_weight;
     for (int m = 0; m < 2; ++m) { seed.weight[m] = p->weight[m]; seed.huber_a[m] = p->huber_a[m]; }
     const int first = run[0] ? 0 : (run[1] ? 1 : -1);
-    ILAUNCH(hs[0] ? hs[0] : hs[1], icp_kf_pose_kernel, 1, 1, u.blk, -1, first, seed);      // rpyxyz from the incoming pose (:154)
+    ILAUNCH(hs[0] ? hs[0] : hs[1], icp_kf_pose_kernel, 1, 1, u.blk, -1, first, seed, u.link);      // rpyxyz from the incoming pose (:154)
     for (int m = 0; m < 2; ++m) {
         if (!run[m]) continue;
         lvb_icp* h = hs[m];
@@ -1153,7 +1208,7 @@ static int kf_register(lvb_icp* const hs[2], const bool run[2], const KfMap maps
         ILAUNCH(h, icp_associate_kernel, inblk(ns[m], ITPB), ITPB, d);
         for (int pass = 0; pass <= p->options.max_num_iterations; ++pass) LVB_TRY(enqueue_pass(h, d));
         // pose = map_pose * rpyxyz2se3(rpyxyz) (:165, :177); after the ground solve it also seeds the surf registration
-        ILAUNCH(h, icp_kf_pose_kernel, 1, 1, u.blk, m, m == 0 && run[1] ? 1 : -1, seed);
+        ILAUNCH(h, icp_kf_pose_kernel, 1, 1, u.blk, m, m == 0 && run[1] ? 1 : -1, seed, u.link);
     }
     return LVB_OK;
 }
@@ -1273,7 +1328,8 @@ static int fill_bboxes(lvb_icp* h, const std::vector<lvb_icp::Segment*>& segs) {
 
 // Capacities of a map frame whose cloud lies inside the box lo..hi: icp_map_grid_kernel's ring-4 grid of the box (the voxel counts per
 // axis only shrink with a smaller box or a coarser ring), capped at MAX_CELLS -- above it the device picks a coarser ring or fails.
-struct MapBound { size_t cells, coarse, qsort; bool finite; };
+// qcap: the most query-sort counters the grid kernel picks for a grid no larger than the box's at ring 4 (it bounds qsort)
+struct MapBound { size_t cells, coarse, qsort, qcap; bool finite; };
 static MapBound map_bound(const float* lo, const float* hi, float cell_size) {
     MapBound b;
     const float cell = cell_size * 1.0001f / 4.0f, inv = 1.0f / cell;
@@ -1284,11 +1340,12 @@ static MapBound map_bound(const float* lo, const float* hi, float cell_size) {
         if (!(hi[a] >= lo[a]) || !std::isfinite(w)) { b.finite = false; d[a] = 0; } else d[a] = std::floor((double)w * inv) + 1;
     }
     const double cap = (double)MAX_CELLS;
-    if (!b.finite) { b.cells = b.coarse = MAX_CELLS; b.qsort = 8000000; return b; }
+    if (!b.finite) { b.cells = b.coarse = MAX_CELLS; b.qsort = b.qcap = 8000000; return b; }
     auto blocks = [&](int sh) { double v = 1; for (int a = 0; a < 3; ++a) v *= std::ceil(d[a] / (double)(1 << sh)); return v; };
     b.cells = (size_t)std::min(cap, d[0] * d[1] * d[2]);
     b.coarse = (size_t)std::min(cap, blocks(2));
     b.qsort = (size_t)std::min(8.0e6, blocks(1));          // the grid kernel keeps the sort grid at <= 8 M counters
+    b.qcap = (size_t)std::min(8.0e6, (std::floor(d[0] / 2) + 1) * (std::floor(d[1] / 2) + 1) * (std::floor(d[2] / 2) + 1));
     return b;
 }
 
@@ -1296,7 +1353,9 @@ static MapBound map_bound(const float* lo, const float* hi, float cell_size) {
 // merge order, the merged sizes, which side is built (an empty merged cloud: BuildMapFrame fails on that side and nothing registers,
 // :155,167), the descriptor seeds and the capacity bounds of the builds.  The missing bounding boxes of both handles are computed here,
 // with one synchronisation.
-struct KfPlan { std::vector<lvb_icp::Segment*> pick[2]; size_t total[2] = {0, 0}; bool build[2]; MapBound bound[2]; MapDesc seed[2]; };
+// cap: the limits the grid kernel keeps to (kGridLimits when the bounds come from exact boxes)
+struct KfPlan { std::vector<lvb_icp::Segment*> pick[2]; size_t total[2] = {0, 0}; bool build[2]; MapBound bound[2]; MapDesc seed[2];
+                GridCap cap[2] = {kGridLimits, kGridLimits}; };
 static int kf_plan(lvb_icp* const hs[2], const long long* keys, int n_keys, const float cell_size[2], bool ransac, const char* fn, KfPlan& pl) {
     for (int k = 0; k < n_keys; ++k) {
         for (int m = 0; m < 2; ++m) {
@@ -1349,7 +1408,7 @@ static int kf_build(lvb_icp* const hs[2], const KfPlan& pl, const float cell_siz
         }
         const unsigned char* cp = reinterpret_cast<const unsigned char*>(cloud);
         ILAUNCH(h, icp_bbox_kernel, std::min(1024, inblk(n, 256)), 256, cp, 16, md);
-        ILAUNCH(h, icp_map_grid_kernel, 1, 1, md, cell_size[m]);
+        ILAUNCH(h, icp_map_grid_kernel, 1, 1, md, cell_size[m], pl.cap[m]);
         LVB_TRY(enqueue_hash(h, cp, n, 16, md, pl.bound[m].cells, pl.bound[m].coarse, false, out));
         maps[m] = {out.sorted.p, out.cell_start.p, out.coarse.p, cell_size[m], pl.bound[m].qsort, false};
     }
@@ -1447,6 +1506,297 @@ int lvb_icp_map_build_optimize_keyframe(lvb_icp* ground, lvb_icp* surf, const lo
         }
     }
     memcpy(pose, u.hb->pose, sizeof(u.hb->pose)); memcpy(rpyxyz, u.hb->rpyxyz, sizeof(u.hb->rpyxyz));
+    return LVB_OK;
+}
+
+// ---- Mapping::Optimize(active_kfs) (mapping.cpp:139-191) for every lidar keyframe of a backend pass in one call
+// (lvb_icp_map_optimize_keyframes).  Keyframe k's map frame may merge the clouds earlier keyframes of the call store: their poses are
+// decided on the device, so the host sizes that map frame from an estimate of their boxes -- the robot-frame box moved by the incoming
+// pose the caller gave, widened by kInCallMargin -- and passes the capacity it allocated to the grid kernel as a limit.  A cloud that
+// ends up outside its estimate makes the kernel take a coarser ring (each ring is exact); only a grid that does not fit at ring 1
+// fails.
+static const float kInCallMargin = 1.0f;        // metres on every side
+static void in_call_box(const void* pts, int n, int stride, const double* pose, float lo[3], float hi[3]) {
+    // compare-and-select: a NaN coordinate never wins; an infinite one leaves the box infinite (the device reports that cloud)
+    float l0 = FLT_MAX, l1 = FLT_MAX, l2 = FLT_MAX, h0 = -FLT_MAX, h1 = -FLT_MAX, h2 = -FLT_MAX;
+    const unsigned char* base = static_cast<const unsigned char*>(pts);
+    for (int i = 0; i < n; ++i) {
+        const float* f = reinterpret_cast<const float*>(base + (size_t)i * stride);
+        l0 = f[0] < l0 ? f[0] : l0; l1 = f[1] < l1 ? f[1] : l1; l2 = f[2] < l2 ? f[2] : l2;
+        h0 = f[0] > h0 ? f[0] : h0; h1 = f[1] > h1 ? f[1] : h1; h2 = f[2] > h2 ? f[2] : h2;
+    }
+    const double mn[3] = {l0, l1, l2}, mx[3] = {h0, h1, h2};
+    double wl[3], wh[3];
+    bool finite = true;
+    for (int a = 0; a < 3; ++a) finite = finite && mn[a] <= mx[a] && std::isfinite(mn[a]) && std::isfinite(mx[a]) && mn[a] > -FLT_MAX && mx[a] < FLT_MAX;
+    if (!finite) {                             // no point, or an infinite one: the keyframe's position
+        for (int a = 0; a < 3; ++a) wl[a] = wh[a] = pose[4 + a];
+    } else {                                   // the world box of the robot-frame box's corners
+        const double qn = std::sqrt(pose[0] * pose[0] + pose[1] * pose[1] + pose[2] * pose[2] + pose[3] * pose[3]);
+        const double x = pose[0] / qn, y = pose[1] / qn, z = pose[2] / qn, w = pose[3] / qn;
+        const double R[9] = {1 - 2 * (y * y + z * z), 2 * (x * y - z * w), 2 * (x * z + y * w),
+                             2 * (x * y + z * w), 1 - 2 * (x * x + z * z), 2 * (y * z - x * w),
+                             2 * (x * z - y * w), 2 * (y * z + x * w), 1 - 2 * (x * x + y * y)};
+        for (int a = 0; a < 3; ++a) { wl[a] = INFINITY; wh[a] = -INFINITY; }
+        for (int c = 0; c < 8; ++c) {
+            const double p[3] = {c & 1 ? mx[0] : mn[0], c & 2 ? mx[1] : mn[1], c & 4 ? mx[2] : mn[2]};
+            for (int a = 0; a < 3; ++a) {
+                const double v = R[3 * a] * p[0] + R[3 * a + 1] * p[1] + R[3 * a + 2] * p[2] + pose[4 + a];
+                wl[a] = std::min(wl[a], v); wh[a] = std::max(wh[a], v);
+            }
+        }
+    }
+    for (int a = 0; a < 3; ++a) {
+        lo[a] = std::nextafter((float)(wl[a] - kInCallMargin), -INFINITY);
+        hi[a] = std::nextafter((float)(wh[a] + kInCallMargin), INFINITY);
+    }
+}
+
+// the call's parameters with keyframe kf's own weights and prior weight (ScanToMapWith* read them from each frame)
+static lvb_map_optimize_params kf_params(const lvb_map_optimize_params& p, const lvb_map_keyframe& kf) {
+    lvb_map_optimize_params q = p;
+    q.weight[0] = kf.weight[0]; q.weight[1] = kf.weight[1]; q.prior_weight = kf.prior_weight;
+    return q;
+}
+
+// One call for a chain of keyframes, entirely on the device: per keyframe the incoming pose chained through the earlier keyframes'
+// transforms, the map frame (resident clouds and clouds of earlier keyframes) built into one of two slots per side, both registrations,
+// the transform and ToWorld into staged clouds.  One pinned upload, one read-back, one host synchronisation; the staged clouds and the
+// map frames are committed only when every keyframe succeeded.
+int lvb_icp_map_optimize_keyframes(lvb_icp* ground, lvb_icp* surf, lvb_map_keyframe* kfs, int n_kf, const float cell_size[2],
+                                   double ground_threshold, int stride, const lvb_map_optimize_params* p) {
+    static const char* fn = "lvb_icp_map_optimize_keyframes";
+    lvb_icp* hs[2] = {ground, surf};
+    if (!ground || !surf || ground == surf || !cell_size || !p || n_kf < 0 || (n_kf > 0 && !kfs)) { set_error("%s: null or bad argument", fn); return LVB_ERR_INVALID; }
+    {
+        const void* none[2] = {nullptr, nullptr};
+        const int zero[2] = {0, 0};
+        LVB_TRY(kf_check_args(hs, cell_size, none, zero, stride, p, fn));
+    }
+    std::unordered_map<long long, int> batch;
+    for (int k = 0; k < n_kf; ++k) {
+        const lvb_map_keyframe& kf = kfs[k];
+        const void* pts[2] = {kf.ground_pts, kf.surf_pts};
+        const int ns[2] = {kf.n_ground, kf.n_surf};
+        LVB_TRY(kf_check_args(hs, cell_size, pts, ns, stride, p, fn));
+        if (kf.n_map_keys < 0 || kf.n_map_keys > 3) { set_error("%s: keyframe %d has %d map keys (0 to 3)", fn, k, kf.n_map_keys); return LVB_ERR_INVALID; }
+        if (!batch.emplace(kf.key, k).second) { set_error("%s: key %lld is listed twice", fn, kf.key); return LVB_ERR_INVALID; }
+    }
+    // each map key: the cloud an earlier keyframe of the call stores (kf >= 0), else the resident one of both handles
+    struct Src { int kf; lvb_icp::Segment* seg[2]; };
+    std::vector<std::vector<Src>> srcs(n_kf);
+    for (int k = 0; k < n_kf; ++k) {
+        for (int i = 0; i < kfs[k].n_map_keys; ++i) {
+            const long long mk = kfs[k].map_keys[i];
+            if (mk == kfs[k].key) { set_error("%s: key %lld is its own map key", fn, mk); return LVB_ERR_INVALID; }
+            Src sr = {-1, {nullptr, nullptr}};
+            const auto it = batch.find(mk);
+            if (it != batch.end() && it->second < k) sr.kf = it->second;
+            else {
+                for (int m = 0; m < 2; ++m) for (auto& sg : hs[m]->segments) if (sg.key == mk) sr.seg[m] = &sg;
+                if (!sr.seg[0] || !sr.seg[1]) {
+                    set_error("%s: map key %lld of keyframe %d is neither resident nor an earlier keyframe of the call", fn, mk, k); return LVB_ERR_INVALID; }
+            }
+            srcs[k].push_back(sr);
+        }
+    }
+    if (n_kf == 0) return LVB_OK;
+    lvb_ctx* ctx = ground->ctx;
+    LVB_CUDA(cudaSetDevice(ctx->device)); lvb::g_alloc_stream = ctx->stream;
+    {   // the missing boxes of the resident clouds, with one synchronisation
+        std::vector<lvb_icp::Segment*> res;
+        std::unordered_set<lvb_icp::Segment*> seen;
+        for (auto& v : srcs) for (auto& sr : v) if (sr.kf < 0) for (int m = 0; m < 2; ++m) if (seen.insert(sr.seg[m]).second) res.push_back(sr.seg[m]);
+        LVB_TRY(fill_bboxes(ground, res));
+    }
+    const bool ransac = ground_threshold > 0.0;
+    auto n_of = [&](int k, int m) { return m ? kfs[k].n_surf : kfs[k].n_ground; };
+    std::vector<lvb_icp::Segment> stage(2 * (size_t)n_kf);          // [2 k + m]: the clouds ToWorld stores for keyframe k
+    // what is known before any launch: merge lists, sizes, which sides are built and into which slot (nx first, then in turn), the
+    // union of the resident clouds' boxes.  The estimated boxes of the call's own clouds, and with them the bounds of the map frames
+    // that merge them, are formed just before each keyframe is enqueued, while the device runs the keyframes before it.
+    std::vector<KfPlan> pl(n_kf);
+    std::vector<int> map_from(n_kf, -1), slot(2 * (size_t)n_kf, -1);
+    std::vector<float> box(12 * (size_t)n_kf);                      // [12 k + 6 m]: lo, hi of the resident clouds in keyframe k's map frame
+    int turn[2] = {-1, -1};
+    for (int k = 0; k < n_kf; ++k) {
+        for (int m = 0; m < 2; ++m) {
+            float* lo = &box[12 * (size_t)k + 6 * m];
+            float* hi = lo + 3;
+            for (int a = 0; a < 3; ++a) { lo[a] = FLT_MAX; hi[a] = -FLT_MAX; }
+            bool resident = false;
+            for (auto& sr : srcs[k]) {
+                if (sr.kf >= 0) { pl[k].pick[m].push_back(&stage[2 * (size_t)sr.kf + m]); pl[k].total[m] += n_of(sr.kf, m); continue; }
+                pl[k].pick[m].push_back(sr.seg[m]); pl[k].total[m] += sr.seg[m]->n;
+                for (int a = 0; a < 3; ++a) { lo[a] = std::min(lo[a], sr.seg[m]->lo[a]); hi[a] = std::max(hi[a], sr.seg[m]->hi[a]); }
+                resident = true;
+            }
+            if (pl[k].total[m] > 0x7fffffffull) { set_error("%s: map frame of more than 2^31 points", fn); return LVB_ERR_INVALID; }
+            pl[k].build[m] = pl[k].total[m] > 0;
+            pl[k].seed[m] = desc_seed(pl[k].build[m] && !(m == 0 && ransac) ? (int)pl[k].total[m] : 0);
+            if (!pl[k].build[m]) continue;
+            turn[m] = turn[m] < 0 ? 0 : 1 - turn[m];
+            slot[2 * k + m] = turn[m];
+            // the estimates of the call's clouds are finite: only the resident ones can make the box infinite here
+            if (resident && !map_bound(lo, hi, cell_size[m]).finite && !(m == 0 && ransac)) { set_error("%s: map cloud has no finite bounding box", fn); return LVB_ERR_INVALID; }
+        }
+        if (!srcs[k].empty() && srcs[k].back().kf >= 0) map_from[k] = srcs[k].back().kf;
+    }
+    std::vector<float> est(12 * (size_t)n_kf);                      // [12 k + 6 m]: the estimated box of keyframe k's stored cloud
+    std::vector<char> have_est(2 * (size_t)n_kf, 0);
+    // keyframe k's bounds (kf_plan's, with the estimates of its in-call clouds) and the grid limits that follow from them
+    auto plan_bounds = [&](int k) {
+        bool in_call = false;
+        for (int m = 0; m < 2; ++m) {
+            if (!pl[k].build[m]) continue;
+            float lo[3], hi[3];
+            for (int a = 0; a < 3; ++a) { lo[a] = box[12 * (size_t)k + 6 * m + a]; hi[a] = box[12 * (size_t)k + 6 * m + 3 + a]; }
+            for (auto& sr : srcs[k]) {
+                if (sr.kf < 0) continue;
+                const size_t e = 2 * (size_t)sr.kf + m;
+                if (!have_est[e]) {
+                    in_call_box(m ? kfs[sr.kf].surf_pts : kfs[sr.kf].ground_pts, n_of(sr.kf, m), stride, kfs[sr.kf].pose, &est[6 * e], &est[6 * e + 3]);
+                    have_est[e] = 1;
+                }
+                for (int a = 0; a < 3; ++a) { lo[a] = std::min(lo[a], est[6 * e + a]); hi[a] = std::max(hi[a], est[6 * e + 3 + a]); }
+                in_call = true;
+            }
+            pl[k].bound[m] = map_bound(lo, hi, cell_size[m]);
+        }
+        for (int m = 0; m < 2 && in_call; ++m) {
+            if (!pl[k].build[m]) continue;
+            MapBound& b = pl[k].bound[m];
+            b.qsort = b.qcap;
+            pl[k].cap[m] = {(double)b.cells, (double)b.coarse, (double)b.qcap};
+        }
+    };
+
+    const auto t0 = std::chrono::steady_clock::now();
+    cudaStream_t s = ctx->stream;
+    lvb::timing_mark(s, "begin");
+    // one pinned upload: [KfBlock x n_kf | KfLink x n_kf | ground and surf scan of each keyframe]
+    const size_t blk_bytes = ((size_t)n_kf * sizeof(KfBlock) + 255) & ~(size_t)255;
+    const size_t back_bytes = blk_bytes + (size_t)n_kf * sizeof(KfLink);
+    std::vector<size_t> off(2 * (size_t)n_kf);
+    size_t all = (back_bytes + 255) & ~(size_t)255;
+    for (int k = 0; k < n_kf; ++k)
+        for (int m = 0; m < 2; ++m) { off[2 * k + m] = all; all = (all + (size_t)n_of(k, m) * stride + 255) & ~(size_t)255; }
+    LVB_TRY(lvb::stage_wait(ctx));
+    LVB_TRY(lvb::stage_grow(ctx, all, 0));
+    KfBlock* hb = reinterpret_cast<KfBlock*>(ctx->stage_h);
+    KfLink* hl = reinterpret_cast<KfLink*>(ctx->stage_h + blk_bytes);
+    memset(hb, 0, (size_t)n_kf * sizeof(KfBlock));
+    memset(hl, 0, (size_t)n_kf * sizeof(KfLink));
+    for (int k = 0; k < n_kf; ++k) {
+        memcpy(hb[k].map_pose, kfs[k].map_pose, sizeof(hb[k].map_pose)); memcpy(hb[k].pose, kfs[k].pose, sizeof(hb[k].pose));
+        hl[k].k = k; hl[k].map_from = map_from[k];
+        for (int m = 0; m < 2; ++m) {
+            hb[k].map[m] = pl[k].seed[m];
+            bbox_seed(hb[k].out_bbox[m]);
+            const size_t bytes = (size_t)n_of(k, m) * stride;
+            if (bytes) memcpy(ctx->stage_h + off[2 * k + m], m ? kfs[k].surf_pts : kfs[k].ground_pts, bytes);
+        }
+    }
+    auto arena = std::make_shared<DevBuf<unsigned char>>();
+    LVB_TRY(arena->ensure(all));
+    LVB_CUDA(cudaMemcpyAsync(arena->p, ctx->stage_h, all, cudaMemcpyHostToDevice, s));
+    LVB_TRY(lvb::stage_mark_busy(ctx, s));
+    KfBlock* dblk = reinterpret_cast<KfBlock*>(arena->p);
+    KfLink* dlink = reinterpret_cast<KfLink*>(arena->p + blk_bytes);
+
+    ScanState saved[2];
+    for (int m = 0; m < 2; ++m) saved[m].save(hs[m]);
+    int first[2] = {-1, -1}, last[2] = {-1, -1};       // per side: the keyframes of the first and the latest build
+    // the descriptor of what the latest build's slot holds: its own map frame, or (after icp_map_keep_kernel) the one it kept
+    auto kept_desc = [&](const KfBlock* b, const KfLink* l, int m) -> const MapDesc* { return first[m] == last[m] ? &b[last[m]].map[m] : &l[last[m]].kept[m]; };
+    // per side and slot: the sizes the slot's buffers hold at least (a slot may take over the other slot's map frame)
+    size_t held[2][2][3] = {};
+    int rc = LVB_OK;
+    for (int k = 0; k < n_kf && rc == LVB_OK; ++k) {
+        KfUpload u;
+        u.arena = arena; u.blk = dblk + k; u.hb = hb + k; u.off[0] = off[2 * k]; u.off[1] = off[2 * k + 1]; u.link = dlink + k;
+        const int ns[2] = {kfs[k].n_ground, kfs[k].n_surf};
+        const lvb_map_optimize_params pk = kf_params(*p, kfs[k]);
+        KfMap maps[2];
+        plan_bounds(k);
+        for (int m = 0; m < 2 && rc == LVB_OK; ++m) {
+            const int sl = slot[2 * k + m];
+            if (sl < 0) continue;
+            size_t* need = held[m][sl];
+            need[0] = pl[k].total[m]; need[1] = pl[k].bound[m].cells; need[2] = pl[k].bound[m].coarse;
+            if (last[m] >= 0) {
+                for (int i = 0; i < 3; ++i) need[i] = std::max(need[i], held[m][1 - sl][i]);
+                lvb_icp::MapBufs& b = sl ? hs[m]->chain : hs[m]->nx;
+                rc = b.sorted.ensure(need[0]);
+                if (rc == LVB_OK) rc = b.cell_start.ensure(need[1] + 1);
+                if (rc == LVB_OK) rc = b.coarse.ensure(need[2]);
+                if (rc != LVB_OK) break;
+            }
+            KfPlan one = pl[k];
+            one.build[1 - m] = false;
+            rc = kf_build(hs, one, cell_size, ground_threshold, u, sl ? &lvb_icp::chain : &lvb_icp::nx, maps);
+            if (rc == LVB_OK && last[m] >= 0) {
+                lvb_icp* h = hs[m];
+                const lvb_icp::MapBufs& src = sl ? h->nx : h->chain;
+                lvb_icp::MapBufs& dst = sl ? h->chain : h->nx;
+                ILAUNCH(h, icp_map_keep_kernel, 2 * ctx->sm_count, 256, &dblk[k].map[m], kept_desc(dblk, dlink, m), &dlink[k].kept[m],
+                        src.sorted.p, src.cell_start.p, src.coarse.p, dst.sorted.p, dst.cell_start.p, dst.coarse.p);
+            }
+            if (first[m] < 0) first[m] = k;
+            last[m] = k;
+        }
+        if (rc == LVB_OK) rc = kf_register(hs, pl[k].build, maps, u, ns, stride, &pk);
+        if (rc == LVB_OK) rc = kf_to_world(hs, u, ns, stride, true, &stage[2 * (size_t)k]);
+    }
+    if (rc == LVB_OK) rc = icheck(fn);
+    // the one read-back: every keyframe's solver states, poses, map descriptors and stored boxes, and its link (transform, kept frames)
+    if (rc == LVB_OK && cudaMemcpyAsync(hb, dblk, back_bytes, cudaMemcpyDeviceToHost, s) != cudaSuccess) rc = lvb::cuda_fail(cudaGetLastError(), "read-back", __FILE__, __LINE__);
+    if (rc == LVB_OK) rc = host_sync(ctx, s);
+    if (rc == LVB_OK) ctx->stage_busy = false;
+    for (int k = 0; k < n_kf && rc == LVB_OK; ++k) {
+        for (int m = 0; m < 2 && rc == LVB_OK; ++m) {
+            if (!pl[k].build[m]) continue;
+            const MapDesc& md = hb[k].map[m];
+            if (md.err == 2 && pl[k].cap[m].cells < (double)MAX_CELLS) {
+                set_error("%s: the voxel grid of keyframe %d's %s map frame exceeds, at every ring, the capacity sized from the incoming poses", fn, k,
+                          m ? "surf" : "ground");
+                rc = LVB_ERR_UNSUPPORTED;
+            } else rc = grid_error(md, fn, m ? "surf " : "ground ");
+        }
+    }
+    if (rc != LVB_OK) {        // nothing was committed: the resident clouds, the map frames and the scans are as they were
+        for (auto& sg : stage) sg.release();
+        for (int m = 0; m < 2; ++m) saved[m].restore(hs[m]);
+        return rc;
+    }
+    const double el = std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
+    for (int m = 0; m < 2; ++m) {
+        lvb_icp* h = hs[m];
+        if (last[m] >= 0) {    // the newest map frame with points replaces the one before, as the step-by-step loop leaves it
+            const MapDesc& kd = *kept_desc(hb, hl, m);
+            if (kd.P > 0) {
+                lvb_icp::MapBufs& sl = slot[2 * last[m] + m] ? h->chain : h->nx;
+                swap_buf(h->map_sorted, sl.sorted); swap_buf(h->cell_start, sl.cell_start); swap_buf(h->coarse, sl.coarse);
+                h->map = kd; h->cell_size = cell_size[m]; h->have_map = true;
+            }
+        }
+        h->scan_n = n_of(n_kf - 1, m); h->scan_stride = stride; h->scan_dev = arena->p + off[2 * (n_kf - 1) + m]; h->kf_arena = arena;
+    }
+    for (int k = 0; k < n_kf; ++k) {
+        lvb_map_keyframe& kf = kfs[k];
+        for (int m = 0; m < 2; ++m) {
+            lvb_icp::Segment& sg = stage[2 * (size_t)k + m];
+            bbox_store(sg, hb[k].out_bbox[m]);
+            store_segment(hs[m], kf.key, sg);
+            const MapDesc& md = hb[k].map[m];
+            const bool built = pl[k].build[m] && md.P > 0;
+            kf.n_map_points[m] = built ? md.P : 0;
+            if (built) fill_summary(hb[k].st[m], kf.prior_weight, el, &kf.summary[m]);
+            else { memset(&kf.summary[m], 0, sizeof(kf.summary[m])); kf.summary[m].termination_type = -1; }
+        }
+        memcpy(kf.pose, hb[k].pose, sizeof(kf.pose)); memcpy(kf.rpyxyz, hb[k].rpyxyz, sizeof(kf.rpyxyz));
+        memcpy(kf.transform, hl[k].T, sizeof(kf.transform));
+    }
     return LVB_OK;
 }
 
@@ -1583,6 +1933,13 @@ int lvb_icp_map_to_world(lvb_icp* ground, lvb_icp* surf, const long long* keys, 
     LVB_TRY(host_sync(ctx, s));
     ctx->stage_busy = false;
     for (size_t i = 0; i < S; ++i) bbox_store(*segs[i], hbox + 6 * i);
+    return LVB_OK;
+}
+
+int lvb_debug_icp_map_grid(lvb_icp* h, int grid[4]) {
+    if (!h || !grid) { set_error("null argument"); return LVB_ERR_INVALID; }
+    if (!h->have_map) { set_error("no map"); return LVB_ERR_STATE; }
+    grid[0] = h->map.g.ring; grid[1] = h->map.g.gx; grid[2] = h->map.g.gy; grid[3] = h->map.g.gz;
     return LVB_OK;
 }
 
