@@ -270,6 +270,7 @@ LVB_API int lvb_icp_map_optimize_keyframe(lvb_icp* ground, lvb_icp* surf, const 
                                           double rpyxyz[6] /* out */, lvb_solve_summary summary[2]);
 /* Mapping::BuildMapFrame + the body of Mapping::Optimize's loop for one keyframe (mapping.cpp:114-137, 147-185): the two
  * lvb_icp_map_build calls and lvb_icp_map_optimize_keyframe in one call, with one host synchronisation.
+ * It runs as the chain of one: lvb_icp_map_optimize_keyframes' implementation with this keyframe and p's weights and prior weight.
  *   keys / n_keys  the map frame's keyframes in merge order, as for lvb_icp_map_build, resident on both handles; `key` may not be one
  *                  of them.  n_keys == 0 is the first lidar keyframe (BuildMapFrame returns early, :118-119): nothing is registered
  *                  and both clouds are stored at the incoming pose.

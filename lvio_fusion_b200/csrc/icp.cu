@@ -15,6 +15,7 @@
 #include <math.h>
 #include <algorithm>
 #include <chrono>
+#include <functional>
 #include <memory>
 #include <stdlib.h>
 #include <string.h>
@@ -743,8 +744,8 @@ struct lvb_icp {
     DevBuf<int> q_key, q_counts, q_start, q_fill, q_sums, q_total, q_order;
     // device-resident world clouds per keyframe (Mapping::pointclouds_surf / _ground, mapping.cpp:208-219) and the merged map frame
     // robot: the same records in the robot frame (x, y, z, intensity), kept so that lvb_icp_map_to_world can re-anchor the cloud
-    // lo / hi: the cloud's bounding box (icp_bbox_kernel's), recorded by lvb_icp_map_build_optimize_keyframe and lvb_icp_map_to_world
-    // for the clouds they write and computed by the former once for the others (has_bbox false)
+    // lo / hi: the cloud's bounding box (icp_bbox_kernel's), recorded by the calls that build map frames (kf_chain) and by
+    // lvb_icp_map_to_world for the clouds they write, and computed by the former once for the others (has_bbox false)
     struct Segment {
         long long key; DevBuf<float4>* pts = nullptr; DevBuf<float4>* robot = nullptr; int n; bool has_bbox = false; float lo[3], hi[3];
         void release() { delete pts; delete robot; pts = robot = nullptr; }
@@ -757,7 +758,7 @@ struct lvb_icp {
     MapBufs chain;       // lvb_icp_map_optimize_keyframes builds its map frames into nx and this slot in turn
     int scan_n = 0, scan_stride = 0;          // the scan of the last upload_scan (reusable by lvb_icp_map_append)
     const unsigned char* scan_dev = nullptr;  // where that scan lies: scan_raw, or this handle's part of kf_arena
-    // the keyframe calls' upload: [KfBlock | ground scan | surf scan] in one allocation, held by both handles of the call
+    // the keyframe calls' upload (kf_upload: blocks, links, scans) in one allocation, held by both handles of the call
     // so that either one's scan stays valid for lvb_icp_map_append(NULL) until that handle uploads another scan
     std::shared_ptr<DevBuf<unsigned char>> kf_arena;
     ~lvb_icp() { for (auto& sg : segments) sg.release(); }
@@ -1142,41 +1143,54 @@ int lvb_icp_scan_to_map(lvb_icp* h, int mode, const void* scan, int n, int strid
     return LVB_OK;
 }
 
-// ---- Mapping::Optimize for one keyframe on the device: lvb_icp_map_optimize_keyframe against the handles' map frames, and
-// lvb_icp_map_build_optimize_keyframe, which builds them in the same call
-struct KfUpload {
-    std::shared_ptr<DevBuf<unsigned char>> arena;     // [KfBlock | ground scan | surf scan]
+// ---- Mapping::Optimize on the device: lvb_icp_map_optimize_keyframe against the handles' map frames, and the calls that build them
+// in the same call (lvb_icp_map_optimize_keyframes, lvb_icp_map_build_optimize_keyframe, lvb_icp_map_relocate)
+struct KfUpload {                                     // one keyframe's part of its call's upload
+    std::shared_ptr<DevBuf<unsigned char>> arena;     // [KfBlock x n | KfLink x n (lvb_icp_map_optimize_keyframes) | ground, surf scan of each]
     KfBlock* blk;                                     // its KfBlock (device)
-    KfBlock* hb;                                      // the pinned staging area: the upload, then the read-back
-    size_t off[2];                                    // where the scans lie in the arena
-    KfLink* link = nullptr;                           // its KfLink (device; lvb_icp_map_optimize_keyframes only)
+    KfBlock* hb;                                      // its KfBlock in the pinned staging area: the upload, then the read-back
+    size_t off[2];                                    // where its scans lie in the arena
+    KfLink* link = nullptr;                           // its KfLink (device), with links
+    KfLink* hl = nullptr;                             // its KfLink in the staging area
 };
 
-// One copy from the pinned staging area: the poses (with `reloc`, lvb_icp_map_relocate's old_pose and relative guess), the two map
-// frames' descriptors (map[m]), and the scans of the handles given.  The staging area stays busy until the caller's read-back.
-static int kf_upload(lvb_ctx* ctx, lvb_icp* const hs[2], const double* map_pose, const double* pose, const MapDesc map[2],
-                     const void* const pts[2], const int ns[2], int stride, KfUpload& u, const double* const reloc[2] = nullptr) {
-    size_t bytes[2], all = (sizeof(KfBlock) + 255) & ~(size_t)255;
-    for (int m = 0; m < 2; ++m) {
-        bytes[m] = hs[m] ? (size_t)ns[m] * stride : 0;
-        u.off[m] = all; all = (all + bytes[m] + 255) & ~(size_t)255;
-    }
+// One copy from the pinned staging area for n keyframes: the blocks (zero but for the out_bbox seeds and what fill(k, u[k]) writes
+// into keyframe k's: poses, map descriptors), with `links` the links (zero but for fill's), and the scans pts[2 k + m] of ns[2 k + m]
+// records.  u[k]: keyframe k's views; back: the bytes of the blocks and links, which the read-back copies.  The staging area stays
+// busy until the caller's read-back.
+static int kf_upload(lvb_ctx* ctx, int n, bool links, const void* const* pts, const int* ns, int stride, std::vector<KfUpload>& u,
+                     size_t& back, const std::function<void(int, KfUpload&)>& fill) {
+    const size_t blk_bytes = ((size_t)n * sizeof(KfBlock) + 255) & ~(size_t)255;
+    back = blk_bytes + (links ? (size_t)n * sizeof(KfLink) : 0);
+    u.assign(n, KfUpload());
+    size_t all = (back + 255) & ~(size_t)255;
+    for (int k = 0; k < n; ++k)
+        for (int m = 0; m < 2; ++m) { u[k].off[m] = all; all = (all + (size_t)ns[2 * k + m] * stride + 255) & ~(size_t)255; }
     LVB_TRY(lvb::stage_wait(ctx));
     LVB_TRY(lvb::stage_grow(ctx, all, 0));
-    u.hb = reinterpret_cast<KfBlock*>(ctx->stage_h);
-    memset(u.hb, 0, sizeof(KfBlock));
-    memcpy(u.hb->map_pose, map_pose, sizeof(u.hb->map_pose)); memcpy(u.hb->pose, pose, sizeof(u.hb->pose));
-    if (reloc) { memcpy(u.hb->old_pose, reloc[0], sizeof(u.hb->old_pose)); memcpy(u.hb->rel, reloc[1], sizeof(u.hb->rel)); }
-    for (int m = 0; m < 2; ++m) {
-        u.hb->map[m] = map[m];
-        bbox_seed(u.hb->out_bbox[m]);
-        if (bytes[m]) memcpy(ctx->stage_h + u.off[m], pts[m], bytes[m]);
+    KfBlock* hb = reinterpret_cast<KfBlock*>(ctx->stage_h);
+    KfLink* hl = reinterpret_cast<KfLink*>(ctx->stage_h + blk_bytes);
+    memset(hb, 0, (size_t)n * sizeof(KfBlock));
+    if (links) memset(hl, 0, (size_t)n * sizeof(KfLink));
+    for (int k = 0; k < n; ++k) {
+        u[k].hb = hb + k;
+        if (links) u[k].hl = hl + k;
+        for (int m = 0; m < 2; ++m) {
+            bbox_seed(hb[k].out_bbox[m]);
+            const size_t bytes = (size_t)ns[2 * k + m] * stride;
+            if (bytes) memcpy(ctx->stage_h + u[k].off[m], pts[2 * k + m], bytes);
+        }
+        fill(k, u[k]);
     }
-    u.arena = std::make_shared<DevBuf<unsigned char>>();
-    LVB_TRY(u.arena->ensure(all));
-    LVB_CUDA(cudaMemcpyAsync(u.arena->p, ctx->stage_h, all, cudaMemcpyHostToDevice, ctx->stream));
+    auto arena = std::make_shared<DevBuf<unsigned char>>();
+    LVB_TRY(arena->ensure(all));
+    LVB_CUDA(cudaMemcpyAsync(arena->p, ctx->stage_h, all, cudaMemcpyHostToDevice, ctx->stream));
     LVB_TRY(lvb::stage_mark_busy(ctx, ctx->stream));
-    u.blk = reinterpret_cast<KfBlock*>(u.arena->p);
+    for (int k = 0; k < n; ++k) {
+        u[k].arena = arena;
+        u[k].blk = reinterpret_cast<KfBlock*>(arena->p) + k;
+        if (links) u[k].link = reinterpret_cast<KfLink*>(arena->p + blk_bytes) + k;
+    }
     return LVB_OK;
 }
 
@@ -1265,14 +1279,17 @@ int lvb_icp_map_optimize_keyframe(lvb_icp* ground, lvb_icp* surf, const double m
     cudaStream_t s = ctx->stream;
     lvb::timing_mark(s, "begin");
     const bool run[2] = {ground != nullptr, surf != nullptr};
-    MapDesc desc[2];
+    const int up[2] = {ground ? n_ground : 0, surf ? n_surf : 0};          // the scans of the handles given
     KfMap maps[2];
-    for (int m = 0; m < 2; ++m) {
-        desc[m] = hs[m] ? hs[m]->map : desc_seed(0);          // P = 0: no registration on that side
+    for (int m = 0; m < 2; ++m)
         if (hs[m]) maps[m] = {hs[m]->map_sorted.p, hs[m]->cell_start.p, hs[m]->coarse.p, hs[m]->cell_size, (size_t)hs[m]->map.nc, true};
-    }
-    KfUpload u;
-    LVB_TRY(kf_upload(ctx, hs, map_pose, pose, desc, pts, ns, stride, u));
+    std::vector<KfUpload> uk;
+    size_t back;
+    LVB_TRY(kf_upload(ctx, 1, false, pts, up, stride, uk, back, [&](int, KfUpload& v) {
+        memcpy(v.hb->map_pose, map_pose, sizeof(v.hb->map_pose)); memcpy(v.hb->pose, pose, sizeof(v.hb->pose));
+        for (int m = 0; m < 2; ++m) v.hb->map[m] = hs[m] ? hs[m]->map : desc_seed(0);          // P = 0: no registration on that side
+    }));
+    const KfUpload& u = uk[0];
     lvb_icp::Segment fresh[2];
     LVB_TRY(kf_register(hs, run, maps, u, ns, stride, p));
     LVB_TRY(kf_to_world(hs, u, ns, stride, false, fresh));
@@ -1280,7 +1297,7 @@ int lvb_icp_map_optimize_keyframe(lvb_icp* ground, lvb_icp* surf, const double m
     if (rc != LVB_OK) { fresh[0].release(); fresh[1].release(); return rc; }
     for (int m = 0; m < 2; ++m) if (hs[m]) store_segment(hs[m], key, fresh[m]);
     // the one read-back: both solver states, rpyxyz and the pose
-    LVB_CUDA(cudaMemcpyAsync(u.hb, u.blk, sizeof(KfBlock), cudaMemcpyDeviceToHost, s));
+    LVB_CUDA(cudaMemcpyAsync(u.hb, u.blk, back, cudaMemcpyDeviceToHost, s));
     LVB_TRY(host_sync(ctx, s));
     ctx->stage_busy = false;
     const double el = std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
@@ -1295,7 +1312,8 @@ int lvb_icp_map_optimize_keyframe(lvb_icp* ground, lvb_icp* surf, const double m
     return LVB_OK;
 }
 
-// ---- Mapping::BuildMapFrame + Mapping::Optimize for one keyframe in one call (lvb_icp_map_build_optimize_keyframe)
+// ---- Map frames built inside a call: Mapping::BuildMapFrame (lvb_icp_map_optimize_keyframes, lvb_icp_map_build_optimize_keyframe)
+// and Mapping::BuildOldMapFrame (lvb_icp_map_relocate)
 static void bbox_store(lvb_icp::Segment& sg, const int* b) {
     for (int a = 0; a < 3; ++a) { sg.lo[a] = ord2f(b[a]); sg.hi[a] = ord2f(b[3 + a]); }
     sg.has_bbox = true;
@@ -1349,69 +1367,98 @@ static MapBound map_bound(const float* lo, const float* hi, float cell_size) {
     return b;
 }
 
-// The map frame of `keys` (BuildMapFrame, mapping.cpp:114-137; BuildOldMapFrame, :78-112) on both handles: the resident clouds in
-// merge order, the merged sizes, which side is built (an empty merged cloud: BuildMapFrame fails on that side and nothing registers,
-// :155,167), the descriptor seeds and the capacity bounds of the builds.  The missing bounding boxes of both handles are computed here,
-// with one synchronisation.
+// A map key's clouds: the ones keyframe kf of the call stores (kf >= 0), else the ones resident on both handles (seg)
+struct KfSrc { int kf; lvb_icp::Segment* seg[2]; };
+static bool find_resident(lvb_icp* const hs[2], long long key, KfSrc& sr) {
+    for (int m = 0; m < 2; ++m) { sr.seg[m] = nullptr; for (auto& sg : hs[m]->segments) if (sg.key == key) sr.seg[m] = &sg; }
+    return sr.seg[0] && sr.seg[1];
+}
+
+// One keyframe's map frame (BuildMapFrame, mapping.cpp:114-137; BuildOldMapFrame, :78-112) on both handles: the clouds in merge order,
+// the merged sizes, which side is built (an empty merged cloud: BuildMapFrame fails on that side and nothing registers, :155,167), the
+// descriptor seeds, the union lo..hi of the resident clouds' boxes and the capacity bounds of the builds.
 // cap: the limits the grid kernel keeps to (kGridLimits when the bounds come from exact boxes)
 struct KfPlan { std::vector<lvb_icp::Segment*> pick[2]; size_t total[2] = {0, 0}; bool build[2]; MapBound bound[2]; MapDesc seed[2];
-                GridCap cap[2] = {kGridLimits, kGridLimits}; };
-static int kf_plan(lvb_icp* const hs[2], const long long* keys, int n_keys, const float cell_size[2], bool ransac, const char* fn, KfPlan& pl) {
-    for (int k = 0; k < n_keys; ++k) {
+                GridCap cap[2] = {kGridLimits, kGridLimits}; float lo[2][3], hi[2][3]; };
+
+// A keyframe of kf_chain: lvb_map_keyframe with the map keys as a pointer and a count
+struct KfRec {
+    long long key; const long long* map_keys; int n_map_keys;
+    const void* pts[2]; int n[2];                 // the robot-frame clouds: ground, surf
+    const double* map_pose;
+    double pose[7];                               // in: frame->pose; out: optimised
+    double weight[2], prior_weight;
+    double transform[7], rpyxyz[6]; lvb_solve_summary summary[2]; int n_map_points[2];        // out
+};
+
+// The plans of the map frames of srcs[k], one per keyframe k.  The clouds keyframe j of the call stores (stage[2 j + m], of
+// kfs[j].n[m] points) have no box yet: the bounds are those of the resident clouds, and the caller widens them by the estimates of the
+// others (in_call_box).  The missing boxes of the resident clouds are computed with one synchronisation, after the checks that need none.
+static int plan_frames(lvb_icp* const hs[2], const std::vector<std::vector<KfSrc>>& srcs, const KfRec* kfs, lvb_icp::Segment* stage,
+                       const float cell_size[2], bool ransac, const char* fn, std::vector<KfPlan>& pl) {
+    pl.assign(srcs.size(), KfPlan());
+    std::vector<lvb_icp::Segment*> res;           // the resident clouds, each once
+    std::unordered_set<lvb_icp::Segment*> seen;
+    for (size_t k = 0; k < srcs.size(); ++k) {
+        KfPlan& q = pl[k];
+        for (auto& sr : srcs[k]) {
+            for (int m = 0; m < 2; ++m) {
+                if (sr.kf >= 0) { q.pick[m].push_back(&stage[2 * (size_t)sr.kf + m]); q.total[m] += kfs[sr.kf].n[m]; continue; }
+                q.pick[m].push_back(sr.seg[m]); q.total[m] += sr.seg[m]->n;
+                if (seen.insert(sr.seg[m]).second) res.push_back(sr.seg[m]);
+            }
+        }
         for (int m = 0; m < 2; ++m) {
-            lvb_icp::Segment* f = nullptr;
-            for (auto& sg : hs[m]->segments) if (sg.key == keys[k]) f = &sg;
-            if (!f) { set_error("%s: key %lld is not resident", fn, keys[k]); return LVB_ERR_INVALID; }
-            pl.pick[m].push_back(f); pl.total[m] += f->n;
+            if (q.total[m] > 0x7fffffffull) { set_error("%s: map frame of more than 2^31 points", fn); return LVB_ERR_INVALID; }
+            q.build[m] = q.total[m] > 0;
+            q.seed[m] = desc_seed(q.build[m] && !(m == 0 && ransac) ? (int)q.total[m] : 0);      // the ground count comes from SegmentGround
         }
     }
-    if (pl.total[0] > 0x7fffffffull || pl.total[1] > 0x7fffffffull) { set_error("%s: map frame of more than 2^31 points", fn); return LVB_ERR_INVALID; }
-    {   // both handles' missing boxes with one synchronisation
-        std::vector<lvb_icp::Segment*> both(pl.pick[0]);
-        both.insert(both.end(), pl.pick[1].begin(), pl.pick[1].end());
-        LVB_TRY(fill_bboxes(hs[0], both));
-    }
-    for (int m = 0; m < 2; ++m) {
-        pl.build[m] = pl.total[m] > 0;
-        pl.seed[m] = desc_seed(pl.build[m] && !(m == 0 && ransac) ? (int)pl.total[m] : 0);      // the ground count comes from SegmentGround
-        if (!pl.build[m]) continue;
-        float lo[3] = {FLT_MAX, FLT_MAX, FLT_MAX}, hi[3] = {-FLT_MAX, -FLT_MAX, -FLT_MAX};
-        for (auto* sg : pl.pick[m]) for (int a = 0; a < 3; ++a) { lo[a] = std::min(lo[a], sg->lo[a]); hi[a] = std::max(hi[a], sg->hi[a]); }
-        pl.bound[m] = map_bound(lo, hi, cell_size[m]);
-        // without SegmentGround the map frame's box is the union: the grid kernel's check can be made here (after it, on the device)
-        if (!pl.bound[m].finite && !(m == 0 && ransac)) { set_error("%s: map cloud has no finite bounding box", fn); return LVB_ERR_INVALID; }
+    LVB_TRY(fill_bboxes(hs[0], res));
+    for (size_t k = 0; k < srcs.size(); ++k) {
+        KfPlan& q = pl[k];
+        for (int m = 0; m < 2; ++m) {
+            float* lo = q.lo[m]; float* hi = q.hi[m];
+            for (int a = 0; a < 3; ++a) { lo[a] = FLT_MAX; hi[a] = -FLT_MAX; }
+            bool resident = false;
+            for (auto& sr : srcs[k]) {
+                if (sr.kf >= 0) continue;
+                for (int a = 0; a < 3; ++a) { lo[a] = std::min(lo[a], sr.seg[m]->lo[a]); hi[a] = std::max(hi[a], sr.seg[m]->hi[a]); }
+                resident = true;
+            }
+            if (!q.build[m]) continue;
+            q.bound[m] = map_bound(lo, hi, cell_size[m]);
+            // without SegmentGround the map frame's box is the union: the grid kernel's check can be made here (after it, on the device).
+            // The estimates of the call's clouds are finite: only the resident ones can make the box infinite.
+            if (resident && !q.bound[m].finite && !(m == 0 && ransac)) { set_error("%s: map cloud has no finite bounding box", fn); return LVB_ERR_INVALID; }
+        }
     }
     return LVB_OK;
 }
 
-// The builds of a plan: merge in key order, SegmentGround on the ground side (ground_threshold > 0), voxel hash sized by the bound into
-// the handle's buffers `slot`, grid decided on the device into u.blk->map[m].  maps[m]: what registration m reads of it.
-static int kf_build(lvb_icp* const hs[2], const KfPlan& pl, const float cell_size[2], double ground_threshold, const KfUpload& u,
-                    lvb_icp::MapBufs lvb_icp::* slot, KfMap maps[2]) {
-    lvb_ctx* ctx = hs[0]->ctx;
+// The build of side m of a plan: merge in key order, SegmentGround on the ground side (ground_threshold > 0), voxel hash sized by the
+// bound into `out`, grid decided on the device into u.blk->map[m].  map: what registration m reads of it.
+static int kf_build(lvb_icp* h, const KfPlan& pl, int m, float cell_size, double ground_threshold, const KfUpload& u,
+                    lvb_icp::MapBufs& out, KfMap& map) {
+    lvb_ctx* ctx = h->ctx;
     cudaStream_t s = ctx->stream;
-    for (int m = 0; m < 2; ++m) {
-        if (!pl.build[m]) continue;
-        lvb_icp* h = hs[m];
-        lvb_icp::MapBufs& out = h->*slot;
-        MapDesc* md = &u.blk->map[m];
-        const int n = (int)pl.total[m];
-        LVB_TRY(h->merged.ensure(n));
-        size_t o = 0;
-        for (auto* f : pl.pick[m]) { if (f->n) LVB_CUDA(cudaMemcpyAsync(h->merged.p + o, f->pts->p, (size_t)f->n * sizeof(float4), cudaMemcpyDeviceToDevice, s)); o += f->n; }
-        const float4* cloud = h->merged.p;
-        if (m == 0 && ground_threshold > 0.0) {
-            LVB_TRY(h->merged2.ensure(n));
-            LVB_TRY(lidar_segment_ground_device_async(ctx, h->merged.p, n, ground_threshold, h->merged2.p, &md->P));
-            lvb::g_alloc_stream = ctx->stream;
-            cloud = h->merged2.p;
-        }
-        const unsigned char* cp = reinterpret_cast<const unsigned char*>(cloud);
-        ILAUNCH(h, icp_bbox_kernel, std::min(1024, inblk(n, 256)), 256, cp, 16, md);
-        ILAUNCH(h, icp_map_grid_kernel, 1, 1, md, cell_size[m], pl.cap[m]);
-        LVB_TRY(enqueue_hash(h, cp, n, 16, md, pl.bound[m].cells, pl.bound[m].coarse, false, out));
-        maps[m] = {out.sorted.p, out.cell_start.p, out.coarse.p, cell_size[m], pl.bound[m].qsort, false};
+    MapDesc* md = &u.blk->map[m];
+    const int n = (int)pl.total[m];
+    LVB_TRY(h->merged.ensure(n));
+    size_t o = 0;
+    for (auto* f : pl.pick[m]) { if (f->n) LVB_CUDA(cudaMemcpyAsync(h->merged.p + o, f->pts->p, (size_t)f->n * sizeof(float4), cudaMemcpyDeviceToDevice, s)); o += f->n; }
+    const float4* cloud = h->merged.p;
+    if (m == 0 && ground_threshold > 0.0) {
+        LVB_TRY(h->merged2.ensure(n));
+        LVB_TRY(lidar_segment_ground_device_async(ctx, h->merged.p, n, ground_threshold, h->merged2.p, &md->P));
+        lvb::g_alloc_stream = ctx->stream;
+        cloud = h->merged2.p;
     }
+    const unsigned char* cp = reinterpret_cast<const unsigned char*>(cloud);
+    ILAUNCH(h, icp_bbox_kernel, std::min(1024, inblk(n, 256)), 256, cp, 16, md);
+    ILAUNCH(h, icp_map_grid_kernel, 1, 1, md, cell_size, pl.cap[m]);
+    LVB_TRY(enqueue_hash(h, cp, n, 16, md, pl.bound[m].cells, pl.bound[m].coarse, false, out));
+    map = {out.sorted.p, out.cell_start.p, out.coarse.p, cell_size, pl.bound[m].qsort, false};
     return LVB_OK;
 }
 
@@ -1422,7 +1469,7 @@ struct ScanState {
     void restore(lvb_icp* h) const { h->scan_n = n; h->scan_stride = stride; h->scan_dev = dev; h->kf_arena = arena; }
 };
 
-// The argument checks both map-building calls share; they come before any state changes
+// The argument checks of the calls that build map frames; they come before any state changes
 static int kf_check_args(lvb_icp* const hs[2], const float cell_size[2], const void* const pts[2], const int ns[2], int stride,
                          const lvb_map_optimize_params* p, const char* fn) {
     lvb_ctx* ctx = hs[0]->ctx;
@@ -1440,81 +1487,12 @@ static int kf_check_args(lvb_icp* const hs[2], const float cell_size[2], const v
     return LVB_OK;
 }
 
-// Mapping::BuildMapFrame (mapping.cpp:114-137) + the body of Mapping::Optimize's loop (:147-185) for one keyframe.  The host knows
-// every size the launches depend on -- the scans, the merged clouds (sums of resident cloud sizes), max_num_iterations -- and an upper
-// bound on each map frame's grid (map_bound of the union of the resident clouds' boxes); the device decides the grid itself
-// (icp_map_grid_kernel) and every counter is used up to that size.  One pinned upload, one read-back, one host synchronisation.
-int lvb_icp_map_build_optimize_keyframe(lvb_icp* ground, lvb_icp* surf, const long long* keys, int n_keys, const float cell_size[2],
-                                        double ground_threshold, const double map_pose[7], long long key, const void* ground_pts, int n_ground,
-                                        const void* surf_pts, int n_surf, int stride, const lvb_map_optimize_params* p, double pose[7],
-                                        double rpyxyz[6], lvb_solve_summary summary[2], int n_map_points[2]) {
-    static const char* fn = "lvb_icp_map_build_optimize_keyframe";
-    lvb_icp* hs[2] = {ground, surf};
-    const void* pts[2] = {ground_pts, surf_pts};
-    const int ns[2] = {n_ground, n_surf};
-    if (!ground || !surf || ground == surf || !cell_size || !map_pose || !p || !pose || !rpyxyz || n_keys < 0 || (n_keys && !keys)) {
-        set_error("%s: null or bad argument", fn); return LVB_ERR_INVALID; }
-    LVB_TRY(kf_check_args(hs, cell_size, pts, ns, stride, p, fn));
-    lvb_ctx* ctx = ground->ctx;
-    // the map frame: keys resident on both handles, in merge order; `key` is the keyframe being registered, not one of them
-    for (int k = 0; k < n_keys; ++k)
-        if (keys[k] == key) { set_error("%s: key %lld is one of the map frame's keys", fn, key); return LVB_ERR_INVALID; }
-    LVB_CUDA(cudaSetDevice(ctx->device)); lvb::g_alloc_stream = ctx->stream;
-    KfPlan pl;
-    LVB_TRY(kf_plan(hs, keys, n_keys, cell_size, ground_threshold > 0.0, fn, pl));
-    const auto t0 = std::chrono::steady_clock::now();
-    cudaStream_t s = ctx->stream;
-    lvb::timing_mark(s, "begin");
-    KfUpload u;
-    LVB_TRY(kf_upload(ctx, hs, map_pose, pose, pl.seed, pts, ns, stride, u));
-    KfMap maps[2];
-    LVB_TRY(kf_build(hs, pl, cell_size, ground_threshold, u, &lvb_icp::nx, maps));
-
-    // the registrations, each against the map frame just built
-    ScanState saved[2];
-    for (int m = 0; m < 2; ++m) saved[m].save(hs[m]);
-    lvb_icp::Segment fresh[2];
-    int rc = kf_register(hs, pl.build, maps, u, ns, stride, p);
-    if (rc == LVB_OK) rc = kf_to_world(hs, u, ns, stride, true, fresh);
-    if (rc == LVB_OK) rc = icheck("map_build_optimize_keyframe");
-    // the one read-back: solver states, pose, rpyxyz, both map descriptors (grid, point count, failure), the stored clouds' boxes
-    if (rc == LVB_OK && cudaMemcpyAsync(u.hb, u.blk, sizeof(KfBlock), cudaMemcpyDeviceToHost, s) != cudaSuccess) rc = lvb::cuda_fail(cudaGetLastError(), "read-back", __FILE__, __LINE__);
-    if (rc == LVB_OK) rc = host_sync(ctx, s);
-    if (rc == LVB_OK) ctx->stage_busy = false;
-    for (int m = 0; m < 2 && rc == LVB_OK; ++m) if (pl.build[m]) rc = grid_error(u.hb->map[m], fn, m ? "surf " : "ground ");
-    if (rc != LVB_OK) {        // nothing was committed: the resident clouds and the map frames are as they were
-        fresh[0].release(); fresh[1].release();
-        for (int m = 0; m < 2; ++m) saved[m].restore(hs[m]);
-        return rc;
-    }
-    const double el = std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
-    for (int m = 0; m < 2; ++m) {
-        lvb_icp* h = hs[m];
-        const MapDesc& md = u.hb->map[m];
-        const bool built = pl.build[m] && md.P > 0;
-        if (built) {           // the new map frame replaces the one before, as lvb_icp_map_build would
-            swap_buf(h->map_sorted, h->nx.sorted); swap_buf(h->cell_start, h->nx.cell_start); swap_buf(h->coarse, h->nx.coarse);
-            h->map = md; h->cell_size = cell_size[m]; h->have_map = true;
-        }
-        bbox_store(fresh[m], u.hb->out_bbox[m]);
-        store_segment(h, key, fresh[m]);
-        h->scan_n = ns[m]; h->scan_stride = stride; h->scan_dev = u.arena->p + u.off[m]; h->kf_arena = u.arena;
-        if (n_map_points) n_map_points[m] = built ? md.P : 0;
-        if (summary) {
-            if (built) fill_summary(u.hb->st[m], p->prior_weight, el, &summary[m]);
-            else { memset(&summary[m], 0, sizeof(summary[m])); summary[m].termination_type = -1; }
-        }
-    }
-    memcpy(pose, u.hb->pose, sizeof(u.hb->pose)); memcpy(rpyxyz, u.hb->rpyxyz, sizeof(u.hb->rpyxyz));
-    return LVB_OK;
-}
-
 // ---- Mapping::Optimize(active_kfs) (mapping.cpp:139-191) for every lidar keyframe of a backend pass in one call
-// (lvb_icp_map_optimize_keyframes).  Keyframe k's map frame may merge the clouds earlier keyframes of the call store: their poses are
-// decided on the device, so the host sizes that map frame from an estimate of their boxes -- the robot-frame box moved by the incoming
-// pose the caller gave, widened by kInCallMargin -- and passes the capacity it allocated to the grid kernel as a limit.  A cloud that
-// ends up outside its estimate makes the kernel take a coarser ring (each ring is exact); only a grid that does not fit at ring 1
-// fails.
+// (lvb_icp_map_optimize_keyframes), and for one keyframe (lvb_icp_map_build_optimize_keyframe) as the chain of one.  Keyframe k's map
+// frame may merge the clouds earlier keyframes of the call store: their poses are decided on the device, so the host sizes that map
+// frame from an estimate of their boxes -- the robot-frame box moved by the incoming pose the caller gave, widened by kInCallMargin --
+// and passes the capacity it allocated to the grid kernel as a limit.  A cloud that ends up outside its estimate makes the kernel take a
+// coarser ring (each ring is exact); only a grid that does not fit at ring 1 fails.
 static const float kInCallMargin = 1.0f;        // metres on every side
 static void in_call_box(const void* pts, int n, int stride, const double* pose, float lo[3], float hi[3]) {
     // compare-and-select: a NaN coordinate never wins; an infinite one leaves the box infinite (the device reports that cloud)
@@ -1553,109 +1531,61 @@ static void in_call_box(const void* pts, int n, int stride, const double* pose, 
 }
 
 // the call's parameters with keyframe kf's own weights and prior weight (ScanToMapWith* read them from each frame)
-static lvb_map_optimize_params kf_params(const lvb_map_optimize_params& p, const lvb_map_keyframe& kf) {
+static lvb_map_optimize_params kf_params(const lvb_map_optimize_params& p, const KfRec& kf) {
     lvb_map_optimize_params q = p;
     q.weight[0] = kf.weight[0]; q.weight[1] = kf.weight[1]; q.prior_weight = kf.prior_weight;
     return q;
 }
 
-// One call for a chain of keyframes, entirely on the device: per keyframe the incoming pose chained through the earlier keyframes'
-// transforms, the map frame (resident clouds and clouds of earlier keyframes) built into one of two slots per side, both registrations,
-// the transform and ToWorld into staged clouds.  One pinned upload, one read-back, one host synchronisation; the staged clouds and the
-// map frames are committed only when every keyframe succeeded.
-int lvb_icp_map_optimize_keyframes(lvb_icp* ground, lvb_icp* surf, lvb_map_keyframe* kfs, int n_kf, const float cell_size[2],
-                                   double ground_threshold, int stride, const lvb_map_optimize_params* p) {
-    static const char* fn = "lvb_icp_map_optimize_keyframes";
-    lvb_icp* hs[2] = {ground, surf};
-    if (!ground || !surf || ground == surf || !cell_size || !p || n_kf < 0 || (n_kf > 0 && !kfs)) { set_error("%s: null or bad argument", fn); return LVB_ERR_INVALID; }
-    {
-        const void* none[2] = {nullptr, nullptr};
-        const int zero[2] = {0, 0};
-        LVB_TRY(kf_check_args(hs, cell_size, none, zero, stride, p, fn));
-    }
-    std::unordered_map<long long, int> batch;
-    for (int k = 0; k < n_kf; ++k) {
-        const lvb_map_keyframe& kf = kfs[k];
-        const void* pts[2] = {kf.ground_pts, kf.surf_pts};
-        const int ns[2] = {kf.n_ground, kf.n_surf};
-        LVB_TRY(kf_check_args(hs, cell_size, pts, ns, stride, p, fn));
-        if (kf.n_map_keys < 0 || kf.n_map_keys > 3) { set_error("%s: keyframe %d has %d map keys (0 to 3)", fn, k, kf.n_map_keys); return LVB_ERR_INVALID; }
-        if (!batch.emplace(kf.key, k).second) { set_error("%s: key %lld is listed twice", fn, kf.key); return LVB_ERR_INVALID; }
-    }
-    // each map key: the cloud an earlier keyframe of the call stores (kf >= 0), else the resident one of both handles
-    struct Src { int kf; lvb_icp::Segment* seg[2]; };
-    std::vector<std::vector<Src>> srcs(n_kf);
+// A chain of keyframes, entirely on the device: per keyframe the incoming pose chained through the earlier keyframes' transforms, the
+// map frame (resident clouds and clouds of earlier keyframes) built into one of two slots per side, both registrations, the transform
+// and ToWorld into staged clouds.  The host knows every size the launches depend on -- the scans, the merged clouds, max_num_iterations
+// -- and an upper bound on each map frame's grid; the device decides the grid itself (icp_map_grid_kernel) and every counter is used up
+// to that size.  One pinned upload, one read-back, one host synchronisation; the staged clouds and the map frames are committed, and
+// the records' outputs written, only when every keyframe succeeded.  The callers have checked the arguments (kf_check_args).
+static int kf_chain(lvb_icp* const hs[2], KfRec* kfs, int n_kf, const float cell_size[2], double ground_threshold, int stride,
+                    const lvb_map_optimize_params* p, const char* fn) {
+    // each map key: the cloud an earlier keyframe of the call stores, else the resident one of both handles
+    std::vector<std::vector<KfSrc>> srcs(n_kf);
     for (int k = 0; k < n_kf; ++k) {
         for (int i = 0; i < kfs[k].n_map_keys; ++i) {
             const long long mk = kfs[k].map_keys[i];
             if (mk == kfs[k].key) { set_error("%s: key %lld is its own map key", fn, mk); return LVB_ERR_INVALID; }
-            Src sr = {-1, {nullptr, nullptr}};
-            const auto it = batch.find(mk);
-            if (it != batch.end() && it->second < k) sr.kf = it->second;
-            else {
-                for (int m = 0; m < 2; ++m) for (auto& sg : hs[m]->segments) if (sg.key == mk) sr.seg[m] = &sg;
-                if (!sr.seg[0] || !sr.seg[1]) {
-                    set_error("%s: map key %lld of keyframe %d is neither resident nor an earlier keyframe of the call", fn, mk, k); return LVB_ERR_INVALID; }
-            }
+            KfSrc sr = {-1, {nullptr, nullptr}};
+            for (int j = 0; j < k; ++j) if (kfs[j].key == mk) sr.kf = j;
+            if (sr.kf < 0 && !find_resident(hs, mk, sr)) {
+                set_error("%s: map key %lld of keyframe %d is neither resident nor an earlier keyframe of the call", fn, mk, k); return LVB_ERR_INVALID; }
             srcs[k].push_back(sr);
         }
     }
-    if (n_kf == 0) return LVB_OK;
-    lvb_ctx* ctx = ground->ctx;
+    lvb_ctx* ctx = hs[0]->ctx;
     LVB_CUDA(cudaSetDevice(ctx->device)); lvb::g_alloc_stream = ctx->stream;
-    {   // the missing boxes of the resident clouds, with one synchronisation
-        std::vector<lvb_icp::Segment*> res;
-        std::unordered_set<lvb_icp::Segment*> seen;
-        for (auto& v : srcs) for (auto& sr : v) if (sr.kf < 0) for (int m = 0; m < 2; ++m) if (seen.insert(sr.seg[m]).second) res.push_back(sr.seg[m]);
-        LVB_TRY(fill_bboxes(ground, res));
-    }
-    const bool ransac = ground_threshold > 0.0;
-    auto n_of = [&](int k, int m) { return m ? kfs[k].n_surf : kfs[k].n_ground; };
     std::vector<lvb_icp::Segment> stage(2 * (size_t)n_kf);          // [2 k + m]: the clouds ToWorld stores for keyframe k
-    // what is known before any launch: merge lists, sizes, which sides are built and into which slot (nx first, then in turn), the
-    // union of the resident clouds' boxes.  The estimated boxes of the call's own clouds, and with them the bounds of the map frames
-    // that merge them, are formed just before each keyframe is enqueued, while the device runs the keyframes before it.
-    std::vector<KfPlan> pl(n_kf);
+    std::vector<KfPlan> pl;
+    LVB_TRY(plan_frames(hs, srcs, kfs, stage.data(), cell_size, ground_threshold > 0.0, fn, pl));
+    // which slot each build goes into (nx first, then in turn), and the keyframe whose optimised pose is the map pose
     std::vector<int> map_from(n_kf, -1), slot(2 * (size_t)n_kf, -1);
-    std::vector<float> box(12 * (size_t)n_kf);                      // [12 k + 6 m]: lo, hi of the resident clouds in keyframe k's map frame
     int turn[2] = {-1, -1};
     for (int k = 0; k < n_kf; ++k) {
-        for (int m = 0; m < 2; ++m) {
-            float* lo = &box[12 * (size_t)k + 6 * m];
-            float* hi = lo + 3;
-            for (int a = 0; a < 3; ++a) { lo[a] = FLT_MAX; hi[a] = -FLT_MAX; }
-            bool resident = false;
-            for (auto& sr : srcs[k]) {
-                if (sr.kf >= 0) { pl[k].pick[m].push_back(&stage[2 * (size_t)sr.kf + m]); pl[k].total[m] += n_of(sr.kf, m); continue; }
-                pl[k].pick[m].push_back(sr.seg[m]); pl[k].total[m] += sr.seg[m]->n;
-                for (int a = 0; a < 3; ++a) { lo[a] = std::min(lo[a], sr.seg[m]->lo[a]); hi[a] = std::max(hi[a], sr.seg[m]->hi[a]); }
-                resident = true;
-            }
-            if (pl[k].total[m] > 0x7fffffffull) { set_error("%s: map frame of more than 2^31 points", fn); return LVB_ERR_INVALID; }
-            pl[k].build[m] = pl[k].total[m] > 0;
-            pl[k].seed[m] = desc_seed(pl[k].build[m] && !(m == 0 && ransac) ? (int)pl[k].total[m] : 0);
-            if (!pl[k].build[m]) continue;
-            turn[m] = turn[m] < 0 ? 0 : 1 - turn[m];
-            slot[2 * k + m] = turn[m];
-            // the estimates of the call's clouds are finite: only the resident ones can make the box infinite here
-            if (resident && !map_bound(lo, hi, cell_size[m]).finite && !(m == 0 && ransac)) { set_error("%s: map cloud has no finite bounding box", fn); return LVB_ERR_INVALID; }
-        }
+        for (int m = 0; m < 2; ++m) if (pl[k].build[m]) { turn[m] = turn[m] < 0 ? 0 : 1 - turn[m]; slot[2 * k + m] = turn[m]; }
         if (!srcs[k].empty() && srcs[k].back().kf >= 0) map_from[k] = srcs[k].back().kf;
     }
+    // The estimated boxes of the call's own clouds, and with them the bounds of the map frames that merge them, are formed just before
+    // each keyframe is enqueued, while the device runs the keyframes before it.
     std::vector<float> est(12 * (size_t)n_kf);                      // [12 k + 6 m]: the estimated box of keyframe k's stored cloud
     std::vector<char> have_est(2 * (size_t)n_kf, 0);
-    // keyframe k's bounds (kf_plan's, with the estimates of its in-call clouds) and the grid limits that follow from them
+    // keyframe k's bounds (the resident clouds' union with the estimates of its in-call clouds) and the grid limits that follow from them
     auto plan_bounds = [&](int k) {
         bool in_call = false;
         for (int m = 0; m < 2; ++m) {
             if (!pl[k].build[m]) continue;
             float lo[3], hi[3];
-            for (int a = 0; a < 3; ++a) { lo[a] = box[12 * (size_t)k + 6 * m + a]; hi[a] = box[12 * (size_t)k + 6 * m + 3 + a]; }
+            for (int a = 0; a < 3; ++a) { lo[a] = pl[k].lo[m][a]; hi[a] = pl[k].hi[m][a]; }
             for (auto& sr : srcs[k]) {
                 if (sr.kf < 0) continue;
                 const size_t e = 2 * (size_t)sr.kf + m;
                 if (!have_est[e]) {
-                    in_call_box(m ? kfs[sr.kf].surf_pts : kfs[sr.kf].ground_pts, n_of(sr.kf, m), stride, kfs[sr.kf].pose, &est[6 * e], &est[6 * e + 3]);
+                    in_call_box(kfs[sr.kf].pts[m], kfs[sr.kf].n[m], stride, kfs[sr.kf].pose, &est[6 * e], &est[6 * e + 3]);
                     have_est[e] = 1;
                 }
                 for (int a = 0; a < 3; ++a) { lo[a] = std::min(lo[a], est[6 * e + a]); hi[a] = std::max(hi[a], est[6 * e + 3 + a]); }
@@ -1674,35 +1604,18 @@ int lvb_icp_map_optimize_keyframes(lvb_icp* ground, lvb_icp* surf, lvb_map_keyfr
     const auto t0 = std::chrono::steady_clock::now();
     cudaStream_t s = ctx->stream;
     lvb::timing_mark(s, "begin");
-    // one pinned upload: [KfBlock x n_kf | KfLink x n_kf | ground and surf scan of each keyframe]
-    const size_t blk_bytes = ((size_t)n_kf * sizeof(KfBlock) + 255) & ~(size_t)255;
-    const size_t back_bytes = blk_bytes + (size_t)n_kf * sizeof(KfLink);
-    std::vector<size_t> off(2 * (size_t)n_kf);
-    size_t all = (back_bytes + 255) & ~(size_t)255;
-    for (int k = 0; k < n_kf; ++k)
-        for (int m = 0; m < 2; ++m) { off[2 * k + m] = all; all = (all + (size_t)n_of(k, m) * stride + 255) & ~(size_t)255; }
-    LVB_TRY(lvb::stage_wait(ctx));
-    LVB_TRY(lvb::stage_grow(ctx, all, 0));
-    KfBlock* hb = reinterpret_cast<KfBlock*>(ctx->stage_h);
-    KfLink* hl = reinterpret_cast<KfLink*>(ctx->stage_h + blk_bytes);
-    memset(hb, 0, (size_t)n_kf * sizeof(KfBlock));
-    memset(hl, 0, (size_t)n_kf * sizeof(KfLink));
-    for (int k = 0; k < n_kf; ++k) {
-        memcpy(hb[k].map_pose, kfs[k].map_pose, sizeof(hb[k].map_pose)); memcpy(hb[k].pose, kfs[k].pose, sizeof(hb[k].pose));
-        hl[k].k = k; hl[k].map_from = map_from[k];
-        for (int m = 0; m < 2; ++m) {
-            hb[k].map[m] = pl[k].seed[m];
-            bbox_seed(hb[k].out_bbox[m]);
-            const size_t bytes = (size_t)n_of(k, m) * stride;
-            if (bytes) memcpy(ctx->stage_h + off[2 * k + m], m ? kfs[k].surf_pts : kfs[k].ground_pts, bytes);
-        }
-    }
-    auto arena = std::make_shared<DevBuf<unsigned char>>();
-    LVB_TRY(arena->ensure(all));
-    LVB_CUDA(cudaMemcpyAsync(arena->p, ctx->stage_h, all, cudaMemcpyHostToDevice, s));
-    LVB_TRY(lvb::stage_mark_busy(ctx, s));
-    KfBlock* dblk = reinterpret_cast<KfBlock*>(arena->p);
-    KfLink* dlink = reinterpret_cast<KfLink*>(arena->p + blk_bytes);
+    std::vector<const void*> pts(2 * (size_t)n_kf);
+    std::vector<int> ns(2 * (size_t)n_kf);
+    for (int k = 0; k < n_kf; ++k) for (int m = 0; m < 2; ++m) { pts[2 * k + m] = kfs[k].pts[m]; ns[2 * k + m] = kfs[k].n[m]; }
+    std::vector<KfUpload> u;
+    size_t back;
+    LVB_TRY(kf_upload(ctx, n_kf, true, pts.data(), ns.data(), stride, u, back, [&](int k, KfUpload& v) {
+        memcpy(v.hb->map_pose, kfs[k].map_pose, sizeof(v.hb->map_pose)); memcpy(v.hb->pose, kfs[k].pose, sizeof(v.hb->pose));
+        for (int m = 0; m < 2; ++m) v.hb->map[m] = pl[k].seed[m];
+        v.hl->k = k; v.hl->map_from = map_from[k];
+    }));
+    KfBlock* dblk = u[0].blk;
+    KfLink* dlink = u[0].link;
 
     ScanState saved[2];
     for (int m = 0; m < 2; ++m) saved[m].save(hs[m]);
@@ -1713,44 +1626,40 @@ int lvb_icp_map_optimize_keyframes(lvb_icp* ground, lvb_icp* surf, lvb_map_keyfr
     size_t held[2][2][3] = {};
     int rc = LVB_OK;
     for (int k = 0; k < n_kf && rc == LVB_OK; ++k) {
-        KfUpload u;
-        u.arena = arena; u.blk = dblk + k; u.hb = hb + k; u.off[0] = off[2 * k]; u.off[1] = off[2 * k + 1]; u.link = dlink + k;
-        const int ns[2] = {kfs[k].n_ground, kfs[k].n_surf};
         const lvb_map_optimize_params pk = kf_params(*p, kfs[k]);
         KfMap maps[2];
         plan_bounds(k);
         for (int m = 0; m < 2 && rc == LVB_OK; ++m) {
             const int sl = slot[2 * k + m];
             if (sl < 0) continue;
+            lvb_icp* h = hs[m];
+            lvb_icp::MapBufs& dst = sl ? h->chain : h->nx;
             size_t* need = held[m][sl];
             need[0] = pl[k].total[m]; need[1] = pl[k].bound[m].cells; need[2] = pl[k].bound[m].coarse;
             if (last[m] >= 0) {
                 for (int i = 0; i < 3; ++i) need[i] = std::max(need[i], held[m][1 - sl][i]);
-                lvb_icp::MapBufs& b = sl ? hs[m]->chain : hs[m]->nx;
-                rc = b.sorted.ensure(need[0]);
-                if (rc == LVB_OK) rc = b.cell_start.ensure(need[1] + 1);
-                if (rc == LVB_OK) rc = b.coarse.ensure(need[2]);
+                rc = dst.sorted.ensure(need[0]);
+                if (rc == LVB_OK) rc = dst.cell_start.ensure(need[1] + 1);
+                if (rc == LVB_OK) rc = dst.coarse.ensure(need[2]);
                 if (rc != LVB_OK) break;
             }
-            KfPlan one = pl[k];
-            one.build[1 - m] = false;
-            rc = kf_build(hs, one, cell_size, ground_threshold, u, sl ? &lvb_icp::chain : &lvb_icp::nx, maps);
+            rc = kf_build(h, pl[k], m, cell_size[m], ground_threshold, u[k], dst, maps[m]);
             if (rc == LVB_OK && last[m] >= 0) {
-                lvb_icp* h = hs[m];
                 const lvb_icp::MapBufs& src = sl ? h->nx : h->chain;
-                lvb_icp::MapBufs& dst = sl ? h->chain : h->nx;
                 ILAUNCH(h, icp_map_keep_kernel, 2 * ctx->sm_count, 256, &dblk[k].map[m], kept_desc(dblk, dlink, m), &dlink[k].kept[m],
                         src.sorted.p, src.cell_start.p, src.coarse.p, dst.sorted.p, dst.cell_start.p, dst.coarse.p);
             }
             if (first[m] < 0) first[m] = k;
             last[m] = k;
         }
-        if (rc == LVB_OK) rc = kf_register(hs, pl[k].build, maps, u, ns, stride, &pk);
-        if (rc == LVB_OK) rc = kf_to_world(hs, u, ns, stride, true, &stage[2 * (size_t)k]);
+        if (rc == LVB_OK) rc = kf_register(hs, pl[k].build, maps, u[k], kfs[k].n, stride, &pk);
+        if (rc == LVB_OK) rc = kf_to_world(hs, u[k], kfs[k].n, stride, true, &stage[2 * (size_t)k]);
     }
     if (rc == LVB_OK) rc = icheck(fn);
     // the one read-back: every keyframe's solver states, poses, map descriptors and stored boxes, and its link (transform, kept frames)
-    if (rc == LVB_OK && cudaMemcpyAsync(hb, dblk, back_bytes, cudaMemcpyDeviceToHost, s) != cudaSuccess) rc = lvb::cuda_fail(cudaGetLastError(), "read-back", __FILE__, __LINE__);
+    const KfBlock* hb = u[0].hb;
+    const KfLink* hl = u[0].hl;
+    if (rc == LVB_OK && cudaMemcpyAsync(u[0].hb, dblk, back, cudaMemcpyDeviceToHost, s) != cudaSuccess) rc = lvb::cuda_fail(cudaGetLastError(), "read-back", __FILE__, __LINE__);
     if (rc == LVB_OK) rc = host_sync(ctx, s);
     if (rc == LVB_OK) ctx->stage_busy = false;
     for (int k = 0; k < n_kf && rc == LVB_OK; ++k) {
@@ -1780,10 +1689,11 @@ int lvb_icp_map_optimize_keyframes(lvb_icp* ground, lvb_icp* surf, lvb_map_keyfr
                 h->map = kd; h->cell_size = cell_size[m]; h->have_map = true;
             }
         }
-        h->scan_n = n_of(n_kf - 1, m); h->scan_stride = stride; h->scan_dev = arena->p + off[2 * (n_kf - 1) + m]; h->kf_arena = arena;
+        const KfUpload& ul = u[n_kf - 1];
+        h->scan_n = kfs[n_kf - 1].n[m]; h->scan_stride = stride; h->scan_dev = ul.arena->p + ul.off[m]; h->kf_arena = ul.arena;
     }
     for (int k = 0; k < n_kf; ++k) {
-        lvb_map_keyframe& kf = kfs[k];
+        KfRec& kf = kfs[k];
         for (int m = 0; m < 2; ++m) {
             lvb_icp::Segment& sg = stage[2 * (size_t)k + m];
             bbox_store(sg, hb[k].out_bbox[m]);
@@ -1800,10 +1710,69 @@ int lvb_icp_map_optimize_keyframes(lvb_icp* ground, lvb_icp* surf, lvb_map_keyfr
     return LVB_OK;
 }
 
+// Mapping::BuildMapFrame (mapping.cpp:114-137) + the body of Mapping::Optimize's loop (:147-185) for one keyframe: kf_chain of one
+// keyframe with the call's weights and prior weight
+int lvb_icp_map_build_optimize_keyframe(lvb_icp* ground, lvb_icp* surf, const long long* keys, int n_keys, const float cell_size[2],
+                                        double ground_threshold, const double map_pose[7], long long key, const void* ground_pts, int n_ground,
+                                        const void* surf_pts, int n_surf, int stride, const lvb_map_optimize_params* p, double pose[7],
+                                        double rpyxyz[6], lvb_solve_summary summary[2], int n_map_points[2]) {
+    static const char* fn = "lvb_icp_map_build_optimize_keyframe";
+    lvb_icp* hs[2] = {ground, surf};
+    const void* pts[2] = {ground_pts, surf_pts};
+    const int ns[2] = {n_ground, n_surf};
+    if (!ground || !surf || ground == surf || !cell_size || !map_pose || !p || !pose || !rpyxyz || n_keys < 0 || (n_keys && !keys)) {
+        set_error("%s: null or bad argument", fn); return LVB_ERR_INVALID; }
+    LVB_TRY(kf_check_args(hs, cell_size, pts, ns, stride, p, fn));
+    KfRec kf = {key, keys, n_keys, {ground_pts, surf_pts}, {n_ground, n_surf}, map_pose, {}, {p->weight[0], p->weight[1]}, p->prior_weight};
+    memcpy(kf.pose, pose, sizeof(kf.pose));
+    LVB_TRY(kf_chain(hs, &kf, 1, cell_size, ground_threshold, stride, p, fn));
+    memcpy(pose, kf.pose, sizeof(kf.pose)); memcpy(rpyxyz, kf.rpyxyz, sizeof(kf.rpyxyz));
+    if (summary) memcpy(summary, kf.summary, sizeof(kf.summary));
+    if (n_map_points) memcpy(n_map_points, kf.n_map_points, sizeof(kf.n_map_points));
+    return LVB_OK;
+}
+
+int lvb_icp_map_optimize_keyframes(lvb_icp* ground, lvb_icp* surf, lvb_map_keyframe* kfs, int n_kf, const float cell_size[2],
+                                   double ground_threshold, int stride, const lvb_map_optimize_params* p) {
+    static const char* fn = "lvb_icp_map_optimize_keyframes";
+    lvb_icp* hs[2] = {ground, surf};
+    if (!ground || !surf || ground == surf || !cell_size || !p || n_kf < 0 || (n_kf > 0 && !kfs)) { set_error("%s: null or bad argument", fn); return LVB_ERR_INVALID; }
+    {
+        const void* none[2] = {nullptr, nullptr};
+        const int zero[2] = {0, 0};
+        LVB_TRY(kf_check_args(hs, cell_size, none, zero, stride, p, fn));
+    }
+    std::unordered_set<long long> batch;
+    for (int k = 0; k < n_kf; ++k) {
+        const lvb_map_keyframe& kf = kfs[k];
+        const void* pts[2] = {kf.ground_pts, kf.surf_pts};
+        const int ns[2] = {kf.n_ground, kf.n_surf};
+        LVB_TRY(kf_check_args(hs, cell_size, pts, ns, stride, p, fn));
+        if (kf.n_map_keys < 0 || kf.n_map_keys > 3) { set_error("%s: keyframe %d has %d map keys (0 to 3)", fn, k, kf.n_map_keys); return LVB_ERR_INVALID; }
+        if (!batch.insert(kf.key).second) { set_error("%s: key %lld is listed twice", fn, kf.key); return LVB_ERR_INVALID; }
+    }
+    if (n_kf == 0) return LVB_OK;
+    std::vector<KfRec> rec(n_kf);
+    for (int k = 0; k < n_kf; ++k) {
+        const lvb_map_keyframe& kf = kfs[k];
+        rec[k] = {kf.key, kf.map_keys, kf.n_map_keys, {kf.ground_pts, kf.surf_pts}, {kf.n_ground, kf.n_surf}, kf.map_pose, {},
+                  {kf.weight[0], kf.weight[1]}, kf.prior_weight};
+        memcpy(rec[k].pose, kf.pose, sizeof(kf.pose));
+    }
+    LVB_TRY(kf_chain(hs, rec.data(), n_kf, cell_size, ground_threshold, stride, p, fn));
+    for (int k = 0; k < n_kf; ++k) {
+        lvb_map_keyframe& kf = kfs[k];
+        memcpy(kf.pose, rec[k].pose, sizeof(kf.pose)); memcpy(kf.rpyxyz, rec[k].rpyxyz, sizeof(kf.rpyxyz));
+        memcpy(kf.transform, rec[k].transform, sizeof(kf.transform));
+        memcpy(kf.summary, rec[k].summary, sizeof(kf.summary)); memcpy(kf.n_map_points, rec[k].n_map_points, sizeof(kf.n_map_points));
+    }
+    return LVB_OK;
+}
+
 // ---- Mapping::Relocate for one loop-closure candidate (mapping.cpp:251-300): BuildOldMapFrame (:78-112) into each handle's
-// relocation slot, then `rounds` rounds of both registrations without a prior, all on the device.  The same sizes are known on the host
-// as in lvb_icp_map_build_optimize_keyframe; one pinned upload, one read-back, one host synchronisation.  Nothing is stored and the
-// handles' map frames, resident clouds and map_append(NULL) scan stay as they were.
+// relocation slot, then `rounds` rounds of both registrations without a prior, all on the device.  The map frame is planned as a
+// keyframe of kf_chain whose keys are all resident; one pinned upload, one read-back, one host synchronisation.  Nothing is stored and
+// the handles' map frames, resident clouds and map_append(NULL) scan stay as they were.
 int lvb_icp_map_relocate(lvb_icp* ground, lvb_icp* surf, const long long* keys, int n_keys, const float cell_size[2], double ground_threshold,
                          const double map_pose[7], const double old_pose[7], const double relative_guess[7],
                          const void* ground_pts, int n_ground, const void* surf_pts, int n_surf, int stride,
@@ -1821,16 +1790,29 @@ int lvb_icp_map_relocate(lvb_icp* ground, lvb_icp* surf, const long long* keys, 
     if (!(p->prior_weight < 0.0)) { set_error("%s: prior_weight must be < 0 (ScanToMapWith* with relocate = true add no prior)", fn); return LVB_ERR_INVALID; }
     lvb_ctx* ctx = ground->ctx;
     LVB_CUDA(cudaSetDevice(ctx->device)); lvb::g_alloc_stream = ctx->stream;
-    KfPlan pl;
-    LVB_TRY(kf_plan(hs, keys, n_keys, cell_size, ground_threshold > 0.0, fn, pl));
+    std::vector<std::vector<KfSrc>> srcs(1);
+    for (int k = 0; k < n_keys; ++k) {
+        KfSrc sr = {-1, {nullptr, nullptr}};
+        if (!find_resident(hs, keys[k], sr)) { set_error("%s: key %lld is not resident", fn, keys[k]); return LVB_ERR_INVALID; }
+        srcs[0].push_back(sr);
+    }
+    std::vector<KfPlan> plans;
+    LVB_TRY(plan_frames(hs, srcs, nullptr, nullptr, cell_size, ground_threshold > 0.0, fn, plans));
+    const KfPlan& pl = plans[0];
     const auto t0 = std::chrono::steady_clock::now();
     cudaStream_t s = ctx->stream;
     lvb::timing_mark(s, "begin");
-    KfUpload u;
-    const double* reloc[2] = {old_pose, relative_guess};
-    LVB_TRY(kf_upload(ctx, hs, map_pose, old_pose /* replaced on the device by old_pose * relative_guess */, pl.seed, pts, ns, stride, u, reloc));
+    std::vector<KfUpload> uk;
+    size_t back;
+    LVB_TRY(kf_upload(ctx, 1, false, pts, ns, stride, uk, back, [&](int, KfUpload& v) {
+        memcpy(v.hb->map_pose, map_pose, sizeof(v.hb->map_pose));
+        memcpy(v.hb->pose, old_pose, sizeof(v.hb->pose));          // replaced on the device by old_pose * relative_guess
+        memcpy(v.hb->old_pose, old_pose, sizeof(v.hb->old_pose)); memcpy(v.hb->rel, relative_guess, sizeof(v.hb->rel));
+        for (int m = 0; m < 2; ++m) v.hb->map[m] = pl.seed[m];
+    }));
+    const KfUpload& u = uk[0];
     KfMap maps[2];
-    LVB_TRY(kf_build(hs, pl, cell_size, ground_threshold, u, &lvb_icp::reloc, maps));
+    for (int m = 0; m < 2; ++m) if (pl.build[m]) LVB_TRY(kf_build(hs[m], pl, m, cell_size[m], ground_threshold, u, hs[m]->reloc, maps[m]));
 
     ScanState saved[2];
     for (int m = 0; m < 2; ++m) saved[m].save(hs[m]);
@@ -1840,7 +1822,7 @@ int lvb_icp_map_relocate(lvb_icp* ground, lvb_icp* surf, const long long* keys, 
     if (rc == LVB_OK) ILAUNCH(ground, icp_reloc_pose_kernel, 1, 1, u.blk, 1);
     if (rc == LVB_OK) rc = icheck(fn);
     // the one read-back: solver states, pose, relative_o_c, scores, both map descriptors (grid, point count, failure)
-    if (rc == LVB_OK && cudaMemcpyAsync(u.hb, u.blk, sizeof(KfBlock), cudaMemcpyDeviceToHost, s) != cudaSuccess) rc = lvb::cuda_fail(cudaGetLastError(), "read-back", __FILE__, __LINE__);
+    if (rc == LVB_OK && cudaMemcpyAsync(u.hb, u.blk, back, cudaMemcpyDeviceToHost, s) != cudaSuccess) rc = lvb::cuda_fail(cudaGetLastError(), "read-back", __FILE__, __LINE__);
     if (rc == LVB_OK) rc = host_sync(ctx, s);
     if (rc == LVB_OK) ctx->stage_busy = false;
     for (int m = 0; m < 2; ++m) saved[m].restore(hs[m]);
