@@ -326,7 +326,7 @@ typedef struct lvb_map_keyframe {
     long long key;                          /* in: the keyframe's time key */
     long long map_keys[3];                  /* in: its map frame's keys, merge order */
     int n_map_keys;                         /* in: 0 to 3 */
-    int n_ground, n_surf;                   /* in: robot-frame cloud sizes */
+    int n_ground, n_surf;                   /* in: robot-frame cloud sizes (< 0 with NULL clouds: by key, lvb_icp_map_extract_keyframe) */
     const void* ground_pts;                 /* in: n_ground records of stride_bytes */
     const void* surf_pts;                   /* in: n_surf records */
     double map_pose[7];                     /* in: the newest map key's pose (unused when it is a keyframe of the call) */
@@ -411,15 +411,44 @@ LVB_API int lvb_lidar_radius_outlier_removal(lvb_ctx* ctx, const float* xyzi, in
 /* FeatureAssociation::SegmentGround (association.cpp:254-268): inliers of the RANSAC plane (100 iterations, p = 0.99) */
 LVB_API int lvb_lidar_segment_ground(lvb_ctx* ctx, const float* xyzi, int n, double distance_threshold, float* out_xyzi, int32_t* n_out);
 /* FeatureAssociation::Process: raw scan -> frame->feature_lidar {points_ground, points_surf} in the robot frame.
- * Output capacity num_scans * horizon_scan points each. */
+ * Output capacity num_scans * horizon_scan points each.  One host synchronisation: every stage keeps its count on the device. */
 LVB_API int lvb_lidar_extract_features(lvb_ctx* ctx, const lvb_lidar_config* cfg, const void* points, int n, int stride_bytes,
                                        float* ground_xyzi, int32_t* n_ground, float* surf_xyzi, int32_t* n_surf);
+
+/* FeatureAssociation::Process into the resident map (association.cpp:85-109: AddScan -> Process fills frame->feature_lidar, which
+ * Mapping::Optimize registers and stores through ToWorld, mapping.cpp:139-220): lvb_lidar_extract_features on the handles' context, and
+ * the two robot-frame feature clouds stay on the device as the PENDING FEATURES of `key` -- the ground cloud on `ground`, the surf cloud
+ * on `surf`, as packed 16-byte (x, y, z, intensity) records with their robot-frame bounding boxes.  One host synchronisation brings back
+ * the counts (always) and the host copies (ground_xyzi / surf_xyzi may be NULL; capacity num_scans * horizon_scan points each) -- the
+ * same points, in the same order, as lvb_lidar_extract_features.
+ *   Registering by key: an lvb_map_keyframe record (or lvb_icp_map_build_optimize_keyframe's arguments) with ground_pts == NULL &&
+ *   n_ground < 0 and surf_pts == NULL && n_surf < 0 takes the pending features of its key as its two clouds: nothing is uploaded for
+ *   them, and they are read as their own 16-byte records (stride_bytes must still be valid: >= 12, a multiple of 4).  Both sides by
+ *   key or neither; a by-key record without pending features on both handles is LVB_ERR_INVALID before any state changes.  Each
+ *   pending cloud is kept in a buffer of exactly its points; on success it becomes the stored keyframe's robot-frame cloud as it is
+ *   (no copy) and the pending entry is gone; on any failure it stays.  The launches and synchronisations are those of the same call fed
+ *   with the host copies (stride 16).
+ *   Pending features are not resident: lvb_icp_map_build, lvb_icp_map_relocate, lvb_icp_map_to_world and the map keys of the keyframe
+ *   calls do not know a pending-only key.  lvb_icp_map_evict(key) drops them (key < 0: all); another extraction under the same key
+ *   replaces them.
+ * Errors, all before any state changes: LVB_ERR_INVALID for a bad configuration or cloud arguments (lvb_lidar_extract_features'),
+ * NULL or equal handles, NULL n_ground / n_surf, handles of different contexts; a feature voxel grid above 2^26 voxels is
+ * LVB_ERR_UNSUPPORTED, found on the device and reported after the synchronisation, storing nothing.  Not collective: allowed on a
+ * sharded context.  Threading: as lvb_icp_map_relocate, the caller serialises it with the mapping thread's calls on these handles and
+ * their context. */
+LVB_API int lvb_icp_map_extract_keyframe(lvb_icp* ground, lvb_icp* surf, const lvb_lidar_config* cfg, long long key,
+                                         const void* points, int n, int stride_bytes,
+                                         int32_t* n_ground, int32_t* n_surf,              /* out, always */
+                                         float* ground_xyzi, float* surf_xyzi);           /* out, may be NULL */
 
 /* ---- profiling hooks (used by tools/kernel_timing*.py; not part of the drop-in surface) */
 /* enable != 0: record a CUDA event after every kernel of the BA pass (disables the graph); 0: print the per-kernel times */
 LVB_API int lvb_debug_timing(int enable);
 /* as lvb_debug_timing(0), but writes "kernel_name microseconds" lines (launch order) into out instead of printing them */
 LVB_API int lvb_debug_timing_report(char* out, int cap);
+/* the capacities, in 16-byte records, of the buffers the handle keeps for `key`: cap[0] its resident world cloud, cap[1] its
+ * robot-frame cloud, cap[2] its pending features (-1: none) */
+LVB_API int lvb_debug_icp_cloud_capacity(lvb_icp* icp, long long key, long long cap[3]);
 /* the voxel grid of the handle's current map frame: grid[0] = ring (voxels per search radius: 4, 2 or 1), grid[1..3] = voxels per
  * axis.  LVB_ERR_STATE without a map frame. */
 LVB_API int lvb_debug_icp_map_grid(lvb_icp* icp, int grid[4]);

@@ -47,7 +47,38 @@ inline void add_block(P& p, long, bool, ceres::CostFunction* c, ceres::LossFunct
 
 class LVB_ASSOCIATION_CLASS {
 public:
-    explicit LVB_ASSOCIATION_CLASS(double lidar_resolution = 0.2) : resolution_(lidar_resolution) {}
+    explicit LVB_ASSOCIATION_CLASS(double lidar_resolution = 0.2) : resolution_(lidar_resolution) {
+        lvb_lidar_default_config(&lidar_cfg_);
+        lidar_cfg_.resolution = lidar_resolution;
+    }
+    // the lidar configuration ExtractKeyframe uses (FeatureAssociation's constructor arguments, association.h:21-26; by default
+    // kitti.yaml's with this object's resolution and an identity extrinsic), e.g. lvb::LidarFeatureExtractor::config()
+    void SetLidarConfig(const lvb_lidar_config& cfg) { lidar_cfg_ = cfg; }
+
+    // FeatureAssociation::AddScan -> Process (association.cpp:85-109) straight into the resident map (lvb_icp_map_extract_keyframe):
+    // the scan's two feature clouds stay on the device as the pending features of `key`, and frame->feature_lidar->points_ground /
+    // points_surf (which the caller has created; the Relocator and ToWorldKeyframes read them) receive the host copies.
+    // OptimizeKeyframe(frame, keys, ...) and OptimizeKeyframes then register a pending key by key, with no upload; the other
+    // OptimizeKeyframe overload uses the host copies and drops the pending features first.  Threading: as RelocateKeyframe -- it runs
+    // on the handles that keep the resident map (the mapping thread's, once that thread has stored a keyframe) from whichever thread
+    // calls it, and the caller serialises it with that thread's device calls (INTEGRATION.md).  A keyframe call on other handles than
+    // the ones holding the pending features uses the host copies.  false: the call failed and changed nothing (lvb_last_error()).
+    template <class Cloud, class FramePtr>
+    bool ExtractKeyframe(long long key, const Cloud& points, FramePtr frame) {
+        Handles& h = resident_ ? *resident_ : handles_of_thread()[this];
+        if (!ensure_handles(h)) return false;
+        const size_t cap = (size_t)lidar_cfg_.num_scans * (size_t)lidar_cfg_.horizon_scan;
+        extract_ground_.resize(cap); extract_surf_.resize(cap);
+        int32_t ng = 0, ns = 0;
+        const int stride = (int)sizeof(assoc_detail::cloud_data(points, 0)[0]);
+        if (lvb_icp_map_extract_keyframe(h.ground, h.surf, &lidar_cfg_, key, assoc_detail::cloud_data(points, 0), (int)points.size(), stride, &ng, &ns,
+                                         &extract_ground_[0].x, &extract_surf_[0].x) != LVB_OK)
+            return false;
+        unpack(extract_ground_, ng, frame->feature_lidar->points_ground);
+        unpack(extract_surf_, ns, frame->feature_lidar->points_surf);
+        h.pending.insert(key);
+        return true;
+    }
     ~LVB_ASSOCIATION_CLASS() {                      // the calling thread's handles; another thread's go with that thread's context
         auto& m = handles_of_thread();
         auto it = m.find(this);
@@ -158,6 +189,10 @@ public:
         lvb_icp* reg_s = h.surf_map ? h.surf : nullptr;
         lvb_solve_summary sums[2];
         lvb_solve_summary* out = summary ? summary : sums;
+        if (h.pending.erase(key)) {                 // this call stores the host copies: the pending features (and key's clouds) go first
+            if (lvb_icp_map_evict(h.ground, key) != LVB_OK || lvb_icp_map_evict(h.surf, key) != LVB_OK) return false;
+            h.keys.erase(key);
+        }
         if (reg_g || reg_s) {
             const lvb_map_optimize_params p = MapOptimizeParams(frame);
             double rpyxyz[6];
@@ -198,10 +233,13 @@ public:
         lvb_solve_summary sums[2];
         double rpyxyz[6];
         int n_map[2];
+        const bool by_key = h.pending.count(key) > 0;          // ExtractKeyframe left the clouds on the device: NULL clouds, -1 points
         if (lvb_icp_map_build_optimize_keyframe(h.ground, h.surf, keys, n_keys, cells, ground_ransac_threshold, map_pose7, key,
-                                                assoc_detail::cloud_data(g, 0), (int)g.size(), assoc_detail::cloud_data(s, 0), (int)s.size(), stride,
+                                                by_key ? nullptr : assoc_detail::cloud_data(g, 0), by_key ? -1 : (int)g.size(),
+                                                by_key ? nullptr : assoc_detail::cloud_data(s, 0), by_key ? -1 : (int)s.size(), stride,
                                                 &p, frame->pose.data(), rpyxyz, summary ? summary : sums, n_map) != LVB_OK)
             return false;
+        h.pending.erase(key);
         h.ground_map = n_map[0] > 0; h.surf_map = n_map[1] > 0;
         h.resident = h.ground_map && h.surf_map;
         h.keys.insert(key);
@@ -234,8 +272,11 @@ public:
             std::memset(&r, 0, sizeof(r));
             r.key = keys[k]; r.n_map_keys = n_map_keys[k];
             for (int i = 0; i < n_map_keys[k] && i < 3; ++i) r.map_keys[i] = map_keys[3 * k + i];
-            r.ground_pts = assoc_detail::cloud_data(g, 0); r.n_ground = (int)g.size();
-            r.surf_pts = assoc_detail::cloud_data(s, 0); r.n_surf = (int)s.size();
+            if (h.pending.count(keys[k])) { r.ground_pts = r.surf_pts = nullptr; r.n_ground = r.n_surf = -1; }      // by key (ExtractKeyframe)
+            else {
+                r.ground_pts = assoc_detail::cloud_data(g, 0); r.n_ground = (int)g.size();
+                r.surf_pts = assoc_detail::cloud_data(s, 0); r.n_surf = (int)s.size();
+            }
             std::memcpy(r.map_pose, map_poses7 + 7 * k, sizeof(r.map_pose)); std::memcpy(r.pose, frames[k]->pose.data(), sizeof(r.pose));
             const lvb_map_optimize_params pk = MapOptimizeParams(frames[k]);      // each keyframe's own weights and prior weight
             r.weight[0] = pk.weight[0]; r.weight[1] = pk.weight[1]; r.prior_weight = pk.prior_weight;
@@ -250,6 +291,7 @@ public:
             if (transforms7) std::memcpy(transforms7 + 7 * k, r.transform, sizeof(r.transform));
             if (summary) { summary[2 * k] = r.summary[0]; summary[2 * k + 1] = r.summary[1]; }
             h.keys.insert(keys[k]);
+            h.pending.erase(keys[k]);
         }
         // as OptimizeKeyframe(frame, keys, ...) leaves them after the last keyframe: that keyframe's map frames
         h.ground_map = recs[n - 1].n_map_points[0] > 0; h.surf_map = recs[n - 1].n_map_points[1] > 0;
@@ -326,16 +368,23 @@ private:
     // (ceres_shim.h): Mapping::Optimize and Relocator::RelocateByPoints reach the same object from two threads without a lock
     // (mapping.cpp:155-177, relocator.cpp:188-206), so every thread gets its own pair.
     // resident: both map frames built (ScanToMapWith* use them); ground_map / surf_map: that side's map frame is the last BuildMapFrame's;
-    // keys: the keyframes whose clouds both handles hold (ToWorldKeyframes re-anchors those on the device)
+    // keys: the keyframes whose clouds both handles hold (ToWorldKeyframes re-anchors those on the device); pending: the keys whose
+    // features ExtractKeyframe left on these handles
     struct Handles {
         lvb_icp* ground = nullptr; lvb_icp* surf = nullptr; bool resident = false, ground_map = false, surf_map = false;
-        std::unordered_set<long long> keys;
+        std::unordered_set<long long> keys, pending;
     };
+    struct Packed { float x, y, z, intensity; };     // the records lvb_icp_map_extract_keyframe returns
+    template <class CloudOut>
+    static void unpack(const std::vector<Packed>& src, int n, CloudOut& dst) {
+        dst.resize((size_t)n);
+        for (int i = 0; i < n; ++i) { auto& q = dst[(size_t)i]; q.x = src[i].x; q.y = src[i].y; q.z = src[i].z; q.intensity = src[i].intensity; }
+    }
     // ToWorld of one keyframe into h: its two robot-frame clouds replace whatever h held under `key`
     template <class Cloud>
     static bool store_keyframe(Handles& h, long long key, const Cloud& ground_robot, const Cloud& surf_robot, const double* pose7) {
         const int stride = (int)sizeof(assoc_detail::cloud_data(ground_robot, 0)[0]);
-        h.keys.erase(key);
+        h.keys.erase(key); h.pending.erase(key);
         lvb_icp_map_evict(h.ground, key); lvb_icp_map_evict(h.surf, key);            // re-registering a keyframe (ToWorld(start)) replaces its clouds
         if (lvb_icp_map_append(h.ground, key, assoc_detail::cloud_data(ground_robot, 0), (int)ground_robot.size(), stride, pose7) != LVB_OK ||
             lvb_icp_map_append(h.surf, key, assoc_detail::cloud_data(surf_robot, 0), (int)surf_robot.size(), stride, pose7) != LVB_OK)
@@ -350,6 +399,8 @@ private:
     }
     static std::unordered_map<const void*, Handles>& handles_of_thread() { static thread_local std::unordered_map<const void*, Handles> m; return m; }
     double resolution_;
+    lvb_lidar_config lidar_cfg_;
+    std::vector<Packed> extract_ground_, extract_surf_;      // ExtractKeyframe's host copies, num_scans * horizon_scan records each
     Handles* resident_ = nullptr;      // the handles that keep the resident keyframe clouds (RelocateKeyframe); map nodes do not move
 };
 

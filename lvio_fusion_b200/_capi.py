@@ -164,11 +164,14 @@ _LVB_ONLY = {
     "icp_map_to_world": (C.c_int, [VP, VP, C.POINTER(C.c_longlong), C.c_int, c_double_p]),
     "icp_map_optimize_keyframes": (C.c_int, [VP, VP, C.POINTER(MapKeyframe), C.c_int, c_float_p, C.c_double, C.c_int,
                                              C.POINTER(MapOptimizeParams)]),
+    "icp_map_extract_keyframe": (C.c_int, [VP, VP, C.POINTER(LidarConfig), C.c_longlong, VP, C.c_int, C.c_int, c_int32_p, c_int32_p,
+                                           c_float_p, c_float_p]),
     "sync_count": (C.c_longlong, [VP]),
     "debug_timing": (C.c_int, [C.c_int]),
     "debug_cholesky_clocks": (C.c_int, [C.POINTER(C.c_longlong), C.c_int]),
     "debug_timing_report": (C.c_int, [C.c_char_p, C.c_int]),
     "debug_icp_map_grid": (C.c_int, [VP, c_int_p]),
+    "debug_icp_cloud_capacity": (C.c_int, [VP, C.c_longlong, C.POINTER(C.c_longlong)]),
     "debug_band_solve": (C.c_int, [VP, C.c_int, C.c_int, c_double_p, c_double_p, c_double_p, C.c_int, c_int_p]),
 }
 

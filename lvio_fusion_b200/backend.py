@@ -347,14 +347,20 @@ class FeatureAssociation:
         return e, s
 
 
-def _keyframe_args(fn, ground, surf, ground_points, surf_points, weight, prior_weight, huber_a, dist_thr, options, kw):
-    """The clouds, their common stride and the lvb_map_optimize_params of optimize_keyframe / build_and_optimize_keyframe."""
+def _keyframe_args(fn, ground, surf, ground_points, surf_points, weight, prior_weight, huber_a, dist_thr, options, kw, by_key=False):
+    """The clouds, their common stride and the lvb_map_optimize_params of optimize_keyframe / build_and_optimize_keyframe.
+    With by_key, ground_points and surf_points both None stand for the keyframe's pending features (LidarFeatures.extract_into):
+    NULL clouds of -1 points, stride None."""
     if ground is None and surf is None:
         raise ValueError("%s: at least one of ground / surf is needed" % fn)
     api = (ground or surf).api
+    if by_key and (ground_points is None) != (surf_points is None):
+        raise ValueError("%s: give both clouds (host arrays) or neither (None: the pending features of the key)" % fn)
     pts, n, strides = [None, None], [0, 0], set()
+    if by_key and ground_points is None:
+        n, strides = [-1, -1], {None}
     for m, (fa, cloud) in enumerate(((ground, ground_points), (surf, surf_points))):
-        if fa is not None:
+        if fa is not None and n[m] >= 0:
             pts[m], n[m], stride = FeatureAssociation._cloud(cloud)
             strides.add(stride)
     if len(strides) != 1:
@@ -397,11 +403,13 @@ def build_and_optimize_keyframe(ground, surf, keys, cell_sizes, ground_threshold
     synchronisation (CUDA library only): map_build of `keys` on both handles (cell_sizes = (ground, surf); SegmentGround on the
     ground side when ground_threshold > 0), then optimize_keyframe.  Both handles are required; an empty `keys` is the first lidar
     keyframe (nothing registered, both clouds stored at `pose`).  A side whose map frame comes out empty is not registered
-    (termination_type -1).  Returns (pose, rpyxyz, (ground summary, surf summary), (ground map points, surf map points))."""
+    (termination_type -1).  ground_points = surf_points = None: the pending features of `key` (LidarFeatures.extract_into), registered
+    and stored without an upload.  Returns (pose, rpyxyz, (ground summary, surf summary), (ground map points, surf map points))."""
     if ground is None or surf is None:
         raise ValueError("build_and_optimize_keyframe: both the ground and the surf handle are needed")
     api, pts, vp, n, stride, prm = _keyframe_args("build_and_optimize_keyframe", ground, surf, ground_points, surf_points, weight,
-                                                  prior_weight, huber_a, dist_thr, options, kw)
+                                                  prior_weight, huber_a, dist_thr, options, kw, by_key=True)
+    stride = 16 if stride is None else stride
     k = (C.c_longlong * max(1, len(keys)))(*[int(x) for x in keys])
     cs = np.asarray(cell_sizes, dtype=np.float32).reshape(2).copy()
     mp = _f64(map_pose).reshape(7)
@@ -423,7 +431,8 @@ def build_and_optimize_keyframes(ground, surf, keyframes, cell_sizes, ground_thr
     key is resident; pose is the incoming pose as the caller holds it, before the earlier keyframes' ForwardUpdates (the device chains
     them, se3.forward_update restates it).  weight ((ground, surf)) and prior_weight are each keyframe's own, as ScanToMapWith* take
     them from each frame: one value for all keyframes, or one per keyframe (n x 2 and n).  The other arguments are
-    build_and_optimize_keyframe's and apply to every keyframe.
+    build_and_optimize_keyframe's and apply to every keyframe.  ground_points = surf_points = None: that keyframe's pending features
+    (LidarFeatures.extract_into); by-key and host-cloud keyframes may be mixed.
     Returns one (pose, transform, rpyxyz, (ground summary, surf summary), (ground map points, surf map points)) per keyframe, with
     transform = optimised pose * incoming pose^-1, the T of PoseGraph::ForwardUpdate(T, t_k + epsilon)."""
     fn = "build_and_optimize_keyframes"
@@ -452,8 +461,9 @@ def build_and_optimize_keyframes(ground, surf, keyframes, cell_sizes, ground_thr
         mp, p = _f64(map_pose).reshape(-1), _f64(pose).reshape(-1)
         if mp.size != 7 or p.size != 7:
             raise ValueError("%s: keyframe %d: map_pose and pose are 7 doubles [qx qy qz qw tx ty tz]" % (fn, k))
-        api, pts, vp, n, stride, prm = _keyframe_args(fn, ground, surf, gp, sp, w[k], pw[k], huber_a, dist_thr, options, kw)
-        strides.add(stride)
+        api, pts, vp, n, stride, prm = _keyframe_args(fn, ground, surf, gp, sp, w[k], pw[k], huber_a, dist_thr, options, kw, by_key=True)
+        if stride is not None:
+            strides.add(stride)
         seen.append(key)
         keep.append(pts)
         r = recs[k]
@@ -582,6 +592,27 @@ class LidarFeatures:
 
     def segment_ground(self, cloud, threshold):
         return self._filter(self.ctx.api.lidar_segment_ground, "lidar_segment_ground", cloud, C.c_double(threshold))
+
+    def extract_into(self, ground, surf, key, points, copies=True):
+        """FeatureAssociation::Process into the map handles (lvb_icp_map_extract_keyframe, CUDA library only): the robot-frame ground
+        and surf clouds stay on the device as the pending features of `key` on `ground` / `surf` (FeatureAssociation handles of this
+        pipeline's context), for build_and_optimize_keyframe(s) with None clouds.  Returns (points_ground, points_surf) -- host
+        copies, the same as extract() -- with copies, else their sizes (n_ground, n_surf)."""
+        if ground is None or surf is None or ground is surf:
+            raise ValueError("extract_into: two different handles, ground and surf, are needed")
+        if ground.ctx is not self.ctx or surf.ctx is not self.ctx:
+            raise ValueError("extract_into: the handles must belong to this pipeline's context")
+        pts, n, stride = self._raw(points)
+        cap = self.capacity
+        g = np.empty((cap, 4), np.float32) if copies else None
+        s = np.empty((cap, 4), np.float32) if copies else None
+        ng, ns = np.zeros(1, np.int32), np.zeros(1, np.int32)
+        a = self.ctx.api
+        a.check(a.icp_map_extract_keyframe(ground.h, surf.h, C.byref(self.cfg), int(key), pts.ctypes.data_as(C.c_void_p), n, stride, _ip(ng), _ip(ns),
+                                           _fp(g) if copies else None, _fp(s) if copies else None), "icp_map_extract_keyframe")
+        if not copies:
+            return int(ng[0]), int(ns[0])
+        return g[:int(ng[0])].copy(), s[:int(ns[0])].copy()
 
     def extract(self, points):
         """FeatureAssociation::Process: returns (points_ground, points_surf) in the robot frame."""

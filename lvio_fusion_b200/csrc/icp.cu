@@ -761,7 +761,11 @@ struct lvb_icp {
     // the keyframe calls' upload (kf_upload: blocks, links, scans) in one allocation, held by both handles of the call
     // so that either one's scan stays valid for lvb_icp_map_append(NULL) until that handle uploads another scan
     std::shared_ptr<DevBuf<unsigned char>> kf_arena;
-    ~lvb_icp() { for (auto& sg : segments) sg.release(); }
+    // lvb_icp_map_extract_keyframe's robot-frame feature cloud of a keyframe not yet stored (pending features): packed (x, y, z,
+    // intensity) records and their bounding box.  The keyframe calls register it by key and store it as the keyframe's robot cloud.
+    struct Pending { long long key; DevBuf<float4>* pts = nullptr; int n; float lo[3], hi[3]; };
+    std::vector<Pending> pending;
+    ~lvb_icp() { for (auto& sg : segments) sg.release(); for (auto& pd : pending) delete pd.pts; }
 };
 
 #define ILAUNCH(h, kernel, grid, block, ...)                                              \
@@ -920,6 +924,25 @@ static int build_map(lvb_icp* h, const unsigned char* d_points, int n, int strid
     return LVB_OK;
 }
 
+// A cloud stored by a by-key keyframe call keeps the pending buffer as its robot-frame records, and the scan lvb_icp_map_append(NULL)
+// refers to may be that buffer: it goes with the cloud.
+static void release_segment(lvb_icp* h, lvb_icp::Segment& sg) {
+    if (sg.robot && h->scan_dev == reinterpret_cast<const unsigned char*>(sg.robot->p)) { h->scan_n = 0; h->scan_dev = nullptr; }
+    sg.release();
+}
+static lvb_icp::Pending* find_pending(lvb_icp* h, long long key) {
+    for (auto& pd : h->pending) if (pd.key == key) return &pd;
+    return nullptr;
+}
+// drop the pending features of `key` (key < 0: all)
+static void drop_pending(lvb_icp* h, long long key) {
+    size_t w = 0;
+    for (size_t i = 0; i < h->pending.size(); ++i) {
+        if (key < 0 || h->pending[i].key == key) delete h->pending[i].pts; else h->pending[w++] = h->pending[i];
+    }
+    h->pending.resize(w);
+}
+
 extern "C" {
 
 int lvb_icp_create(lvb_ctx* ctx, lvb_icp** out) {
@@ -977,9 +1000,10 @@ int lvb_icp_map_evict(lvb_icp* h, long long key) {
     LVB_CUDA(cudaSetDevice(h->ctx->device)); lvb::g_alloc_stream = h->ctx->stream;
     size_t w = 0;
     for (size_t i = 0; i < h->segments.size(); ++i) {
-        if (key < 0 || h->segments[i].key == key) h->segments[i].release(); else h->segments[w++] = h->segments[i];
+        if (key < 0 || h->segments[i].key == key) release_segment(h, h->segments[i]); else h->segments[w++] = h->segments[i];
     }
     h->segments.resize(w);
+    drop_pending(h, key);
     return LVB_OK;
 }
 
@@ -1152,20 +1176,25 @@ struct KfUpload {                                     // one keyframe's part of 
     size_t off[2];                                    // where its scans lie in the arena
     KfLink* link = nullptr;                           // its KfLink (device), with links
     KfLink* hl = nullptr;                             // its KfLink in the staging area
+    const unsigned char* scan[2];                     // its scans (device): in the arena, or pending features (by_key)
+    int stride[2];                                    // their record sizes
+    bool by_key[2] = {false, false};
 };
 
 // One copy from the pinned staging area for n keyframes: the blocks (zero but for the out_bbox seeds and what fill(k, u[k]) writes
 // into keyframe k's: poses, map descriptors), with `links` the links (zero but for fill's), and the scans pts[2 k + m] of ns[2 k + m]
-// records.  u[k]: keyframe k's views; back: the bytes of the blocks and links, which the read-back copies.  The staging area stays
-// busy until the caller's read-back.
-static int kf_upload(lvb_ctx* ctx, int n, bool links, const void* const* pts, const int* ns, int stride, std::vector<KfUpload>& u,
-                     size_t& back, const std::function<void(int, KfUpload&)>& fill) {
+// records -- except those with dev[2 k + m] (dev may be NULL), pending features already on the device, which are not copied.
+// u[k]: keyframe k's views; back: the bytes of the blocks and links, which the read-back copies.  The staging area stays busy until
+// the caller's read-back.
+static int kf_upload(lvb_ctx* ctx, int n, bool links, const void* const* pts, const float4* const* dev, const int* ns, int stride,
+                     std::vector<KfUpload>& u, size_t& back, const std::function<void(int, KfUpload&)>& fill) {
+    auto on_device = [&](int e) { return dev && dev[e]; };
     const size_t blk_bytes = ((size_t)n * sizeof(KfBlock) + 255) & ~(size_t)255;
     back = blk_bytes + (links ? (size_t)n * sizeof(KfLink) : 0);
     u.assign(n, KfUpload());
     size_t all = (back + 255) & ~(size_t)255;
     for (int k = 0; k < n; ++k)
-        for (int m = 0; m < 2; ++m) { u[k].off[m] = all; all = (all + (size_t)ns[2 * k + m] * stride + 255) & ~(size_t)255; }
+        for (int m = 0; m < 2; ++m) { u[k].off[m] = all; all = (all + (on_device(2 * k + m) ? 0 : (size_t)ns[2 * k + m] * stride) + 255) & ~(size_t)255; }
     LVB_TRY(lvb::stage_wait(ctx));
     LVB_TRY(lvb::stage_grow(ctx, all, 0));
     KfBlock* hb = reinterpret_cast<KfBlock*>(ctx->stage_h);
@@ -1177,7 +1206,7 @@ static int kf_upload(lvb_ctx* ctx, int n, bool links, const void* const* pts, co
         if (links) u[k].hl = hl + k;
         for (int m = 0; m < 2; ++m) {
             bbox_seed(hb[k].out_bbox[m]);
-            const size_t bytes = (size_t)ns[2 * k + m] * stride;
+            const size_t bytes = on_device(2 * k + m) ? 0 : (size_t)ns[2 * k + m] * stride;
             if (bytes) memcpy(ctx->stage_h + u[k].off[m], pts[2 * k + m], bytes);
         }
         fill(k, u[k]);
@@ -1190,6 +1219,12 @@ static int kf_upload(lvb_ctx* ctx, int n, bool links, const void* const* pts, co
         u[k].arena = arena;
         u[k].blk = reinterpret_cast<KfBlock*>(arena->p) + k;
         if (links) u[k].link = reinterpret_cast<KfLink*>(arena->p + blk_bytes) + k;
+        for (int m = 0; m < 2; ++m) {
+            const int e = 2 * k + m;
+            u[k].by_key[m] = on_device(e);
+            u[k].scan[m] = on_device(e) ? reinterpret_cast<const unsigned char*>(dev[e]) : arena->p + u[k].off[m];
+            u[k].stride[m] = on_device(e) ? (int)sizeof(float4) : stride;
+        }
     }
     return LVB_OK;
 }
@@ -1202,7 +1237,7 @@ struct KfMap { const float4* sorted; const int* cell_start; const int* coarse; f
 // run (run[m]): se32rpyxyz of the pose on the device, ScanToMapWithGround + Solve, the pose hand-off, ScanToMapWithSegmented + Solve,
 // the pose hand-off.  Nothing waits for the host: each registration runs max_num_iterations + 1 LM passes (the kernels return at once
 // after the solver stopped), and the pose kernels write the query transform the next association reads.
-static int kf_register(lvb_icp* const hs[2], const bool run[2], const KfMap maps[2], const KfUpload& u, const int ns[2], int stride,
+static int kf_register(lvb_icp* const hs[2], const bool run[2], const KfMap maps[2], const KfUpload& u, const int ns[2],
                        const lvb_map_optimize_params* p) {
     KfSeed seed;
     seed.o = p->options; seed.prior_w = p->prior_weight;
@@ -1215,7 +1250,7 @@ static int kf_register(lvb_icp* const hs[2], const bool run[2], const KfMap maps
         const KfMap& km = maps[m];
         IcpDev d;
         d.map = km.sorted; d.cell_start = km.cell_start; d.coarse = km.coarse;
-        LVB_TRY(bind_scan(h, u.arena->p + u.off[m], ns[m], stride, &u.blk->map[m], u.blk->tf, km.cell_size * km.cell_size, p->dist_thr[m],
+        LVB_TRY(bind_scan(h, u.scan[m], ns[m], u.stride[m], &u.blk->map[m], u.blk->tf, km.cell_size * km.cell_size, p->dist_thr[m],
                           km.nc, km.exact, d));
         h->kf_arena = u.arena;
         d.st = &u.blk->st[m];
@@ -1229,16 +1264,16 @@ static int kf_register(lvb_icp* const hs[2], const bool run[2], const KfMap maps
 
 // The end of Mapping::Optimize's loop body: ToWorld (:185, :205-220) of the scans of every handle given, transformed by the final
 // pose.cast<float>(), into fresh[] with their robot-frame records (not yet stored; with `boxes`, their bounding boxes into
-// blk->out_bbox)
-static int kf_to_world(lvb_icp* const hs[2], const KfUpload& u, const int ns[2], int stride, bool boxes, lvb_icp::Segment fresh[2]) {
+// blk->out_bbox).  A scan of pending features is its own robot-frame record: fresh[m].robot stays NULL until the caller commits.
+static int kf_to_world(lvb_icp* const hs[2], const KfUpload& u, const int ns[2], bool boxes, lvb_icp::Segment fresh[2]) {
     for (int m = 0; m < 2; ++m) {
         if (!hs[m]) continue;
-        fresh[m].key = -1; fresh[m].n = ns[m]; fresh[m].pts = new DevBuf<float4>(); fresh[m].robot = new DevBuf<float4>();
+        fresh[m].key = -1; fresh[m].n = ns[m]; fresh[m].pts = new DevBuf<float4>(); fresh[m].robot = u.by_key[m] ? nullptr : new DevBuf<float4>();
         int rc = fresh[m].pts->ensure(std::max(1, ns[m]));
-        if (rc == LVB_OK) rc = fresh[m].robot->ensure(std::max(1, ns[m]));
+        if (rc == LVB_OK && fresh[m].robot) rc = fresh[m].robot->ensure(std::max(1, ns[m]));
         if (rc != LVB_OK) { fresh[0].release(); fresh[1].release(); return rc; }
-        ILAUNCH(hs[m], icp_to_world_kernel, inblk(ns[m], 256), 256, u.arena->p + u.off[m], fresh[m].pts->p, fresh[m].robot->p, ns[m], stride,
-                u.blk->tf, boxes ? u.blk->out_bbox[m] : nullptr);
+        ILAUNCH(hs[m], icp_to_world_kernel, inblk(ns[m], 256), 256, u.scan[m], fresh[m].pts->p, fresh[m].robot ? fresh[m].robot->p : nullptr, ns[m],
+                u.stride[m], u.blk->tf, boxes ? u.blk->out_bbox[m] : nullptr);
     }
     return LVB_OK;
 }
@@ -1246,7 +1281,7 @@ static int kf_to_world(lvb_icp* const hs[2], const KfUpload& u, const int ns[2],
 // replace the cloud under `key` with sg, or add it
 static void store_segment(lvb_icp* h, long long key, lvb_icp::Segment& sg) {
     sg.key = key;
-    for (auto& old : h->segments) if (old.key == key) { old.release(); old = sg; return; }
+    for (auto& old : h->segments) if (old.key == key) { release_segment(h, old); old = sg; return; }
     h->segments.push_back(sg);
 }
 
@@ -1285,14 +1320,14 @@ int lvb_icp_map_optimize_keyframe(lvb_icp* ground, lvb_icp* surf, const double m
         if (hs[m]) maps[m] = {hs[m]->map_sorted.p, hs[m]->cell_start.p, hs[m]->coarse.p, hs[m]->cell_size, (size_t)hs[m]->map.nc, true};
     std::vector<KfUpload> uk;
     size_t back;
-    LVB_TRY(kf_upload(ctx, 1, false, pts, up, stride, uk, back, [&](int, KfUpload& v) {
+    LVB_TRY(kf_upload(ctx, 1, false, pts, nullptr, up, stride, uk, back, [&](int, KfUpload& v) {
         memcpy(v.hb->map_pose, map_pose, sizeof(v.hb->map_pose)); memcpy(v.hb->pose, pose, sizeof(v.hb->pose));
         for (int m = 0; m < 2; ++m) v.hb->map[m] = hs[m] ? hs[m]->map : desc_seed(0);          // P = 0: no registration on that side
     }));
     const KfUpload& u = uk[0];
     lvb_icp::Segment fresh[2];
-    LVB_TRY(kf_register(hs, run, maps, u, ns, stride, p));
-    LVB_TRY(kf_to_world(hs, u, ns, stride, false, fresh));
+    LVB_TRY(kf_register(hs, run, maps, u, ns, p));
+    LVB_TRY(kf_to_world(hs, u, ns, false, fresh));
     int rc = icheck("map_optimize_keyframe");
     if (rc != LVB_OK) { fresh[0].release(); fresh[1].release(); return rc; }
     for (int m = 0; m < 2; ++m) if (hs[m]) store_segment(hs[m], key, fresh[m]);
@@ -1385,6 +1420,7 @@ struct KfPlan { std::vector<lvb_icp::Segment*> pick[2]; size_t total[2] = {0, 0}
 struct KfRec {
     long long key; const long long* map_keys; int n_map_keys;
     const void* pts[2]; int n[2];                 // the robot-frame clouds: ground, surf
+    lvb_icp::Pending* pend[2];                    // by key: the pending features of `key` on each handle (pts unused), else NULL
     const double* map_pose;
     double pose[7];                               // in: frame->pose; out: optimised
     double weight[2], prior_weight;
@@ -1494,16 +1530,9 @@ static int kf_check_args(lvb_icp* const hs[2], const float cell_size[2], const v
 // and passes the capacity it allocated to the grid kernel as a limit.  A cloud that ends up outside its estimate makes the kernel take a
 // coarser ring (each ring is exact); only a grid that does not fit at ring 1 fails.
 static const float kInCallMargin = 1.0f;        // metres on every side
-static void in_call_box(const void* pts, int n, int stride, const double* pose, float lo[3], float hi[3]) {
-    // compare-and-select: a NaN coordinate never wins; an infinite one leaves the box infinite (the device reports that cloud)
-    float l0 = FLT_MAX, l1 = FLT_MAX, l2 = FLT_MAX, h0 = -FLT_MAX, h1 = -FLT_MAX, h2 = -FLT_MAX;
-    const unsigned char* base = static_cast<const unsigned char*>(pts);
-    for (int i = 0; i < n; ++i) {
-        const float* f = reinterpret_cast<const float*>(base + (size_t)i * stride);
-        l0 = f[0] < l0 ? f[0] : l0; l1 = f[1] < l1 ? f[1] : l1; l2 = f[2] < l2 ? f[2] : l2;
-        h0 = f[0] > h0 ? f[0] : h0; h1 = f[1] > h1 ? f[1] : h1; h2 = f[2] > h2 ? f[2] : h2;
-    }
-    const double mn[3] = {l0, l1, l2}, mx[3] = {h0, h1, h2};
+// The estimate from the robot-frame box rlo..rhi (FLT_MAX / -FLT_MAX when empty)
+static void world_box(const float rlo[3], const float rhi[3], const double* pose, float lo[3], float hi[3]) {
+    const double mn[3] = {rlo[0], rlo[1], rlo[2]}, mx[3] = {rhi[0], rhi[1], rhi[2]};
     double wl[3], wh[3];
     bool finite = true;
     for (int a = 0; a < 3; ++a) finite = finite && mn[a] <= mx[a] && std::isfinite(mn[a]) && std::isfinite(mx[a]) && mn[a] > -FLT_MAX && mx[a] < FLT_MAX;
@@ -1528,6 +1557,17 @@ static void in_call_box(const void* pts, int n, int stride, const double* pose, 
         lo[a] = std::nextafter((float)(wl[a] - kInCallMargin), -INFINITY);
         hi[a] = std::nextafter((float)(wh[a] + kInCallMargin), INFINITY);
     }
+}
+// The estimate of a host cloud.  Pending features carry the box the device computed over their points (all finite), which is this one.
+static void in_call_box(const void* pts, int n, int stride, const double* pose, float lo[3], float hi[3]) {
+    // compare-and-select: a NaN coordinate never wins; an infinite one leaves the box infinite (the device reports that cloud)
+    float l[3] = {FLT_MAX, FLT_MAX, FLT_MAX}, h[3] = {-FLT_MAX, -FLT_MAX, -FLT_MAX};
+    const unsigned char* base = static_cast<const unsigned char*>(pts);
+    for (int i = 0; i < n; ++i) {
+        const float* f = reinterpret_cast<const float*>(base + (size_t)i * stride);
+        for (int a = 0; a < 3; ++a) { l[a] = f[a] < l[a] ? f[a] : l[a]; h[a] = f[a] > h[a] ? f[a] : h[a]; }
+    }
+    world_box(l, h, pose, lo, hi);
 }
 
 // the call's parameters with keyframe kf's own weights and prior weight (ScanToMapWith* read them from each frame)
@@ -1585,7 +1625,9 @@ static int kf_chain(lvb_icp* const hs[2], KfRec* kfs, int n_kf, const float cell
                 if (sr.kf < 0) continue;
                 const size_t e = 2 * (size_t)sr.kf + m;
                 if (!have_est[e]) {
-                    in_call_box(kfs[sr.kf].pts[m], kfs[sr.kf].n[m], stride, kfs[sr.kf].pose, &est[6 * e], &est[6 * e + 3]);
+                    const KfRec& src = kfs[sr.kf];
+                    if (src.pend[m]) world_box(src.pend[m]->lo, src.pend[m]->hi, src.pose, &est[6 * e], &est[6 * e + 3]);
+                    else in_call_box(src.pts[m], src.n[m], stride, src.pose, &est[6 * e], &est[6 * e + 3]);
                     have_est[e] = 1;
                 }
                 for (int a = 0; a < 3; ++a) { lo[a] = std::min(lo[a], est[6 * e + a]); hi[a] = std::max(hi[a], est[6 * e + 3 + a]); }
@@ -1605,11 +1647,13 @@ static int kf_chain(lvb_icp* const hs[2], KfRec* kfs, int n_kf, const float cell
     cudaStream_t s = ctx->stream;
     lvb::timing_mark(s, "begin");
     std::vector<const void*> pts(2 * (size_t)n_kf);
+    std::vector<const float4*> dev(2 * (size_t)n_kf);
     std::vector<int> ns(2 * (size_t)n_kf);
-    for (int k = 0; k < n_kf; ++k) for (int m = 0; m < 2; ++m) { pts[2 * k + m] = kfs[k].pts[m]; ns[2 * k + m] = kfs[k].n[m]; }
+    for (int k = 0; k < n_kf; ++k)
+        for (int m = 0; m < 2; ++m) { pts[2 * k + m] = kfs[k].pts[m]; dev[2 * k + m] = kfs[k].pend[m] ? kfs[k].pend[m]->pts->p : nullptr; ns[2 * k + m] = kfs[k].n[m]; }
     std::vector<KfUpload> u;
     size_t back;
-    LVB_TRY(kf_upload(ctx, n_kf, true, pts.data(), ns.data(), stride, u, back, [&](int k, KfUpload& v) {
+    LVB_TRY(kf_upload(ctx, n_kf, true, pts.data(), dev.data(), ns.data(), stride, u, back, [&](int k, KfUpload& v) {
         memcpy(v.hb->map_pose, kfs[k].map_pose, sizeof(v.hb->map_pose)); memcpy(v.hb->pose, kfs[k].pose, sizeof(v.hb->pose));
         for (int m = 0; m < 2; ++m) v.hb->map[m] = pl[k].seed[m];
         v.hl->k = k; v.hl->map_from = map_from[k];
@@ -1652,8 +1696,8 @@ static int kf_chain(lvb_icp* const hs[2], KfRec* kfs, int n_kf, const float cell
             if (first[m] < 0) first[m] = k;
             last[m] = k;
         }
-        if (rc == LVB_OK) rc = kf_register(hs, pl[k].build, maps, u[k], kfs[k].n, stride, &pk);
-        if (rc == LVB_OK) rc = kf_to_world(hs, u[k], kfs[k].n, stride, true, &stage[2 * (size_t)k]);
+        if (rc == LVB_OK) rc = kf_register(hs, pl[k].build, maps, u[k], kfs[k].n, &pk);
+        if (rc == LVB_OK) rc = kf_to_world(hs, u[k], kfs[k].n, true, &stage[2 * (size_t)k]);
     }
     if (rc == LVB_OK) rc = icheck(fn);
     // the one read-back: every keyframe's solver states, poses, map descriptors and stored boxes, and its link (transform, kept frames)
@@ -1690,12 +1734,13 @@ static int kf_chain(lvb_icp* const hs[2], KfRec* kfs, int n_kf, const float cell
             }
         }
         const KfUpload& ul = u[n_kf - 1];
-        h->scan_n = kfs[n_kf - 1].n[m]; h->scan_stride = stride; h->scan_dev = ul.arena->p + ul.off[m]; h->kf_arena = ul.arena;
+        h->scan_n = kfs[n_kf - 1].n[m]; h->scan_stride = ul.stride[m]; h->scan_dev = ul.scan[m]; h->kf_arena = ul.arena;
     }
     for (int k = 0; k < n_kf; ++k) {
         KfRec& kf = kfs[k];
         for (int m = 0; m < 2; ++m) {
             lvb_icp::Segment& sg = stage[2 * (size_t)k + m];
+            if (kf.pend[m]) { sg.robot = kf.pend[m]->pts; kf.pend[m]->pts = nullptr; }     // moved: the pending entry goes below
             bbox_store(sg, hb[k].out_bbox[m]);
             store_segment(hs[m], kf.key, sg);
             const MapDesc& md = hb[k].map[m];
@@ -1707,6 +1752,26 @@ static int kf_chain(lvb_icp* const hs[2], KfRec* kfs, int n_kf, const float cell
         memcpy(kf.pose, hb[k].pose, sizeof(kf.pose)); memcpy(kf.rpyxyz, hb[k].rpyxyz, sizeof(kf.rpyxyz));
         memcpy(kf.transform, hl[k].T, sizeof(kf.transform));
     }
+    for (int m = 0; m < 2; ++m) {
+        auto& pv = hs[m]->pending;
+        pv.erase(std::remove_if(pv.begin(), pv.end(), [](const lvb_icp::Pending& pd) { return pd.pts == nullptr; }), pv.end());
+    }
+    return LVB_OK;
+}
+
+// A record's clouds by key (ground_pts == NULL && n_ground < 0, and the same for surf): the pending features of its key on both
+// handles.  One side alone, or a key with nothing pending on a handle, is an error; nothing changes.
+static int resolve_by_key(lvb_icp* const hs[2], KfRec& kf, const char* fn) {
+    const bool bk[2] = {!kf.pts[0] && kf.n[0] < 0, !kf.pts[1] && kf.n[1] < 0};
+    kf.pend[0] = kf.pend[1] = nullptr;
+    if (!bk[0] && !bk[1]) return LVB_OK;
+    if (!bk[0] || !bk[1]) { set_error("%s: keyframe %lld: give both clouds by key or neither", fn, kf.key); return LVB_ERR_INVALID; }
+    lvb_icp::Pending* pd[2];
+    for (int m = 0; m < 2; ++m) {
+        pd[m] = find_pending(hs[m], kf.key);
+        if (!pd[m]) { set_error("%s: key %lld has no pending features on the %s handle", fn, kf.key, m ? "surf" : "ground"); return LVB_ERR_INVALID; }
+    }
+    for (int m = 0; m < 2; ++m) { kf.pend[m] = pd[m]; kf.pts[m] = pd[m]->pts->p; kf.n[m] = pd[m]->n; }
     return LVB_OK;
 }
 
@@ -1718,12 +1783,11 @@ int lvb_icp_map_build_optimize_keyframe(lvb_icp* ground, lvb_icp* surf, const lo
                                         double rpyxyz[6], lvb_solve_summary summary[2], int n_map_points[2]) {
     static const char* fn = "lvb_icp_map_build_optimize_keyframe";
     lvb_icp* hs[2] = {ground, surf};
-    const void* pts[2] = {ground_pts, surf_pts};
-    const int ns[2] = {n_ground, n_surf};
     if (!ground || !surf || ground == surf || !cell_size || !map_pose || !p || !pose || !rpyxyz || n_keys < 0 || (n_keys && !keys)) {
         set_error("%s: null or bad argument", fn); return LVB_ERR_INVALID; }
-    LVB_TRY(kf_check_args(hs, cell_size, pts, ns, stride, p, fn));
-    KfRec kf = {key, keys, n_keys, {ground_pts, surf_pts}, {n_ground, n_surf}, map_pose, {}, {p->weight[0], p->weight[1]}, p->prior_weight};
+    KfRec kf = {key, keys, n_keys, {ground_pts, surf_pts}, {n_ground, n_surf}, {nullptr, nullptr}, map_pose, {}, {p->weight[0], p->weight[1]}, p->prior_weight};
+    LVB_TRY(resolve_by_key(hs, kf, fn));
+    LVB_TRY(kf_check_args(hs, cell_size, kf.pts, kf.n, stride, p, fn));
     memcpy(kf.pose, pose, sizeof(kf.pose));
     LVB_TRY(kf_chain(hs, &kf, 1, cell_size, ground_threshold, stride, p, fn));
     memcpy(pose, kf.pose, sizeof(kf.pose)); memcpy(rpyxyz, kf.rpyxyz, sizeof(kf.rpyxyz));
@@ -1743,22 +1807,18 @@ int lvb_icp_map_optimize_keyframes(lvb_icp* ground, lvb_icp* surf, lvb_map_keyfr
         LVB_TRY(kf_check_args(hs, cell_size, none, zero, stride, p, fn));
     }
     std::unordered_set<long long> batch;
+    std::vector<KfRec> rec(n_kf);
     for (int k = 0; k < n_kf; ++k) {
         const lvb_map_keyframe& kf = kfs[k];
-        const void* pts[2] = {kf.ground_pts, kf.surf_pts};
-        const int ns[2] = {kf.n_ground, kf.n_surf};
-        LVB_TRY(kf_check_args(hs, cell_size, pts, ns, stride, p, fn));
+        rec[k] = {kf.key, kf.map_keys, kf.n_map_keys, {kf.ground_pts, kf.surf_pts}, {kf.n_ground, kf.n_surf}, {nullptr, nullptr}, kf.map_pose, {},
+                  {kf.weight[0], kf.weight[1]}, kf.prior_weight};
+        memcpy(rec[k].pose, kf.pose, sizeof(kf.pose));
+        LVB_TRY(resolve_by_key(hs, rec[k], fn));
+        LVB_TRY(kf_check_args(hs, cell_size, rec[k].pts, rec[k].n, stride, p, fn));
         if (kf.n_map_keys < 0 || kf.n_map_keys > 3) { set_error("%s: keyframe %d has %d map keys (0 to 3)", fn, k, kf.n_map_keys); return LVB_ERR_INVALID; }
         if (!batch.insert(kf.key).second) { set_error("%s: key %lld is listed twice", fn, kf.key); return LVB_ERR_INVALID; }
     }
     if (n_kf == 0) return LVB_OK;
-    std::vector<KfRec> rec(n_kf);
-    for (int k = 0; k < n_kf; ++k) {
-        const lvb_map_keyframe& kf = kfs[k];
-        rec[k] = {kf.key, kf.map_keys, kf.n_map_keys, {kf.ground_pts, kf.surf_pts}, {kf.n_ground, kf.n_surf}, kf.map_pose, {},
-                  {kf.weight[0], kf.weight[1]}, kf.prior_weight};
-        memcpy(rec[k].pose, kf.pose, sizeof(kf.pose));
-    }
     LVB_TRY(kf_chain(hs, rec.data(), n_kf, cell_size, ground_threshold, stride, p, fn));
     for (int k = 0; k < n_kf; ++k) {
         lvb_map_keyframe& kf = kfs[k];
@@ -1804,7 +1864,7 @@ int lvb_icp_map_relocate(lvb_icp* ground, lvb_icp* surf, const long long* keys, 
     lvb::timing_mark(s, "begin");
     std::vector<KfUpload> uk;
     size_t back;
-    LVB_TRY(kf_upload(ctx, 1, false, pts, ns, stride, uk, back, [&](int, KfUpload& v) {
+    LVB_TRY(kf_upload(ctx, 1, false, pts, nullptr, ns, stride, uk, back, [&](int, KfUpload& v) {
         memcpy(v.hb->map_pose, map_pose, sizeof(v.hb->map_pose));
         memcpy(v.hb->pose, old_pose, sizeof(v.hb->pose));          // replaced on the device by old_pose * relative_guess
         memcpy(v.hb->old_pose, old_pose, sizeof(v.hb->old_pose)); memcpy(v.hb->rel, relative_guess, sizeof(v.hb->rel));
@@ -1818,7 +1878,7 @@ int lvb_icp_map_relocate(lvb_icp* ground, lvb_icp* surf, const long long* keys, 
     for (int m = 0; m < 2; ++m) saved[m].save(hs[m]);
     int rc = LVB_OK;
     ILAUNCH(ground, icp_reloc_pose_kernel, 1, 1, u.blk, 0);
-    for (int r = 0; r < rounds && rc == LVB_OK; ++r) rc = kf_register(hs, pl.build, maps, u, ns, stride, p);
+    for (int r = 0; r < rounds && rc == LVB_OK; ++r) rc = kf_register(hs, pl.build, maps, u, ns, p);
     if (rc == LVB_OK) ILAUNCH(ground, icp_reloc_pose_kernel, 1, 1, u.blk, 1);
     if (rc == LVB_OK) rc = icheck(fn);
     // the one read-back: solver states, pose, relative_o_c, scores, both map descriptors (grid, point count, failure)
@@ -1915,6 +1975,48 @@ int lvb_icp_map_to_world(lvb_icp* ground, lvb_icp* surf, const long long* keys, 
     LVB_TRY(host_sync(ctx, s));
     ctx->stage_busy = false;
     for (size_t i = 0; i < S; ++i) bbox_store(*segs[i], hbox + 6 * i);
+    return LVB_OK;
+}
+
+// ---- FeatureAssociation::Process (association.cpp:85-109) into the map handles: the keyframe's feature clouds stay on the device as
+// the pending features of `key`, which lvb_icp_map_optimize_keyframes / lvb_icp_map_build_optimize_keyframe register and store by key
+int lvb_icp_map_extract_keyframe(lvb_icp* ground, lvb_icp* surf, const lvb_lidar_config* cfg, long long key, const void* points, int n, int stride,
+                                 int32_t* n_ground, int32_t* n_surf, float* ground_xyzi, float* surf_xyzi) {
+    static const char* fn = "lvb_icp_map_extract_keyframe";
+    if (!ground || !surf || ground == surf || !n_ground || !n_surf) { set_error("%s: null or bad argument", fn); return LVB_ERR_INVALID; }
+    if (ground->ctx != surf->ctx) { set_error("%s: the two handles belong to different contexts", fn); return LVB_ERR_INVALID; }
+    DevBuf<float4> feat[2];
+    float box[12];
+    int32_t counts[2];
+    LVB_TRY(lidar_extract_keyframe(ground->ctx, cfg, points, n, stride, fn, feat[0], feat[1], &counts[0], &counts[1], box, ground_xyzi, surf_xyzi));
+    // The extraction buffers hold num_scans * horizon_scan records; a pending cloud becomes a resident keyframe's robot-frame cloud, so
+    // it keeps exactly its points, as a host cloud stored by the keyframe calls does (stream-ordered copy, no wait)
+    lvb_icp::Pending pd[2];
+    int rc = LVB_OK;
+    for (int m = 0; m < 2; ++m) {
+        pd[m].key = key; pd[m].n = counts[m]; pd[m].pts = new DevBuf<float4>();
+        for (int a = 0; a < 3; ++a) { pd[m].lo[a] = box[6 * m + a]; pd[m].hi[a] = box[6 * m + 3 + a]; }
+        if (rc == LVB_OK) rc = pd[m].pts->ensure(std::max(1, counts[m]));
+        if (rc == LVB_OK && counts[m] &&
+            cudaMemcpyAsync(pd[m].pts->p, feat[m].p, (size_t)counts[m] * sizeof(float4), cudaMemcpyDeviceToDevice, ground->ctx->stream) != cudaSuccess)
+            rc = lvb::cuda_fail(cudaGetLastError(), "pending copy", __FILE__, __LINE__);
+    }
+    if (rc != LVB_OK) { delete pd[0].pts; delete pd[1].pts; return rc; }
+    lvb_icp* hs[2] = {ground, surf};
+    for (int m = 0; m < 2; ++m) {
+        drop_pending(hs[m], key);              // a second extraction under the same key replaces the first
+        hs[m]->pending.push_back(pd[m]);
+    }
+    *n_ground = counts[0]; *n_surf = counts[1];
+    return LVB_OK;
+}
+
+int lvb_debug_icp_cloud_capacity(lvb_icp* h, long long key, long long cap[3]) {
+    if (!h || !cap) { set_error("null argument"); return LVB_ERR_INVALID; }
+    cap[0] = cap[1] = cap[2] = -1;
+    for (auto& sg : h->segments)
+        if (sg.key == key) { cap[0] = sg.pts ? (long long)sg.pts->n : -1; cap[1] = sg.robot ? (long long)sg.robot->n : -1; }
+    if (const lvb_icp::Pending* pd = find_pending(h, key)) cap[2] = (long long)pd->pts->n;
     return LVB_OK;
 }
 

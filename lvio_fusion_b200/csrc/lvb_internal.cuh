@@ -69,6 +69,14 @@ void timing_mark(cudaStream_t s, const char* name);
 // SegmentGround on a device cloud (lidar.cu): the inlier count stays on the device at n_out_dev (0 when n < 3 or no plane is found),
 // `out` holds n records; nothing is waited for
 int lidar_segment_ground_device_async(lvb_ctx* ctx, const float4* in, int n, double thr, float4* out, int* n_out_dev);
+template <class T> struct DevBuf;
+// FeatureAssociation::Process of one scan (lidar.cu), with one host synchronisation: the robot-frame feature clouds stay on the device in
+// ground / surf (*n_ground / *n_surf records), with box (may be NULL) their bounding boxes {min xyz, max xyz} x {ground, surf} (FLT_MAX /
+// -FLT_MAX when empty), and ground_xyzi / surf_xyzi (may be NULL) receive host copies.  Argument errors come before any work; a
+// voxel grid above 2^26 voxels is LVB_ERR_UNSUPPORTED after the synchronisation, with ground / surf untouched.  fn names the caller.
+int lidar_extract_keyframe(lvb_ctx* ctx, const lvb_lidar_config* cfg, const void* points, int n, int stride, const char* fn,
+                           DevBuf<float4>& ground, DevBuf<float4>& surf, int32_t* n_ground, int32_t* n_surf, float box[12],
+                           float* ground_xyzi, float* surf_xyzi);
 // every host wait on a context's stream goes through here and is counted in ctx->syncs (lvb_sync_count)
 int host_sync(lvb_ctx* ctx, cudaStream_t s);
 // The context's pinned staging area (lvb_ctx::stage_h), used by ba.cu (Stager) and icp.cu (lvb_icp_map_optimize_keyframe):
