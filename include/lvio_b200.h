@@ -198,6 +198,25 @@ LVB_API int lvb_imu_preintegrate(lvb_ctx* ctx, int n, const int32_t* first /* n+
 /* ---- lidar scan-to-map: stands behind pcl::KdTreeFLANN + FeatureAssociation::ScanToMapWith*
  * (association.cpp:270-384) and the two Solve calls of Mapping::Optimize (mapping.cpp:139-191) */
 LVB_API int lvb_icp_create(lvb_ctx* ctx, lvb_icp** out);
+/* A handle on ctx that shares `owner`'s resident keyframe clouds and pending features (its store); its map frames, relocation
+ * slot and scratch are its own.  ctx: any context on owner's device (typically another host thread's).  Sharing a shared handle
+ * shares the same store; lvb_icp_destroy of any handle, the owner included, leaves the store alive for the others (what a handle
+ * drops last is freed on its own context's stream).  lvb_icp_create makes a fresh, unshared store.
+ * Errors, before anything is created: LVB_ERR_INVALID for NULL arguments or a context on another device; LVB_ERR_UNSUPPORTED on a
+ * context with world_size > 1 (sharded stores stay per rank).
+ * Concurrency on one store, each handle on its own thread's context:
+ *   - read-only calls run concurrently from any thread's handles: lvb_icp_map_build, lvb_icp_map_relocate and the map keys of the
+ *     keyframe calls;
+ *   - lvb_icp_map_extract_keyframe runs concurrently too: it writes only the pending entry of its own key;
+ *   - calls that store, re-anchor or evict a key (the keyframe calls, lvb_icp_map_append, lvb_icp_map_to_world, lvb_icp_map_evict)
+ *     are serialised by the caller among themselves, as the reference's backend_->mutex does for Mapping::Optimize and ToWorld;
+ *   - each call sees every cloud as committed when it took its snapshot of the store (a writer commits after its synchronisation),
+ *     and the results are those of some serial order of the calls.  A by-key keyframe call sees the pending features committed
+ *     before it started, and otherwise fails with LVB_ERR_INVALID.
+ * On a shared store lvb_icp_map_to_world writes each re-anchored cloud into a new buffer and publishes it at its commit (a
+ * concurrent reader keeps the old one until it returns), and lvb_icp_map_extract_keyframe waits for its pending copies before it
+ * publishes them (one more host synchronisation).  An unshared store behaves as if sharing did not exist. */
+LVB_API int lvb_icp_share(lvb_ctx* ctx, lvb_icp* owner, lvb_icp** out);
 LVB_API void lvb_icp_destroy(lvb_icp* icp);
 /* KdTreeFLANN::setInputCloud (association.cpp:278-279,336-337).  points: n records of
  * stride_bytes (>= 12) whose first three floats are x,y,z -- 32 for pcl::PointXYZI, 16 for a
@@ -360,7 +379,8 @@ LVB_API int lvb_icp_map_optimize_keyframes(lvb_icp* ground, lvb_icp* surf, lvb_m
  * many points SegmentGround keeps.  A resident cloud without a recorded bounding box costs one more synchronisation, once.
  * Errors, all before any state changes: as lvb_icp_map_build_optimize_keyframe (unknown key, time limit set, sharded context), and
  * LVB_ERR_INVALID for n_keys outside 1..3, rounds outside 1..16 or prior_weight >= 0; failures found on the device (no finite bounding
- * box, grid overflow) leave every cloud and map frame as they were. */
+ * box, grid overflow) leave every cloud and map frame as they were.  Threading: read-only on the store; it may run on handles
+ * lvb_icp_share made (another thread's context) concurrently with any call on the same store (see lvb_icp_share). */
 LVB_API int lvb_icp_map_relocate(lvb_icp* ground, lvb_icp* surf, const long long* keys, int n_keys, const float cell_size[2],
                                  double ground_threshold, const double map_pose[7], const double old_pose[7], const double relative_guess[7],
                                  const void* ground_pts, int n_ground, const void* surf_pts, int n_surf, int stride_bytes,
@@ -377,7 +397,7 @@ LVB_API int lvb_icp_map_relocate(lvb_icp* ground, lvb_icp* surf, const long long
  * One pinned upload, one kernel over every point of every listed cloud, one host synchronisation, whatever n_keys is; n_keys == 0
  * launches and waits for nothing.  The bounding boxes of the new clouds are recorded, so the next lvb_icp_map_build_optimize_keyframe
  * or lvb_icp_map_relocate that merges them pays no extra synchronisation for them.
- * The world clouds are overwritten in place; nothing else changes: the handles' map frames (copies made by their builds), the
+ * The world clouds are overwritten in place (on a shared store: replaced by new buffers, see lvb_icp_share); nothing else changes: the handles' map frames (copies made by their builds), the
  * relocation slots, the scan lvb_icp_map_append(NULL) refers to and every cloud not listed stay as they were.  Nothing is exchanged
  * between ranks: the call is not collective on a sharded context.
  * Errors, all before any state changes: LVB_ERR_INVALID for an unknown or duplicated key, NULL keys / poses with n_keys > 0,
@@ -434,8 +454,8 @@ LVB_API int lvb_lidar_extract_features(lvb_ctx* ctx, const lvb_lidar_config* cfg
  * Errors, all before any state changes: LVB_ERR_INVALID for a bad configuration or cloud arguments (lvb_lidar_extract_features'),
  * NULL or equal handles, NULL n_ground / n_surf, handles of different contexts; a feature voxel grid above 2^26 voxels is
  * LVB_ERR_UNSUPPORTED, found on the device and reported after the synchronisation, storing nothing.  Not collective: allowed on a
- * sharded context.  Threading: as lvb_icp_map_relocate, the caller serialises it with the mapping thread's calls on these handles and
- * their context. */
+ * sharded context.  Threading: it may run on handles lvb_icp_share made (another thread's context) concurrently with the keyframe
+ * calls and relocations on the same store (see lvb_icp_share). */
 LVB_API int lvb_icp_map_extract_keyframe(lvb_icp* ground, lvb_icp* surf, const lvb_lidar_config* cfg, long long key,
                                          const void* points, int n, int stride_bytes,
                                          int32_t* n_ground, int32_t* n_surf,              /* out, always */

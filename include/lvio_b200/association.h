@@ -13,7 +13,9 @@
 //   frame->weights.lidar_ground / lidar_surf / visual,  frame->features_left.size()
 #pragma once
 #include <algorithm>
+#include <atomic>
 #include <cmath>
+#include <mutex>
 #include <type_traits>
 #include <unordered_map>
 #include <unordered_set>
@@ -59,14 +61,15 @@ public:
     // the scan's two feature clouds stay on the device as the pending features of `key`, and frame->feature_lidar->points_ground /
     // points_surf (which the caller has created; the Relocator and ToWorldKeyframes read them) receive the host copies.
     // OptimizeKeyframe(frame, keys, ...) and OptimizeKeyframes then register a pending key by key, with no upload; the other
-    // OptimizeKeyframe overload uses the host copies and drops the pending features first.  Threading: as RelocateKeyframe -- it runs
-    // on the handles that keep the resident map (the mapping thread's, once that thread has stored a keyframe) from whichever thread
-    // calls it, and the caller serialises it with that thread's device calls (INTEGRATION.md).  A keyframe call on other handles than
-    // the ones holding the pending features uses the host copies.  false: the call failed and changed nothing (lvb_last_error()).
+    // OptimizeKeyframe overload uses the host copies and drops the pending features first.  Threading: it runs on the calling thread's
+    // own handles over the resident store (StoreView), with no lock: the lidar callback extracts while the mapping thread registers
+    // and the Relocator relocates (INTEGRATION.md 3a).  Before the mapping thread has stored a keyframe the features go to the calling
+    // thread's own handles, and a keyframe call on other handles uses the host copies.  false: the call failed and changed nothing
+    // (lvb_last_error()).
     template <class Cloud, class FramePtr>
     bool ExtractKeyframe(long long key, const Cloud& points, FramePtr frame) {
-        Handles& h = resident_ ? *resident_ : handles_of_thread()[this];
-        if (!ensure_handles(h)) return false;
+        StoreView h;
+        if (!store_view(h)) return false;
         const size_t cap = (size_t)lidar_cfg_.num_scans * (size_t)lidar_cfg_.horizon_scan;
         extract_ground_.resize(cap); extract_surf_.resize(cap);
         int32_t ng = 0, ns = 0;
@@ -76,13 +79,15 @@ public:
             return false;
         unpack(extract_ground_, ng, frame->feature_lidar->points_ground);
         unpack(extract_surf_, ns, frame->feature_lidar->points_surf);
-        h.pending.insert(key);
+        std::lock_guard<std::mutex> lk(meta_);
+        h.meta->pending.insert(key);
         return true;
     }
     ~LVB_ASSOCIATION_CLASS() {                      // the calling thread's handles; another thread's go with that thread's context
-        auto& m = handles_of_thread();
-        auto it = m.find(this);
-        if (it != m.end()) { if (it->second.ground) lvb_icp_destroy(it->second.ground); if (it->second.surf) lvb_icp_destroy(it->second.surf); m.erase(it); }
+        for (auto* m : {&handles_of_thread(), &shared_of_thread()}) {
+            auto it = m->find(this);
+            if (it != m->end()) { if (it->second.ground) lvb_icp_destroy(it->second.ground); if (it->second.surf) lvb_icp_destroy(it->second.surf); m->erase(it); }
+        }
     }
 
     // association.cpp:270-326 : pitch/roll/z = para+1,+2,+5 ; gate d2 < 100 res^2 ; TrivialLoss ; PoseErrorRPZ prior
@@ -108,12 +113,15 @@ public:
         Handles& h = handles_of_thread()[this];
         if (!ensure_handles(h)) return false;
         resident_ = &h;
-        return store_keyframe(h, key, ground_robot, surf_robot, pose7);
+        return store_keyframe(h.ground, h.surf, h, key, ground_robot, surf_robot, pose7);
     }
     bool EvictKeyframe(long long key) {
         Handles& h = handles_of_thread()[this];
         if (!ensure_handles(h)) return false;
-        if (key < 0) h.keys.clear(); else h.keys.erase(key);
+        {
+            std::lock_guard<std::mutex> lk(meta_);
+            if (key < 0) h.keys.clear(); else h.keys.erase(key);
+        }
         return lvb_icp_map_evict(h.ground, key) == LVB_OK && lvb_icp_map_evict(h.surf, key) == LVB_OK;
     }
 
@@ -123,12 +131,12 @@ public:
     // clouds stay on the device, one host synchronisation for all of them); a lidar keyframe it has not stored (ToWorld(start) also
     // writes the window's keyframes) goes through AppendKeyframe; a frame without feature_lidar is skipped -- the reference stores
     // empty clouds for it, which no map frame ever merges.  A key listed twice is re-anchored once.  Like RelocateKeyframe this runs on
-    // the handles that keep the resident clouds, from whichever thread calls it, and the caller holds backend_->mutex
-    // (INTEGRATION.md 3a).  false: a library call failed (lvb_last_error()).
+    // the calling thread's own handles over the resident store; it writes, so the caller holds backend_->mutex, which serialises it
+    // with the mapping thread's keyframe calls (INTEGRATION.md 3a).  false: a library call failed (lvb_last_error()).
     template <class FramePtr>
     bool ToWorldKeyframes(const long long* keys, const FramePtr* frames, int n) {
-        Handles& h = resident_ ? *resident_ : handles_of_thread()[this];
-        if (!ensure_handles(h)) return false;
+        StoreView h;
+        if (!store_view(h)) return false;
         std::vector<long long> moved;
         std::vector<double> poses;
         std::unordered_set<long long> seen;
@@ -136,10 +144,15 @@ public:
         for (int i = 0; i < n; ++i) {
             const FramePtr& f = frames[i];
             if (!f->feature_lidar || !seen.insert(keys[i]).second) continue;
-            if (h.keys.count(keys[i])) {
+            bool held;
+            {
+                std::lock_guard<std::mutex> lk(meta_);
+                held = h.meta->keys.count(keys[i]) > 0;
+            }
+            if (held) {
                 moved.push_back(keys[i]);
                 poses.insert(poses.end(), f->pose.data(), f->pose.data() + 7);
-            } else if (!store_keyframe(h, keys[i], f->feature_lidar->points_ground, f->feature_lidar->points_surf, f->pose.data())) {
+            } else if (!store_keyframe(h.ground, h.surf, *h.meta, keys[i], f->feature_lidar->points_ground, f->feature_lidar->points_surf, f->pose.data())) {
                 ok = false;
             }
         }
@@ -189,8 +202,14 @@ public:
         lvb_icp* reg_s = h.surf_map ? h.surf : nullptr;
         lvb_solve_summary sums[2];
         lvb_solve_summary* out = summary ? summary : sums;
-        if (h.pending.erase(key)) {                 // this call stores the host copies: the pending features (and key's clouds) go first
+        bool was_pending;
+        {
+            std::lock_guard<std::mutex> lk(meta_);
+            was_pending = h.pending.erase(key) > 0;
+        }
+        if (was_pending) {                          // this call stores the host copies: the pending features (and key's clouds) go first
             if (lvb_icp_map_evict(h.ground, key) != LVB_OK || lvb_icp_map_evict(h.surf, key) != LVB_OK) return false;
+            std::lock_guard<std::mutex> lk(meta_);
             h.keys.erase(key);
         }
         if (reg_g || reg_s) {
@@ -204,11 +223,15 @@ public:
         }
         // ToWorld of a side that was not registered: the call above stores only the clouds of the handles it was given
         const double* pose = frame->pose.data();
-        h.keys.erase(key);                           // until both sides hold the keyframe's clouds again
+        {
+            std::lock_guard<std::mutex> lk(meta_);
+            h.keys.erase(key);                       // until both sides hold the keyframe's clouds again
+        }
         if (!reg_g && !(lvb_icp_map_evict(h.ground, key) == LVB_OK &&
                         lvb_icp_map_append(h.ground, key, assoc_detail::cloud_data(g, 0), (int)g.size(), stride, pose) == LVB_OK)) return false;
         if (!reg_s && !(lvb_icp_map_evict(h.surf, key) == LVB_OK &&
                         lvb_icp_map_append(h.surf, key, assoc_detail::cloud_data(s, 0), (int)s.size(), stride, pose) == LVB_OK)) return false;
+        std::lock_guard<std::mutex> lk(meta_);
         h.keys.insert(key);
         return true;
     }
@@ -233,16 +256,23 @@ public:
         lvb_solve_summary sums[2];
         double rpyxyz[6];
         int n_map[2];
-        const bool by_key = h.pending.count(key) > 0;          // ExtractKeyframe left the clouds on the device: NULL clouds, -1 points
+        bool by_key;                                           // ExtractKeyframe left the clouds on the device: NULL clouds, -1 points
+        {
+            std::lock_guard<std::mutex> lk(meta_);
+            by_key = h.pending.count(key) > 0;
+        }
         if (lvb_icp_map_build_optimize_keyframe(h.ground, h.surf, keys, n_keys, cells, ground_ransac_threshold, map_pose7, key,
                                                 by_key ? nullptr : assoc_detail::cloud_data(g, 0), by_key ? -1 : (int)g.size(),
                                                 by_key ? nullptr : assoc_detail::cloud_data(s, 0), by_key ? -1 : (int)s.size(), stride,
                                                 &p, frame->pose.data(), rpyxyz, summary ? summary : sums, n_map) != LVB_OK)
             return false;
-        h.pending.erase(key);
+        {
+            std::lock_guard<std::mutex> lk(meta_);
+            h.pending.erase(key);
+            h.keys.insert(key);
+        }
         h.ground_map = n_map[0] > 0; h.surf_map = n_map[1] > 0;
         h.resident = h.ground_map && h.surf_map;
-        h.keys.insert(key);
         resident_ = &h;
         return true;
     }
@@ -264,6 +294,7 @@ public:
         if (n <= 0) return true;
         std::vector<lvb_map_keyframe> recs(n);
         int stride = 0;
+        std::unique_lock<std::mutex> meta_lock(meta_);
         for (int k = 0; k < n; ++k) {
             const auto& g = frames[k]->feature_lidar->points_ground;
             const auto& s = frames[k]->feature_lidar->points_surf;
@@ -281,9 +312,11 @@ public:
             const lvb_map_optimize_params pk = MapOptimizeParams(frames[k]);      // each keyframe's own weights and prior weight
             r.weight[0] = pk.weight[0]; r.weight[1] = pk.weight[1]; r.prior_weight = pk.prior_weight;
         }
+        meta_lock.unlock();
         const lvb_map_optimize_params p = MapOptimizeParams(frames[0]);          // the options, gates and losses every keyframe shares
         const float cells[2] = {cell_of(resolution_ * resolution_ * 100), cell_of(resolution_ * resolution_ * 25)};
         if (lvb_icp_map_optimize_keyframes(h.ground, h.surf, recs.data(), n, cells, ground_ransac_threshold, stride, &p) != LVB_OK) return false;
+        meta_lock.lock();
         for (int k = 0; k < n; ++k) {
             const lvb_map_keyframe& r = recs[k];
             std::memcpy(frames[k]->pose.data(), r.pose, sizeof(r.pose));
@@ -293,6 +326,7 @@ public:
             h.keys.insert(keys[k]);
             h.pending.erase(keys[k]);
         }
+        meta_lock.unlock();
         // as OptimizeKeyframe(frame, keys, ...) leaves them after the last keyframe: that keyframe's map frames
         h.ground_map = recs[n - 1].n_map_points[0] > 0; h.surf_map = recs[n - 1].n_map_points[1] > 0;
         h.resident = h.ground_map && h.surf_map;
@@ -311,14 +345,13 @@ public:
     // or that is NaN (no accepted point), this returns 0 -- a rejected candidate -- so that `score - 20` (relocator.cpp:178) cannot
     // overflow; a sum below -1e9 is returned as -1e9 (the truncation of a larger one is undefined).  A failed library call also
     // returns 0 and leaves relative_o_c as it was (lvb_last_error() says why).
-    // The call runs on the handles that keep the resident map -- those of the thread that stored the keyframes (AppendKeyframe,
-    // OptimizeKeyframe) -- from whichever thread calls it: the caller serialises it with that thread's device calls
-    // (INTEGRATION.md 3a: Relocator::RelocateByPoints holds backend_->mutex, as Backend::Optimize does around Mapping::Optimize).
+    // The call runs on the calling thread's own handles over the resident store (StoreView), read-only and with no lock: the Relocator
+    // relocates its candidates while the mapping thread registers, as the reference does (INTEGRATION.md 3a).
     template <class FramePtr, class Pose>
     int RelocateKeyframe(FramePtr frame, const long long* keys, int n_keys, const double* map_pose7, const double* old_pose7, Pose& relative_o_c,
                          double ground_ransac_threshold, lvb_solve_summary* summary = nullptr) {
-        Handles& h = resident_ ? *resident_ : handles_of_thread()[this];
-        if (!ensure_handles(h)) return 0;
+        StoreView h;
+        if (!store_view(h)) return 0;
         const auto& g = frame->feature_lidar->points_ground;
         const auto& s = frame->feature_lidar->points_surf;
         const int stride = (int)sizeof(assoc_detail::cloud_data(g, 0)[0]);
@@ -380,16 +413,44 @@ private:
         dst.resize((size_t)n);
         for (int i = 0; i < n; ++i) { auto& q = dst[(size_t)i]; q.x = src[i].x; q.y = src[i].y; q.z = src[i].z; q.intensity = src[i].intensity; }
     }
-    // ToWorld of one keyframe into h: its two robot-frame clouds replace whatever h held under `key`
+    // ToWorld of one keyframe into the store of ground / surf, whose keys `meta` lists: its two robot-frame clouds replace whatever the
+    // store held under `key`
     template <class Cloud>
-    static bool store_keyframe(Handles& h, long long key, const Cloud& ground_robot, const Cloud& surf_robot, const double* pose7) {
+    bool store_keyframe(lvb_icp* ground, lvb_icp* surf, Handles& meta, long long key, const Cloud& ground_robot, const Cloud& surf_robot,
+                        const double* pose7) {
         const int stride = (int)sizeof(assoc_detail::cloud_data(ground_robot, 0)[0]);
-        h.keys.erase(key); h.pending.erase(key);
-        lvb_icp_map_evict(h.ground, key); lvb_icp_map_evict(h.surf, key);            // re-registering a keyframe (ToWorld(start)) replaces its clouds
-        if (lvb_icp_map_append(h.ground, key, assoc_detail::cloud_data(ground_robot, 0), (int)ground_robot.size(), stride, pose7) != LVB_OK ||
-            lvb_icp_map_append(h.surf, key, assoc_detail::cloud_data(surf_robot, 0), (int)surf_robot.size(), stride, pose7) != LVB_OK)
+        {
+            std::lock_guard<std::mutex> lk(meta_);
+            meta.keys.erase(key); meta.pending.erase(key);
+        }
+        lvb_icp_map_evict(ground, key); lvb_icp_map_evict(surf, key);                // re-registering a keyframe (ToWorld(start)) replaces its clouds
+        if (lvb_icp_map_append(ground, key, assoc_detail::cloud_data(ground_robot, 0), (int)ground_robot.size(), stride, pose7) != LVB_OK ||
+            lvb_icp_map_append(surf, key, assoc_detail::cloud_data(surf_robot, 0), (int)surf_robot.size(), stride, pose7) != LVB_OK)
             return false;
-        h.keys.insert(key);
+        std::lock_guard<std::mutex> lk(meta_);
+        meta.keys.insert(key);
+        return true;
+    }
+    // The handles a call on the resident store makes from the calling thread: on the thread that keeps the resident pair (or before
+    // there is one) the thread's own pair; on any other thread a pair lvb_icp_share made once for that thread, on its own context, from
+    // the resident pair.  meta: the Handles whose key sets describe that store (read and written under meta_).  The resident pair and
+    // its context belong to the thread that keeps it (thread_local), so that thread must outlive the other threads' calls, as the
+    // reference's mapping thread does; the shared pairs keep the clouds themselves alive.
+    struct StoreView { lvb_icp* ground; lvb_icp* surf; Handles* meta; };
+    bool store_view(StoreView& v) {
+        Handles& own = handles_of_thread()[this];
+        Handles* r = resident_.load();
+        if (!r || r == &own) {
+            if (!ensure_handles(own)) return false;
+            v.ground = own.ground; v.surf = own.surf; v.meta = &own;
+            return true;
+        }
+        lvb::Runtime& rt = lvb::Runtime::get();
+        if (!rt.ensure()) return false;
+        Handles& sh = shared_of_thread()[this];
+        if (!sh.ground && lvb_icp_share(rt.ctx, r->ground, &sh.ground) != LVB_OK) return false;
+        if (!sh.surf && lvb_icp_share(rt.ctx, r->surf, &sh.surf) != LVB_OK) return false;
+        v.ground = sh.ground; v.surf = sh.surf; v.meta = r;
         return true;
     }
     static bool ensure_handles(Handles& h) {
@@ -398,10 +459,27 @@ private:
         return (h.ground || lvb_icp_create(rt.ctx, &h.ground) == LVB_OK) && (h.surf || lvb_icp_create(rt.ctx, &h.surf) == LVB_OK);
     }
     static std::unordered_map<const void*, Handles>& handles_of_thread() { static thread_local std::unordered_map<const void*, Handles> m; return m; }
+    // the calling thread's handles shared from the resident pair (store_view); only their ground / surf members are used
+    static std::unordered_map<const void*, Handles>& shared_of_thread() { static thread_local std::unordered_map<const void*, Handles> m; return m; }
     double resolution_;
     lvb_lidar_config lidar_cfg_;
     std::vector<Packed> extract_ground_, extract_surf_;      // ExtractKeyframe's host copies, num_scans * horizon_scan records each
-    Handles* resident_ = nullptr;      // the handles that keep the resident keyframe clouds (RelocateKeyframe); map nodes do not move
+    // the class stays copyable: a copy takes the resident pointer and gets a mutex of its own
+    struct ResidentPtr {
+        std::atomic<Handles*> p{nullptr};
+        ResidentPtr() = default;
+        ResidentPtr(const ResidentPtr& o) : p(o.p.load()) {}
+        ResidentPtr& operator=(const ResidentPtr& o) { p = o.p.load(); return *this; }
+        ResidentPtr& operator=(Handles* h) { p = h; return *this; }
+        Handles* load() const { return p.load(); }
+    };
+    struct Mutex : std::mutex {
+        Mutex() = default;
+        Mutex(const Mutex&) : std::mutex() {}
+        Mutex& operator=(const Mutex&) { return *this; }
+    };
+    ResidentPtr resident_;             // the handles that keep the resident keyframe clouds (StoreView); map nodes do not move
+    Mutex meta_;                       // guards the key sets (keys, pending) of every Handles: other threads' calls read and write the resident one's
 };
 
 }  // namespace lvio_fusion

@@ -149,6 +149,7 @@ _LVB_ONLY = {
     "comm_unique_id": (C.c_int, [C.c_char_p]),
     "comm_init": (C.c_int, [VP, C.c_int, C.c_int, C.c_char_p]),
     "ba_set_schur_mode": (C.c_int, [VP, C.c_int]),
+    "icp_share": (C.c_int, [VP, VP, C.POINTER(VP)]),
     "icp_map_append": (C.c_int, [VP, C.c_longlong, VP, C.c_int, C.c_int, c_double_p]),
     "icp_map_evict": (C.c_int, [VP, C.c_longlong]),
     "icp_map_build": (C.c_int, [VP, C.POINTER(C.c_longlong), C.c_int, C.c_float, C.c_double, c_int_p]),

@@ -266,6 +266,18 @@ class FeatureAssociation:
         except Exception:
             pass
 
+    def share(self, ctx):
+        """A FeatureAssociation on `ctx` (another thread's context on the same device) over this one's resident keyframe clouds and
+        pending features (lvb_icp_share, CUDA library only); its map frames and relocation slot are its own.  relocate, the map keys
+        of the keyframe calls and LidarFeatures.extract_into on it run concurrently with the calls on this handle; calls that store,
+        re-anchor or evict keys stay serialised by the caller.  The store lives as long as any handle on it."""
+        fa = FeatureAssociation.__new__(FeatureAssociation)
+        fa.ctx, fa.api, fa.h = ctx, ctx.api, None
+        h = C.c_void_p()
+        self.api.check(self.api.icp_share(ctx.h, self.h, C.byref(h)), "icp_share")
+        fa.h = h
+        return fa
+
     @staticmethod
     def _cloud(points):
         pts = np.ascontiguousarray(points, dtype=np.float32)

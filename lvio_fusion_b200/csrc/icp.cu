@@ -15,8 +15,10 @@
 #include <math.h>
 #include <algorithm>
 #include <chrono>
+#include <condition_variable>
 #include <functional>
 #include <memory>
+#include <mutex>
 #include <stdlib.h>
 #include <string.h>
 #include <unordered_map>
@@ -724,6 +726,15 @@ __global__ void icp_map_keep_kernel(const MapDesc* built, const MapDesc* prev, M
 }  // namespace
 
 // ====================================================================================== host side
+// A resident cloud buffer, held by the store's table and by the calls that read it.  It is freed with cudaFreeAsync on the stream of
+// the call that drops the last reference (lvb::g_alloc_stream), not on the allocating handle's, whose context may be gone by then:
+// every holder drops its reference after its own synchronisation, or behind its own queued reads of the buffer.
+using Cloud = std::shared_ptr<DevBuf<float4>>;
+static Cloud new_cloud() {
+    return Cloud(new DevBuf<float4>(), [](DevBuf<float4>* b) { b->s = lvb::g_alloc_stream; delete b; });
+}
+struct IcpStore;
+
 struct lvb_icp {
     lvb_ctx* ctx = nullptr;
     bool have_map = false;
@@ -746,27 +757,67 @@ struct lvb_icp {
     // robot: the same records in the robot frame (x, y, z, intensity), kept so that lvb_icp_map_to_world can re-anchor the cloud
     // lo / hi: the cloud's bounding box (icp_bbox_kernel's), recorded by the calls that build map frames (kf_chain) and by
     // lvb_icp_map_to_world for the clouds they write, and computed by the former once for the others (has_bbox false)
+    // They live in the handle's store (IcpStore), which lvb_icp_share hands to other handles.
     struct Segment {
-        long long key; DevBuf<float4>* pts = nullptr; DevBuf<float4>* robot = nullptr; int n; bool has_bbox = false; float lo[3], hi[3];
-        void release() { delete pts; delete robot; pts = robot = nullptr; }
+        long long key; Cloud pts, robot; int n; bool has_bbox = false; float lo[3], hi[3];
+        void release() { pts.reset(); robot.reset(); }
     };
-    std::vector<Segment> segments;
+    std::shared_ptr<IcpStore> store;
     DevBuf<float4> merged, merged2;
     struct MapBufs { DevBuf<float4> sorted; DevBuf<int> cell_start, coarse; };      // a map frame's sorted cloud and voxel hash
     MapBufs nx;          // every build writes its map frame here; it is swapped in only when the build succeeded
     MapBufs reloc;       // lvb_icp_map_relocate's old map frame: reused by every relocation, never swapped in
     MapBufs chain;       // lvb_icp_map_optimize_keyframes builds its map frames into nx and this slot in turn
     int scan_n = 0, scan_stride = 0;          // the scan of the last upload_scan (reusable by lvb_icp_map_append)
-    const unsigned char* scan_dev = nullptr;  // where that scan lies: scan_raw, or this handle's part of kf_arena
+    const unsigned char* scan_dev = nullptr;  // where that scan lies: scan_raw, this handle's part of kf_arena, or scan_cloud
+    Cloud scan_cloud;                         // the stored robot-frame cloud of a by-key keyframe when the scan is that cloud
     // the keyframe calls' upload (kf_upload: blocks, links, scans) in one allocation, held by both handles of the call
     // so that either one's scan stays valid for lvb_icp_map_append(NULL) until that handle uploads another scan
     std::shared_ptr<DevBuf<unsigned char>> kf_arena;
     // lvb_icp_map_extract_keyframe's robot-frame feature cloud of a keyframe not yet stored (pending features): packed (x, y, z,
     // intensity) records and their bounding box.  The keyframe calls register it by key and store it as the keyframe's robot cloud.
-    struct Pending { long long key; DevBuf<float4>* pts = nullptr; int n; float lo[3], hi[3]; };
-    std::vector<Pending> pending;
-    ~lvb_icp() { for (auto& sg : segments) sg.release(); for (auto& pd : pending) delete pd.pts; }
+    struct Pending { long long key; Cloud pts; int n; float lo[3], hi[3]; };
+    ~lvb_icp();
 };
+
+// The resident keyframe clouds and the pending features, shared by the handles lvb_icp_share makes from one lvb_icp_create.  `mu`
+// guards the two tables and their metadata (references, counts, boxes) and is never held across device work or a synchronisation:
+// a call that reads clouds copies the entries it needs (taking references to the buffers) and unlocks; a call that writes publishes
+// its entries after its synchronisation, so that a reader only ever sees clouds whose device writes are complete.
+struct IcpStore {
+    std::mutex mu;
+    std::vector<lvb_icp::Segment> segments;
+    std::vector<lvb_icp::Pending> pending;
+    int handles = 0;                 // the handles on this store
+    // lvb_icp_map_to_world overwrites the world clouds of an unshared store in place; lvb_icp_share waits until it has committed
+    // (`cv`), so that no handle can read a cloud while it is being overwritten
+    bool in_place = false;
+    std::condition_variable cv;
+};
+lvb_icp::~lvb_icp() {
+    if (!store) return;
+    std::lock_guard<std::mutex> lk(store->mu);
+    --store->handles;
+}
+
+// The store mutexes of a call's handles (either may be NULL; two handles on one store lock it once), taken together
+struct StoreLock {
+    std::unique_lock<std::mutex> a, b;
+    StoreLock(const lvb_icp* g, const lvb_icp* s) {
+        IcpStore* x = g ? g->store.get() : nullptr;
+        IcpStore* y = s ? s->store.get() : nullptr;
+        if (x == y || !x) { x = x ? x : y; y = nullptr; }
+        if (x && y) {
+            a = std::unique_lock<std::mutex>(x->mu, std::defer_lock); b = std::unique_lock<std::mutex>(y->mu, std::defer_lock);
+            std::lock(a, b);
+        } else if (x) a = std::unique_lock<std::mutex>(x->mu);
+    }
+};
+// the entry of `key` (the store's mutex held), or NULL
+static lvb_icp::Segment* find_segment(IcpStore& st, long long key) {
+    for (auto& sg : st.segments) if (sg.key == key) return &sg;
+    return nullptr;
+}
 
 #define ILAUNCH(h, kernel, grid, block, ...)                                              \
     do { if ((grid) > 0) { kernel<<<(grid), (block), 0, (h)->ctx->stream>>>(__VA_ARGS__); (h)->ctx->launches++; lvb::timing_mark((h)->ctx->stream, #kernel); } } while (0)
@@ -843,7 +894,7 @@ static int upload_scan(lvb_icp* h, const void* scan, int n, int stride, const do
     if (n < 0 || stride < 12 || (stride & 3) || (n && !scan)) { set_error("bad scan arguments"); return LVB_ERR_INVALID; }
     cudaStream_t s = h->ctx->stream;
     LVB_TRY(h->scan_raw.upload((const unsigned char*)scan, (size_t)n * stride, s));
-    h->kf_arena.reset();
+    h->kf_arena.reset(); h->scan_cloud.reset();
     lvb_icp::Frame f;
     f.map = h->map;
     for (int i = 0; i < 7; ++i) f.tf[i] = (float)frame_pose[i];
@@ -925,22 +976,25 @@ static int build_map(lvb_icp* h, const unsigned char* d_points, int n, int strid
 }
 
 // A cloud stored by a by-key keyframe call keeps the pending buffer as its robot-frame records, and the scan lvb_icp_map_append(NULL)
-// refers to may be that buffer: it goes with the cloud.
-static void release_segment(lvb_icp* h, lvb_icp::Segment& sg) {
-    if (sg.robot && h->scan_dev == reinterpret_cast<const unsigned char*>(sg.robot->p)) { h->scan_n = 0; h->scan_dev = nullptr; }
+// refers to may be that buffer: it goes with the cloud when h drops it.  The table's references move into `drop`, which the caller
+// releases after unlocking the store.
+static void release_segment(lvb_icp* h, lvb_icp::Segment& sg, std::vector<lvb_icp::Segment>& drop) {
+    if (sg.robot && h->scan_dev == reinterpret_cast<const unsigned char*>(sg.robot->p)) { h->scan_n = 0; h->scan_dev = nullptr; h->scan_cloud.reset(); }
+    drop.push_back(sg);
     sg.release();
 }
-static lvb_icp::Pending* find_pending(lvb_icp* h, long long key) {
-    for (auto& pd : h->pending) if (pd.key == key) return &pd;
+// the pending features of `key` (the store's mutex held), or NULL
+static lvb_icp::Pending* find_pending(IcpStore& st, long long key) {
+    for (auto& pd : st.pending) if (pd.key == key) return &pd;
     return nullptr;
 }
-// drop the pending features of `key` (key < 0: all)
-static void drop_pending(lvb_icp* h, long long key) {
+// drop the pending features of `key` (key < 0: all) into `drop` (the store's mutex held)
+static void drop_pending(IcpStore& st, long long key, std::vector<lvb_icp::Pending>& drop) {
     size_t w = 0;
-    for (size_t i = 0; i < h->pending.size(); ++i) {
-        if (key < 0 || h->pending[i].key == key) delete h->pending[i].pts; else h->pending[w++] = h->pending[i];
+    for (size_t i = 0; i < st.pending.size(); ++i) {
+        if (key < 0 || st.pending[i].key == key) drop.push_back(st.pending[i]); else st.pending[w++] = st.pending[i];
     }
-    h->pending.resize(w);
+    st.pending.resize(w);
 }
 
 extern "C" {
@@ -949,10 +1003,37 @@ int lvb_icp_create(lvb_ctx* ctx, lvb_icp** out) {
     if (!ctx || !out) { set_error("null argument"); return LVB_ERR_INVALID; }
     lvb_icp* h = new lvb_icp();
     h->ctx = ctx;
+    h->store = std::make_shared<IcpStore>();
+    h->store->handles = 1;
     *out = h;
     return LVB_OK;
 }
-void lvb_icp_destroy(lvb_icp* icp) { if (icp) { cudaSetDevice(icp->ctx->device); delete icp; } }
+
+int lvb_icp_share(lvb_ctx* ctx, lvb_icp* owner, lvb_icp** out) {
+    if (!ctx || !owner || !out) { set_error("lvb_icp_share: null argument"); return LVB_ERR_INVALID; }
+    if (ctx->device != owner->ctx->device) {
+        set_error("lvb_icp_share: the context is on device %d, the store on device %d", ctx->device, owner->ctx->device); return LVB_ERR_INVALID; }
+    if (ctx->world > 1 || owner->ctx->world > 1) { set_error("lvb_icp_share: sharded contexts keep their stores per rank"); return LVB_ERR_UNSUPPORTED; }
+    lvb_icp* h = new lvb_icp();
+    h->ctx = ctx;
+    h->store = owner->store;
+    {
+        std::unique_lock<std::mutex> lk(h->store->mu);
+        h->store->cv.wait(lk, [&] { return !h->store->in_place; });
+        ++h->store->handles;
+    }
+    *out = h;
+    return LVB_OK;
+}
+// The store outlives the handle while another handle holds it; what this handle drops is freed on its context's stream.
+void lvb_icp_destroy(lvb_icp* icp) {
+    if (!icp) return;
+    cudaSetDevice(icp->ctx->device);
+    const cudaStream_t prev = lvb::g_alloc_stream;
+    lvb::g_alloc_stream = icp->ctx->stream;
+    delete icp;
+    lvb::g_alloc_stream = prev;
+}
 
 int lvb_icp_set_map(lvb_icp* h, const void* points, int n, int stride, float cell_size) {
     if (n <= 0 || !points || stride < 12 || (stride & 3) || !(cell_size > 0.0f)) { set_error("bad map arguments"); return LVB_ERR_INVALID; }
@@ -979,8 +1060,11 @@ int lvb_icp_map_append(lvb_icp* h, long long key, const void* robot_points, int 
         if (h->scan_n <= 0) { set_error("lvb_icp_map_append: no scan on the device"); return LVB_ERR_STATE; }
         n = h->scan_n; stride = h->scan_stride; src = h->scan_dev;
     }
-    for (auto& sg : h->segments) if (sg.key == key) { set_error("lvb_icp_map_append: key %lld exists", key); return LVB_ERR_INVALID; }
-    lvb_icp::Segment sg; sg.key = key; sg.n = n; sg.pts = new DevBuf<float4>(); sg.robot = new DevBuf<float4>();
+    {
+        std::lock_guard<std::mutex> lk(h->store->mu);
+        if (find_segment(*h->store, key)) { set_error("lvb_icp_map_append: key %lld exists", key); return LVB_ERR_INVALID; }
+    }
+    lvb_icp::Segment sg; sg.key = key; sg.n = n; sg.pts = new_cloud(); sg.robot = new_cloud();
     int rc = sg.pts->ensure(std::max(1, n));
     if (rc == LVB_OK) rc = sg.robot->ensure(std::max(1, n));
     DevBuf<float> d_tf;
@@ -991,19 +1075,24 @@ int lvb_icp_map_append(lvb_icp* h, long long key, const void* robot_points, int 
     rc = icheck("map_append");
     if (rc != LVB_OK) { sg.release(); return rc; }
     LVB_TRY(host_sync(h->ctx, s));
-    h->segments.push_back(sg);
+    std::lock_guard<std::mutex> lk(h->store->mu);
+    h->store->segments.push_back(sg);
     return LVB_OK;
 }
 
 int lvb_icp_map_evict(lvb_icp* h, long long key) {
     if (!h) { set_error("null argument"); return LVB_ERR_INVALID; }
     LVB_CUDA(cudaSetDevice(h->ctx->device)); lvb::g_alloc_stream = h->ctx->stream;
+    std::vector<lvb_icp::Segment> drop;           // released after the store is unlocked
+    std::vector<lvb_icp::Pending> drop_pd;
+    std::lock_guard<std::mutex> lk(h->store->mu);
+    auto& segs = h->store->segments;
     size_t w = 0;
-    for (size_t i = 0; i < h->segments.size(); ++i) {
-        if (key < 0 || h->segments[i].key == key) release_segment(h, h->segments[i]); else h->segments[w++] = h->segments[i];
+    for (size_t i = 0; i < segs.size(); ++i) {
+        if (key < 0 || segs[i].key == key) release_segment(h, segs[i], drop); else segs[w++] = segs[i];
     }
-    h->segments.resize(w);
-    drop_pending(h, key);
+    segs.resize(w);
+    drop_pending(*h->store, key, drop_pd);
     return LVB_OK;
 }
 
@@ -1013,18 +1102,20 @@ int lvb_icp_map_build(lvb_icp* h, const long long* keys, int n_keys, float cell_
     LVB_CUDA(cudaSetDevice(ctx->device)); lvb::g_alloc_stream = ctx->stream;
     cudaStream_t s = ctx->stream;
     size_t total = 0;
-    std::vector<const lvb_icp::Segment*> pick;
-    for (int k = 0; k < n_keys; ++k) {
-        const lvb_icp::Segment* f = nullptr;
-        for (auto& sg : h->segments) if (sg.key == keys[k]) f = &sg;
-        if (!f) { set_error("lvb_icp_map_build: key %lld is not resident", keys[k]); return LVB_ERR_INVALID; }
-        pick.push_back(f); total += f->n;
+    std::vector<lvb_icp::Segment> pick;           // the call's snapshot: references to the clouds it merges
+    {
+        std::lock_guard<std::mutex> lk(h->store->mu);
+        for (int k = 0; k < n_keys; ++k) {
+            const lvb_icp::Segment* f = find_segment(*h->store, keys[k]);
+            if (!f) { set_error("lvb_icp_map_build: key %lld is not resident", keys[k]); return LVB_ERR_INVALID; }
+            pick.push_back(*f); total += f->n;
+        }
     }
     if (total == 0 || total > 0x7fffffffull) { set_error("lvb_icp_map_build: %zu points", total); return LVB_ERR_INVALID; }
     // points_*_merged += pointclouds_*[time] in key order (mapping.cpp:121-125): the position in the merged cloud is the point's index
     LVB_TRY(h->merged.ensure(total));
     size_t off = 0;
-    for (auto* f : pick) { if (f->n) LVB_CUDA(cudaMemcpyAsync(h->merged.p + off, f->pts->p, (size_t)f->n * sizeof(float4), cudaMemcpyDeviceToDevice, s)); off += f->n; }
+    for (auto& f : pick) { if (f.n) LVB_CUDA(cudaMemcpyAsync(h->merged.p + off, f.pts->p, (size_t)f.n * sizeof(float4), cudaMemcpyDeviceToDevice, s)); off += f.n; }
     const float4* cloud = h->merged.p;
     const int n = (int)total;
     const bool ransac = ground_threshold > 0.0;
@@ -1268,7 +1359,7 @@ static int kf_register(lvb_icp* const hs[2], const bool run[2], const KfMap maps
 static int kf_to_world(lvb_icp* const hs[2], const KfUpload& u, const int ns[2], bool boxes, lvb_icp::Segment fresh[2]) {
     for (int m = 0; m < 2; ++m) {
         if (!hs[m]) continue;
-        fresh[m].key = -1; fresh[m].n = ns[m]; fresh[m].pts = new DevBuf<float4>(); fresh[m].robot = u.by_key[m] ? nullptr : new DevBuf<float4>();
+        fresh[m].key = -1; fresh[m].n = ns[m]; fresh[m].pts = new_cloud(); fresh[m].robot = u.by_key[m] ? nullptr : new_cloud();
         int rc = fresh[m].pts->ensure(std::max(1, ns[m]));
         if (rc == LVB_OK && fresh[m].robot) rc = fresh[m].robot->ensure(std::max(1, ns[m]));
         if (rc != LVB_OK) { fresh[0].release(); fresh[1].release(); return rc; }
@@ -1278,11 +1369,11 @@ static int kf_to_world(lvb_icp* const hs[2], const KfUpload& u, const int ns[2],
     return LVB_OK;
 }
 
-// replace the cloud under `key` with sg, or add it
-static void store_segment(lvb_icp* h, long long key, lvb_icp::Segment& sg) {
+// replace the cloud under `key` with sg, or add it (the store's mutex held; the replaced references go to `drop`)
+static void store_segment(lvb_icp* h, long long key, lvb_icp::Segment& sg, std::vector<lvb_icp::Segment>& drop) {
     sg.key = key;
-    for (auto& old : h->segments) if (old.key == key) { release_segment(h, old); old = sg; return; }
-    h->segments.push_back(sg);
+    if (lvb_icp::Segment* old = find_segment(*h->store, key)) { release_segment(h, *old, drop); *old = sg; return; }
+    h->store->segments.push_back(sg);
 }
 
 // Mapping::Optimize for one keyframe (mapping.cpp:147-185, after BuildMapFrame) against the map frames lvb_icp_map_build made, with
@@ -1330,11 +1421,15 @@ int lvb_icp_map_optimize_keyframe(lvb_icp* ground, lvb_icp* surf, const double m
     LVB_TRY(kf_to_world(hs, u, ns, false, fresh));
     int rc = icheck("map_optimize_keyframe");
     if (rc != LVB_OK) { fresh[0].release(); fresh[1].release(); return rc; }
-    for (int m = 0; m < 2; ++m) if (hs[m]) store_segment(hs[m], key, fresh[m]);
-    // the one read-back: both solver states, rpyxyz and the pose
+    // the one read-back: both solver states, rpyxyz and the pose; the clouds are published once it has run
     LVB_CUDA(cudaMemcpyAsync(u.hb, u.blk, back, cudaMemcpyDeviceToHost, s));
     LVB_TRY(host_sync(ctx, s));
     ctx->stage_busy = false;
+    {
+        std::vector<lvb_icp::Segment> drop;
+        StoreLock lk(ground, surf);
+        for (int m = 0; m < 2; ++m) if (hs[m]) store_segment(hs[m], key, fresh[m], drop);
+    }
     const double el = std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
     memcpy(pose, u.hb->pose, sizeof(u.hb->pose)); memcpy(rpyxyz, u.hb->rpyxyz, sizeof(u.hb->rpyxyz));
     if (summary) {
@@ -1354,11 +1449,13 @@ static void bbox_store(lvb_icp::Segment& sg, const int* b) {
     sg.has_bbox = true;
 }
 
-// Clouds stored by lvb_icp_map_append / lvb_icp_map_optimize_keyframe carry no bounding box: compute those of `segs` (of any handle
-// on h's context) once, all with one host synchronisation, and keep them with the segments.
-static int fill_bboxes(lvb_icp* h, const std::vector<lvb_icp::Segment*>& segs) {
+// Clouds stored by lvb_icp_map_append / lvb_icp_map_optimize_keyframe carry no bounding box: compute those of `segs` (a call's
+// snapshot of clouds of any handle on h's context; segs[i] is an entry of stores[i]) once, all with one host synchronisation, and
+// record them in the snapshot and in the stores, for the entries that still hold the same cloud.
+static int fill_bboxes(lvb_icp* h, const std::vector<lvb_icp::Segment*>& segs, const std::vector<IcpStore*>& stores) {
     std::vector<lvb_icp::Segment*> todo;
-    for (auto* sg : segs) if (!sg->has_bbox) todo.push_back(sg);
+    std::vector<IcpStore*> todo_st;
+    for (size_t i = 0; i < segs.size(); ++i) if (!segs[i]->has_bbox) { todo.push_back(segs[i]); todo_st.push_back(stores[i]); }
     if (todo.empty()) return LVB_OK;
     lvb_ctx* ctx = h->ctx;
     cudaStream_t s = ctx->stream;
@@ -1375,7 +1472,12 @@ static int fill_bboxes(lvb_icp* h, const std::vector<lvb_icp::Segment*>& segs) {
     LVB_TRY(icheck("map frame bounding boxes"));
     LVB_CUDA(cudaMemcpyAsync(hb, d.p, bytes, cudaMemcpyDeviceToHost, s));
     LVB_TRY(host_sync(ctx, s));
-    for (size_t i = 0; i < todo.size(); ++i) bbox_store(*todo[i], hb[i].bbox);
+    for (size_t i = 0; i < todo.size(); ++i) {
+        bbox_store(*todo[i], hb[i].bbox);
+        std::lock_guard<std::mutex> lk(todo_st[i]->mu);
+        lvb_icp::Segment* e = find_segment(*todo_st[i], todo[i]->key);
+        if (e && e->pts == todo[i]->pts) bbox_store(*e, hb[i].bbox);
+    }
     return LVB_OK;
 }
 
@@ -1402,10 +1504,23 @@ static MapBound map_bound(const float* lo, const float* hi, float cell_size) {
     return b;
 }
 
-// A map key's clouds: the ones keyframe kf of the call stores (kf >= 0), else the ones resident on both handles (seg)
+// A map key's clouds: the ones keyframe kf of the call stores (kf >= 0), else the ones resident on both handles (seg: entries of the
+// call's snapshot)
 struct KfSrc { int kf; lvb_icp::Segment* seg[2]; };
-static bool find_resident(lvb_icp* const hs[2], long long key, KfSrc& sr) {
-    for (int m = 0; m < 2; ++m) { sr.seg[m] = nullptr; for (auto& sg : hs[m]->segments) if (sg.key == key) sr.seg[m] = &sg; }
+// The resident clouds a call reads, per side: copies of the store entries (references to the clouds), taken under the stores' mutexes
+// (StoreLock) and kept until the call's synchronisation.  Node-based: the entries do not move.
+struct Snapshot { std::unordered_map<long long, lvb_icp::Segment> seg[2]; };
+static bool find_resident(lvb_icp* const hs[2], Snapshot& snap, long long key, KfSrc& sr) {
+    for (int m = 0; m < 2; ++m) {
+        sr.seg[m] = nullptr;
+        auto it = snap.seg[m].find(key);
+        if (it == snap.seg[m].end()) {
+            const lvb_icp::Segment* e = find_segment(*hs[m]->store, key);
+            if (!e) continue;
+            it = snap.seg[m].emplace(key, *e).first;
+        }
+        sr.seg[m] = &it->second;
+    }
     return sr.seg[0] && sr.seg[1];
 }
 
@@ -1420,7 +1535,7 @@ struct KfPlan { std::vector<lvb_icp::Segment*> pick[2]; size_t total[2] = {0, 0}
 struct KfRec {
     long long key; const long long* map_keys; int n_map_keys;
     const void* pts[2]; int n[2];                 // the robot-frame clouds: ground, surf
-    lvb_icp::Pending* pend[2];                    // by key: the pending features of `key` on each handle (pts unused), else NULL
+    lvb_icp::Pending pend[2];                     // by key: the pending features of `key` on each handle (a copy of the entry), else empty
     const double* map_pose;
     double pose[7];                               // in: frame->pose; out: optimised
     double weight[2], prior_weight;
@@ -1433,7 +1548,8 @@ struct KfRec {
 static int plan_frames(lvb_icp* const hs[2], const std::vector<std::vector<KfSrc>>& srcs, const KfRec* kfs, lvb_icp::Segment* stage,
                        const float cell_size[2], bool ransac, const char* fn, std::vector<KfPlan>& pl) {
     pl.assign(srcs.size(), KfPlan());
-    std::vector<lvb_icp::Segment*> res;           // the resident clouds, each once
+    std::vector<lvb_icp::Segment*> res;           // the resident clouds, each once, and their stores
+    std::vector<IcpStore*> res_st;
     std::unordered_set<lvb_icp::Segment*> seen;
     for (size_t k = 0; k < srcs.size(); ++k) {
         KfPlan& q = pl[k];
@@ -1441,7 +1557,7 @@ static int plan_frames(lvb_icp* const hs[2], const std::vector<std::vector<KfSrc
             for (int m = 0; m < 2; ++m) {
                 if (sr.kf >= 0) { q.pick[m].push_back(&stage[2 * (size_t)sr.kf + m]); q.total[m] += kfs[sr.kf].n[m]; continue; }
                 q.pick[m].push_back(sr.seg[m]); q.total[m] += sr.seg[m]->n;
-                if (seen.insert(sr.seg[m]).second) res.push_back(sr.seg[m]);
+                if (seen.insert(sr.seg[m]).second) { res.push_back(sr.seg[m]); res_st.push_back(hs[m]->store.get()); }
             }
         }
         for (int m = 0; m < 2; ++m) {
@@ -1450,7 +1566,7 @@ static int plan_frames(lvb_icp* const hs[2], const std::vector<std::vector<KfSrc
             q.seed[m] = desc_seed(q.build[m] && !(m == 0 && ransac) ? (int)q.total[m] : 0);      // the ground count comes from SegmentGround
         }
     }
-    LVB_TRY(fill_bboxes(hs[0], res));
+    LVB_TRY(fill_bboxes(hs[0], res, res_st));
     for (size_t k = 0; k < srcs.size(); ++k) {
         KfPlan& q = pl[k];
         for (int m = 0; m < 2; ++m) {
@@ -1500,9 +1616,9 @@ static int kf_build(lvb_icp* h, const KfPlan& pl, int m, float cell_size, double
 
 // The scan a handle's lvb_icp_map_append(NULL) refers to (bind_scan moves it to the registration's scan)
 struct ScanState {
-    int n, stride; const unsigned char* dev; std::shared_ptr<DevBuf<unsigned char>> arena;
-    void save(const lvb_icp* h) { n = h->scan_n; stride = h->scan_stride; dev = h->scan_dev; arena = h->kf_arena; }
-    void restore(lvb_icp* h) const { h->scan_n = n; h->scan_stride = stride; h->scan_dev = dev; h->kf_arena = arena; }
+    int n, stride; const unsigned char* dev; std::shared_ptr<DevBuf<unsigned char>> arena; Cloud cloud;
+    void save(const lvb_icp* h) { n = h->scan_n; stride = h->scan_stride; dev = h->scan_dev; arena = h->kf_arena; cloud = h->scan_cloud; }
+    void restore(lvb_icp* h) const { h->scan_n = n; h->scan_stride = stride; h->scan_dev = dev; h->kf_arena = arena; h->scan_cloud = cloud; }
 };
 
 // The argument checks of the calls that build map frames; they come before any state changes
@@ -1585,17 +1701,21 @@ static lvb_map_optimize_params kf_params(const lvb_map_optimize_params& p, const
 // the records' outputs written, only when every keyframe succeeded.  The callers have checked the arguments (kf_check_args).
 static int kf_chain(lvb_icp* const hs[2], KfRec* kfs, int n_kf, const float cell_size[2], double ground_threshold, int stride,
                     const lvb_map_optimize_params* p, const char* fn) {
-    // each map key: the cloud an earlier keyframe of the call stores, else the resident one of both handles
+    // each map key: the cloud an earlier keyframe of the call stores, else the resident one of both handles (one snapshot for all)
     std::vector<std::vector<KfSrc>> srcs(n_kf);
-    for (int k = 0; k < n_kf; ++k) {
-        for (int i = 0; i < kfs[k].n_map_keys; ++i) {
-            const long long mk = kfs[k].map_keys[i];
-            if (mk == kfs[k].key) { set_error("%s: key %lld is its own map key", fn, mk); return LVB_ERR_INVALID; }
-            KfSrc sr = {-1, {nullptr, nullptr}};
-            for (int j = 0; j < k; ++j) if (kfs[j].key == mk) sr.kf = j;
-            if (sr.kf < 0 && !find_resident(hs, mk, sr)) {
-                set_error("%s: map key %lld of keyframe %d is neither resident nor an earlier keyframe of the call", fn, mk, k); return LVB_ERR_INVALID; }
-            srcs[k].push_back(sr);
+    Snapshot snap;
+    {
+        StoreLock lk(hs[0], hs[1]);
+        for (int k = 0; k < n_kf; ++k) {
+            for (int i = 0; i < kfs[k].n_map_keys; ++i) {
+                const long long mk = kfs[k].map_keys[i];
+                if (mk == kfs[k].key) { set_error("%s: key %lld is its own map key", fn, mk); return LVB_ERR_INVALID; }
+                KfSrc sr = {-1, {nullptr, nullptr}};
+                for (int j = 0; j < k; ++j) if (kfs[j].key == mk) sr.kf = j;
+                if (sr.kf < 0 && !find_resident(hs, snap, mk, sr)) {
+                    set_error("%s: map key %lld of keyframe %d is neither resident nor an earlier keyframe of the call", fn, mk, k); return LVB_ERR_INVALID; }
+                srcs[k].push_back(sr);
+            }
         }
     }
     lvb_ctx* ctx = hs[0]->ctx;
@@ -1626,7 +1746,7 @@ static int kf_chain(lvb_icp* const hs[2], KfRec* kfs, int n_kf, const float cell
                 const size_t e = 2 * (size_t)sr.kf + m;
                 if (!have_est[e]) {
                     const KfRec& src = kfs[sr.kf];
-                    if (src.pend[m]) world_box(src.pend[m]->lo, src.pend[m]->hi, src.pose, &est[6 * e], &est[6 * e + 3]);
+                    if (src.pend[m].pts) world_box(src.pend[m].lo, src.pend[m].hi, src.pose, &est[6 * e], &est[6 * e + 3]);
                     else in_call_box(src.pts[m], src.n[m], stride, src.pose, &est[6 * e], &est[6 * e + 3]);
                     have_est[e] = 1;
                 }
@@ -1650,7 +1770,7 @@ static int kf_chain(lvb_icp* const hs[2], KfRec* kfs, int n_kf, const float cell
     std::vector<const float4*> dev(2 * (size_t)n_kf);
     std::vector<int> ns(2 * (size_t)n_kf);
     for (int k = 0; k < n_kf; ++k)
-        for (int m = 0; m < 2; ++m) { pts[2 * k + m] = kfs[k].pts[m]; dev[2 * k + m] = kfs[k].pend[m] ? kfs[k].pend[m]->pts->p : nullptr; ns[2 * k + m] = kfs[k].n[m]; }
+        for (int m = 0; m < 2; ++m) { pts[2 * k + m] = kfs[k].pts[m]; dev[2 * k + m] = kfs[k].pend[m].pts ? kfs[k].pend[m].pts->p : nullptr; ns[2 * k + m] = kfs[k].n[m]; }
     std::vector<KfUpload> u;
     size_t back;
     LVB_TRY(kf_upload(ctx, n_kf, true, pts.data(), dev.data(), ns.data(), stride, u, back, [&](int k, KfUpload& v) {
@@ -1735,14 +1855,17 @@ static int kf_chain(lvb_icp* const hs[2], KfRec* kfs, int n_kf, const float cell
         }
         const KfUpload& ul = u[n_kf - 1];
         h->scan_n = kfs[n_kf - 1].n[m]; h->scan_stride = ul.stride[m]; h->scan_dev = ul.scan[m]; h->kf_arena = ul.arena;
+        h->scan_cloud = kfs[n_kf - 1].pend[m].pts;
     }
+    std::vector<lvb_icp::Segment> drop;           // released after the stores are unlocked
+    StoreLock lk(hs[0], hs[1]);
     for (int k = 0; k < n_kf; ++k) {
         KfRec& kf = kfs[k];
         for (int m = 0; m < 2; ++m) {
             lvb_icp::Segment& sg = stage[2 * (size_t)k + m];
-            if (kf.pend[m]) { sg.robot = kf.pend[m]->pts; kf.pend[m]->pts = nullptr; }     // moved: the pending entry goes below
+            if (kf.pend[m].pts) sg.robot = kf.pend[m].pts;          // the pending cloud becomes the robot-frame cloud; its entry goes below
             bbox_store(sg, hb[k].out_bbox[m]);
-            store_segment(hs[m], kf.key, sg);
+            store_segment(hs[m], kf.key, sg, drop);
             const MapDesc& md = hb[k].map[m];
             const bool built = pl[k].build[m] && md.P > 0;
             kf.n_map_points[m] = built ? md.P : 0;
@@ -1753,8 +1876,10 @@ static int kf_chain(lvb_icp* const hs[2], KfRec* kfs, int n_kf, const float cell
         memcpy(kf.transform, hl[k].T, sizeof(kf.transform));
     }
     for (int m = 0; m < 2; ++m) {
-        auto& pv = hs[m]->pending;
-        pv.erase(std::remove_if(pv.begin(), pv.end(), [](const lvb_icp::Pending& pd) { return pd.pts == nullptr; }), pv.end());
+        auto& pv = hs[m]->store->pending;
+        std::unordered_set<const DevBuf<float4>*> used;
+        for (int k = 0; k < n_kf; ++k) if (kfs[k].pend[m].pts) used.insert(kfs[k].pend[m].pts.get());
+        pv.erase(std::remove_if(pv.begin(), pv.end(), [&](const lvb_icp::Pending& pd) { return used.count(pd.pts.get()) > 0; }), pv.end());
     }
     return LVB_OK;
 }
@@ -1763,15 +1888,19 @@ static int kf_chain(lvb_icp* const hs[2], KfRec* kfs, int n_kf, const float cell
 // handles.  One side alone, or a key with nothing pending on a handle, is an error; nothing changes.
 static int resolve_by_key(lvb_icp* const hs[2], KfRec& kf, const char* fn) {
     const bool bk[2] = {!kf.pts[0] && kf.n[0] < 0, !kf.pts[1] && kf.n[1] < 0};
-    kf.pend[0] = kf.pend[1] = nullptr;
+    kf.pend[0] = kf.pend[1] = lvb_icp::Pending();
     if (!bk[0] && !bk[1]) return LVB_OK;
     if (!bk[0] || !bk[1]) { set_error("%s: keyframe %lld: give both clouds by key or neither", fn, kf.key); return LVB_ERR_INVALID; }
-    lvb_icp::Pending* pd[2];
-    for (int m = 0; m < 2; ++m) {
-        pd[m] = find_pending(hs[m], kf.key);
-        if (!pd[m]) { set_error("%s: key %lld has no pending features on the %s handle", fn, kf.key, m ? "surf" : "ground"); return LVB_ERR_INVALID; }
+    lvb_icp::Pending pd[2];
+    {
+        StoreLock lk(hs[0], hs[1]);
+        for (int m = 0; m < 2; ++m) {
+            const lvb_icp::Pending* e = find_pending(*hs[m]->store, kf.key);
+            if (!e) { set_error("%s: key %lld has no pending features on the %s handle", fn, kf.key, m ? "surf" : "ground"); return LVB_ERR_INVALID; }
+            pd[m] = *e;
+        }
     }
-    for (int m = 0; m < 2; ++m) { kf.pend[m] = pd[m]; kf.pts[m] = pd[m]->pts->p; kf.n[m] = pd[m]->n; }
+    for (int m = 0; m < 2; ++m) { kf.pend[m] = pd[m]; kf.pts[m] = pd[m].pts->p; kf.n[m] = pd[m].n; }
     return LVB_OK;
 }
 
@@ -1785,7 +1914,7 @@ int lvb_icp_map_build_optimize_keyframe(lvb_icp* ground, lvb_icp* surf, const lo
     lvb_icp* hs[2] = {ground, surf};
     if (!ground || !surf || ground == surf || !cell_size || !map_pose || !p || !pose || !rpyxyz || n_keys < 0 || (n_keys && !keys)) {
         set_error("%s: null or bad argument", fn); return LVB_ERR_INVALID; }
-    KfRec kf = {key, keys, n_keys, {ground_pts, surf_pts}, {n_ground, n_surf}, {nullptr, nullptr}, map_pose, {}, {p->weight[0], p->weight[1]}, p->prior_weight};
+    KfRec kf = {key, keys, n_keys, {ground_pts, surf_pts}, {n_ground, n_surf}, {}, map_pose, {}, {p->weight[0], p->weight[1]}, p->prior_weight};
     LVB_TRY(resolve_by_key(hs, kf, fn));
     LVB_TRY(kf_check_args(hs, cell_size, kf.pts, kf.n, stride, p, fn));
     memcpy(kf.pose, pose, sizeof(kf.pose));
@@ -1810,7 +1939,7 @@ int lvb_icp_map_optimize_keyframes(lvb_icp* ground, lvb_icp* surf, lvb_map_keyfr
     std::vector<KfRec> rec(n_kf);
     for (int k = 0; k < n_kf; ++k) {
         const lvb_map_keyframe& kf = kfs[k];
-        rec[k] = {kf.key, kf.map_keys, kf.n_map_keys, {kf.ground_pts, kf.surf_pts}, {kf.n_ground, kf.n_surf}, {nullptr, nullptr}, kf.map_pose, {},
+        rec[k] = {kf.key, kf.map_keys, kf.n_map_keys, {kf.ground_pts, kf.surf_pts}, {kf.n_ground, kf.n_surf}, {}, kf.map_pose, {},
                   {kf.weight[0], kf.weight[1]}, kf.prior_weight};
         memcpy(rec[k].pose, kf.pose, sizeof(kf.pose));
         LVB_TRY(resolve_by_key(hs, rec[k], fn));
@@ -1851,10 +1980,14 @@ int lvb_icp_map_relocate(lvb_icp* ground, lvb_icp* surf, const long long* keys, 
     lvb_ctx* ctx = ground->ctx;
     LVB_CUDA(cudaSetDevice(ctx->device)); lvb::g_alloc_stream = ctx->stream;
     std::vector<std::vector<KfSrc>> srcs(1);
-    for (int k = 0; k < n_keys; ++k) {
-        KfSrc sr = {-1, {nullptr, nullptr}};
-        if (!find_resident(hs, keys[k], sr)) { set_error("%s: key %lld is not resident", fn, keys[k]); return LVB_ERR_INVALID; }
-        srcs[0].push_back(sr);
+    Snapshot snap;
+    {
+        StoreLock lk(ground, surf);
+        for (int k = 0; k < n_keys; ++k) {
+            KfSrc sr = {-1, {nullptr, nullptr}};
+            if (!find_resident(hs, snap, keys[k], sr)) { set_error("%s: key %lld is not resident", fn, keys[k]); return LVB_ERR_INVALID; }
+            srcs[0].push_back(sr);
+        }
     }
     std::vector<KfPlan> plans;
     LVB_TRY(plan_frames(hs, srcs, nullptr, nullptr, cell_size, ground_threshold > 0.0, fn, plans));
@@ -1905,7 +2038,8 @@ int lvb_icp_map_relocate(lvb_icp* ground, lvb_icp* surf, const long long* keys, 
 // ---- Mapping::ToWorld(start) after a GNSS or loop correction (mapping.cpp:222-229; backend.cpp:71-91, relocator.cpp:236-244): the
 // world clouds of n_keys resident keyframes on one or both handles re-made from their robot-frame records at new poses.  One pinned
 // upload of the table [TwSeg per (handle, key) | first block per entry | boxes], one kernel over every point, the boxes read back with
-// one copy, one host synchronisation.  Every check comes before the upload; the clouds are overwritten in place.
+// one copy, one host synchronisation.  Every check comes before the upload; the clouds are overwritten in place, or on a shared store
+// written into new buffers that replace them at the commit.
 int lvb_icp_map_to_world(lvb_icp* ground, lvb_icp* surf, const long long* keys, int n_keys, const double* poses) {
     static const char* fn = "lvb_icp_map_to_world";
     lvb_icp* hs[2] = {ground, surf};
@@ -1919,16 +2053,29 @@ int lvb_icp_map_to_world(lvb_icp* ground, lvb_icp* surf, const long long* keys, 
         const auto dup = std::adjacent_find(sorted.begin(), sorted.end());
         if (dup != sorted.end()) { set_error("%s: key %lld is listed twice", fn, *dup); return LVB_ERR_INVALID; }
     }
-    std::vector<lvb_icp::Segment*> segs;
-    std::vector<int> pose_of;                 // the row of `poses` each entry takes
-    for (int m = 0; m < 2; ++m) {
-        if (!hs[m]) continue;
-        std::unordered_map<long long, lvb_icp::Segment*> at;
-        for (auto& sg : hs[m]->segments) at[sg.key] = &sg;
-        for (int k = 0; k < n_keys; ++k) {
-            const auto it = at.find(keys[k]);
-            if (it == at.end()) { set_error("%s: key %lld is not resident on the %s handle", fn, keys[k], m ? "surf" : "ground"); return LVB_ERR_INVALID; }
-            segs.push_back(it->second); pose_of.push_back(k);
+    // the call's snapshot of the listed clouds; on a store another handle shares, each gets a new world buffer (copy-on-write): another
+    // thread's call may take its snapshot while the kernel runs, and must see the cloud as it was.  An unshared store is overwritten in
+    // place, and lvb_icp_share waits for that write to be committed.
+    std::vector<lvb_icp::Segment> segs;
+    std::vector<int> pose_of, side;           // the row of `poses` each entry takes, and its handle
+    bool cow[2] = {false, false};
+    struct InPlace {                          // clears the in-place flags on every return
+        IcpStore* st[2] = {nullptr, nullptr};
+        ~InPlace() { for (IcpStore* x : st) if (x) { { std::lock_guard<std::mutex> lk(x->mu); x->in_place = false; } x->cv.notify_all(); } }
+    } in_place;
+    {
+        StoreLock lk(ground, surf);
+        for (int m = 0; m < 2; ++m) {
+            if (!hs[m]) continue;
+            std::unordered_map<long long, const lvb_icp::Segment*> at;
+            for (auto& sg : hs[m]->store->segments) at[sg.key] = &sg;
+            for (int k = 0; k < n_keys; ++k) {
+                const auto it = at.find(keys[k]);
+                if (it == at.end()) { set_error("%s: key %lld is not resident on the %s handle", fn, keys[k], m ? "surf" : "ground"); return LVB_ERR_INVALID; }
+                segs.push_back(*it->second); pose_of.push_back(k); side.push_back(m);
+            }
+            cow[m] = hs[m]->store->handles > 1;
+            if (!cow[m]) { hs[m]->store->in_place = true; in_place.st[m] = hs[m]->store.get(); }
         }
     }
     const size_t S = segs.size();
@@ -1936,18 +2083,35 @@ int lvb_icp_map_to_world(lvb_icp* ground, lvb_icp* surf, const long long* keys, 
     size_t blocks = 0;
     for (size_t i = 0; i < S; ++i) {
         first[i] = (int)blocks;
-        blocks += inblk(segs[i]->n, TW_TPB * TW_PER);
+        blocks += inblk(segs[i].n, TW_TPB * TW_PER);
         if (blocks > 0x7fffffffull) { set_error("%s: more than 2^31 blocks of %d points", fn, TW_TPB * TW_PER); return LVB_ERR_INVALID; }
     }
     int seed[6];
     bbox_seed(seed);
+    std::vector<Cloud> fresh(S);              // the copy-on-write world buffers (NULL: in place)
+    std::vector<lvb_icp::Segment> drop;       // the replaced references, released after the stores are unlocked
+    // publish the boxes (boxes + 6 i) and the new buffers of the listed clouds; `commit` is set once the device writes are complete
+    auto publish = [&](const int* boxes) {
+        StoreLock lk(ground, surf);
+        for (size_t i = 0; i < S; ++i) {
+            lvb_icp::Segment* e = find_segment(*hs[side[i]]->store, segs[i].key);
+            if (!e || e->pts != segs[i].pts) continue;
+            if (fresh[i]) { drop.push_back(*e); e->pts = fresh[i]; }
+            bbox_store(*e, boxes ? boxes + 6 * i : seed);
+        }
+    };
     if (blocks == 0) {         // every listed cloud is empty: nothing to write, and their boxes stay the empty seeds
-        for (auto* sg : segs) bbox_store(*sg, seed);
+        publish(nullptr);
         return LVB_OK;
     }
     lvb_ctx* ctx = (ground ? ground : surf)->ctx;
     lvb_icp* h0 = ground ? ground : surf;
     LVB_CUDA(cudaSetDevice(ctx->device)); lvb::g_alloc_stream = ctx->stream;
+    for (size_t i = 0; i < S; ++i) {
+        if (!cow[side[i]]) continue;
+        fresh[i] = new_cloud();
+        LVB_TRY(fresh[i]->ensure(std::max(1, segs[i].n)));
+    }
     cudaStream_t s = ctx->stream;
     const size_t off_first = (S * sizeof(TwSeg) + 255) & ~(size_t)255;
     const size_t off_box = (off_first + S * sizeof(int) + 255) & ~(size_t)255;
@@ -1957,7 +2121,7 @@ int lvb_icp_map_to_world(lvb_icp* ground, lvb_icp* surf, const long long* keys, 
     TwSeg* ht = reinterpret_cast<TwSeg*>(ctx->stage_h);
     int* hbox = reinterpret_cast<int*>(ctx->stage_h + off_box);
     for (size_t i = 0; i < S; ++i) {
-        ht[i].robot = segs[i]->robot->p; ht[i].world = segs[i]->pts->p; ht[i].n = segs[i]->n;
+        ht[i].robot = segs[i].robot->p; ht[i].world = fresh[i] ? fresh[i]->p : segs[i].pts->p; ht[i].n = segs[i].n;
         for (int k = 0; k < 7; ++k) ht[i].tf[k] = (float)poses[7 * (size_t)pose_of[i] + k];      // pose.cast<float>() (mapping.cpp:195)
         memcpy(hbox + 6 * i, seed, sizeof(seed));
     }
@@ -1974,7 +2138,7 @@ int lvb_icp_map_to_world(lvb_icp* ground, lvb_icp* surf, const long long* keys, 
     LVB_CUDA(cudaMemcpyAsync(hbox, dbox, S * 6 * sizeof(int), cudaMemcpyDeviceToHost, s));
     LVB_TRY(host_sync(ctx, s));
     ctx->stage_busy = false;
-    for (size_t i = 0; i < S; ++i) bbox_store(*segs[i], hbox + 6 * i);
+    publish(hbox);
     return LVB_OK;
 }
 
@@ -1994,18 +2158,28 @@ int lvb_icp_map_extract_keyframe(lvb_icp* ground, lvb_icp* surf, const lvb_lidar
     lvb_icp::Pending pd[2];
     int rc = LVB_OK;
     for (int m = 0; m < 2; ++m) {
-        pd[m].key = key; pd[m].n = counts[m]; pd[m].pts = new DevBuf<float4>();
+        pd[m].key = key; pd[m].n = counts[m]; pd[m].pts = new_cloud();
         for (int a = 0; a < 3; ++a) { pd[m].lo[a] = box[6 * m + a]; pd[m].hi[a] = box[6 * m + 3 + a]; }
         if (rc == LVB_OK) rc = pd[m].pts->ensure(std::max(1, counts[m]));
         if (rc == LVB_OK && counts[m] &&
             cudaMemcpyAsync(pd[m].pts->p, feat[m].p, (size_t)counts[m] * sizeof(float4), cudaMemcpyDeviceToDevice, ground->ctx->stream) != cudaSuccess)
             rc = lvb::cuda_fail(cudaGetLastError(), "pending copy", __FILE__, __LINE__);
     }
-    if (rc != LVB_OK) { delete pd[0].pts; delete pd[1].pts; return rc; }
+    if (rc != LVB_OK) return rc;
     lvb_icp* hs[2] = {ground, surf};
+    bool shared = false;
+    {
+        StoreLock lk(ground, surf);
+        for (int m = 0; m < 2; ++m) shared = shared || hs[m]->store->handles > 1;
+    }
+    // the copies are stream-ordered on this context: another handle's stream may read the features next, so on a shared store they are
+    // waited for before they are published
+    if (shared) LVB_TRY(host_sync(ground->ctx, ground->ctx->stream));
+    std::vector<lvb_icp::Pending> drop;
+    StoreLock lk(ground, surf);
     for (int m = 0; m < 2; ++m) {
-        drop_pending(hs[m], key);              // a second extraction under the same key replaces the first
-        hs[m]->pending.push_back(pd[m]);
+        drop_pending(*hs[m]->store, key, drop);          // a second extraction under the same key replaces the first
+        hs[m]->store->pending.push_back(pd[m]);
     }
     *n_ground = counts[0]; *n_surf = counts[1];
     return LVB_OK;
@@ -2014,9 +2188,9 @@ int lvb_icp_map_extract_keyframe(lvb_icp* ground, lvb_icp* surf, const lvb_lidar
 int lvb_debug_icp_cloud_capacity(lvb_icp* h, long long key, long long cap[3]) {
     if (!h || !cap) { set_error("null argument"); return LVB_ERR_INVALID; }
     cap[0] = cap[1] = cap[2] = -1;
-    for (auto& sg : h->segments)
-        if (sg.key == key) { cap[0] = sg.pts ? (long long)sg.pts->n : -1; cap[1] = sg.robot ? (long long)sg.robot->n : -1; }
-    if (const lvb_icp::Pending* pd = find_pending(h, key)) cap[2] = (long long)pd->pts->n;
+    std::lock_guard<std::mutex> lk(h->store->mu);
+    if (const lvb_icp::Segment* sg = find_segment(*h->store, key)) { cap[0] = sg->pts ? (long long)sg->pts->n : -1; cap[1] = sg->robot ? (long long)sg->robot->n : -1; }
+    if (const lvb_icp::Pending* pd = find_pending(*h->store, key)) cap[2] = (long long)pd->pts->n;
     return LVB_OK;
 }
 
