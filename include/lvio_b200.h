@@ -104,8 +104,20 @@ LVB_API void lvb_default_options(lvb_solve_options* o);
 
 /* ---- context ------------------------------------------------------------------------- */
 /* cuda_stream: a cudaStream_t to launch on (e.g. torch.cuda.current_stream().cuda_stream),
- * or NULL to let the context create its own non-blocking stream. */
+ * or NULL to let the context create its own non-blocking stream.  The context's second stream (the parallel branches of an LM pass)
+ * gets the priority of the stream it launches on: the default one with NULL. */
 LVB_API int lvb_ctx_create(int device, void* cuda_stream, lvb_ctx** out);
+/* Scheduling priority of all of a context's device work.  As lvb_ctx_create(device, NULL, out), but both of the context's streams are
+ * made with cudaStreamCreateWithPriority(..., cudaStreamNonBlocking, priority).  CUDA's convention: a lower number runs earlier (its
+ * pending CTAs are dispatched first; running CTAs are not pre-empted), and CUDA clamps the value to the device's range
+ * (lvb_device_priority_range).  Results, launches and synchronisations are those of a default-priority context.  A thread whose calls
+ * others wait on -- the one that runs the window solve and the mapping pass -- can put its work first this way. */
+LVB_API int lvb_ctx_create_with_priority(int device, int priority, lvb_ctx** out);
+/* the priority the context's stream actually has (after clamping, or the caller's stream's) */
+LVB_API int lvb_ctx_priority(lvb_ctx* ctx, int* priority);
+/* cudaDeviceGetStreamPriorityRange of `device`: *greatest <= *least; the default priority is 0.  The calling thread's current device
+ * is left as it was. */
+LVB_API int lvb_device_priority_range(int device, int* least, int* greatest);
 LVB_API void lvb_ctx_destroy(lvb_ctx* ctx);
 LVB_API const char* lvb_last_error(void);            /* thread-local text of the last failure */
 LVB_API long long lvb_launch_count(lvb_ctx* ctx);    /* kernels launched through this context so far */
@@ -466,6 +478,8 @@ LVB_API int lvb_icp_map_extract_keyframe(lvb_icp* ground, lvb_icp* surf, const l
 LVB_API int lvb_debug_timing(int enable);
 /* as lvb_debug_timing(0), but writes "kernel_name microseconds" lines (launch order) into out instead of printing them */
 LVB_API int lvb_debug_timing_report(char* out, int cap);
+/* priority[0]: the priority of the context's stream, priority[1]: that of its side stream */
+LVB_API int lvb_debug_ctx_stream_priorities(lvb_ctx* ctx, int priority[2]);
 /* the capacities, in 16-byte records, of the buffers the handle keeps for `key`: cap[0] its resident world cloud, cap[1] its
  * robot-frame cloud, cap[2] its pending features (-1: none) */
 LVB_API int lvb_debug_icp_cloud_capacity(lvb_icp* icp, long long key, long long cap[3]);

@@ -435,7 +435,8 @@ private:
     // there is one) the thread's own pair; on any other thread a pair lvb_icp_share made once for that thread, on its own context, from
     // the resident pair.  meta: the Handles whose key sets describe that store (read and written under meta_).  The resident pair and
     // its context belong to the thread that keeps it (thread_local), so that thread must outlive the other threads' calls, as the
-    // reference's mapping thread does; the shared pairs keep the clouds themselves alive.
+    // reference's mapping thread does; the shared pairs keep the clouds themselves alive.  Every pair, own or shared, is made on the
+    // calling thread's Runtime::get().ctx, so its calls run at the priority that thread chose with Runtime::set_thread_priority.
     struct StoreView { lvb_icp* ground; lvb_icp* surf; Handles* meta; };
     bool store_view(StoreView& v) {
         Handles& own = handles_of_thread()[this];

@@ -46,7 +46,18 @@ struct Runtime {
     static Runtime& get() { static thread_local Runtime r; return r; }
     bool ensure(int device = 0) {
         if (ctx) return true;
-        if (lvb_ctx_create(device, nullptr, &ctx) != LVB_OK) { error = lvb_last_error(); ctx = nullptr; return false; }
+        const int rc = create_with_priority ? create_with_priority(device, priority, &ctx) : lvb_ctx_create(device, nullptr, &ctx);
+        if (rc != LVB_OK) { error = lvb_last_error(); ctx = nullptr; return false; }
+        return true;
+    }
+    // The CUDA stream priority of this thread's device work (lvb_ctx_create_with_priority; lower runs earlier, see
+    // lvb_device_priority_range), e.g. the greatest for the thread that runs Backend::Optimize, whose pass the frontend waits for.
+    // Call it on the thread, before its first device call: the context is made then.  Once it exists this returns false with a
+    // message in `error` and leaves the priority as it is.
+    bool set_thread_priority(int p) {
+        if (ctx) { error = "set_thread_priority: this thread's context already exists; call it before the thread's first device call"; return false; }
+        priority = p;
+        create_with_priority = &lvb_ctx_create_with_priority;
         return true;
     }
     // cam = { fx fy cx cy  extrinsic[7] } per camera, Camera::Get(0) then Camera::Get(1)
@@ -56,6 +67,10 @@ struct Runtime {
     // (never destroyed: the solver threads of the reference live as long as the process, and tearing a context down from a
     // thread_local destructor at process exit would call into a CUDA runtime that is already unloading)
 private:
+    int priority = 0;
+    // set by set_thread_priority, so that only a program that sets a priority references the entry point (a C ABI server without
+    // stream priorities, such as the CPU oracle, still serves the others)
+    int (*create_with_priority)(int, int, lvb_ctx**) = nullptr;
     struct Rig { double c[22] = {0}; bool have = false; };
     static Rig& rig() { static Rig r; return r; }
     Runtime() : cameras(rig().c), have_cameras(rig().have) {}

@@ -147,6 +147,10 @@ _SIGS = {
 # entry points only the CUDA library exports
 _LVB_ONLY = {
     "comm_unique_id": (C.c_int, [C.c_char_p]),
+    # stream priorities: the CPU oracle has no streams to schedule
+    "ctx_create_with_priority": (C.c_int, [C.c_int, C.c_int, C.POINTER(VP)]),
+    "ctx_priority": (C.c_int, [VP, c_int_p]),
+    "device_priority_range": (C.c_int, [C.c_int, c_int_p, c_int_p]),
     "comm_init": (C.c_int, [VP, C.c_int, C.c_int, C.c_char_p]),
     "ba_set_schur_mode": (C.c_int, [VP, C.c_int]),
     "icp_share": (C.c_int, [VP, VP, C.POINTER(VP)]),
@@ -171,6 +175,7 @@ _LVB_ONLY = {
     "debug_timing": (C.c_int, [C.c_int]),
     "debug_cholesky_clocks": (C.c_int, [C.POINTER(C.c_longlong), C.c_int]),
     "debug_timing_report": (C.c_int, [C.c_char_p, C.c_int]),
+    "debug_ctx_stream_priorities": (C.c_int, [VP, c_int_p]),
     "debug_icp_map_grid": (C.c_int, [VP, c_int_p]),
     "debug_icp_cloud_capacity": (C.c_int, [VP, C.c_longlong, C.POINTER(C.c_longlong)]),
     "debug_band_solve": (C.c_int, [VP, C.c_int, C.c_int, c_double_p, c_double_p, c_double_p, C.c_int, c_int_p]),

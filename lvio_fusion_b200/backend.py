@@ -48,13 +48,30 @@ def _f64(a):
 
 
 class Context:
-    """lvb_ctx: one device + stream."""
+    """lvb_ctx: one device + stream.
 
-    def __init__(self, api=None, device=0, stream=None):
+    stream: a cudaStream_t (int) to launch on, or None for a stream of the context's own.  priority: make that stream, and the context's
+    second one, at this CUDA stream priority (lvb_ctx_create_with_priority, CUDA library only): a lower number runs earlier, CUDA clamps
+    it to priority_range(api, device).  A caller's stream already has a priority, so passing both is an error."""
+
+    def __init__(self, api=None, device=0, stream=None, priority=None):
+        self.h = None
         self.api = api or _capi.load()
+        if stream is not None and priority is not None:
+            raise ValueError("Context: pass stream or priority, not both (a caller's stream keeps its own priority)")
         h = C.c_void_p()
-        self.api.check(self.api.ctx_create(int(device), C.c_void_p(stream) if stream else None, C.byref(h)), "ctx_create")
+        if priority is None:
+            self.api.check(self.api.ctx_create(int(device), C.c_void_p(stream) if stream else None, C.byref(h)), "ctx_create")
+        else:
+            self.api.check(self.api.ctx_create_with_priority(int(device), int(priority), C.byref(h)), "ctx_create_with_priority")
         self.h = h
+
+    @property
+    def priority(self):
+        """The CUDA stream priority the context's work runs at (lvb_ctx_priority, CUDA library only)."""
+        p = C.c_int()
+        self.api.check(self.api.ctx_priority(self.h, C.byref(p)), "ctx_priority")
+        return p.value
 
     def launch_count(self):
         return int(self.api.launch_count(self.h))
@@ -79,6 +96,13 @@ class Context:
             self.close()
         except Exception:
             pass
+
+
+def priority_range(api, device=0):
+    """(least, greatest) CUDA stream priorities of `device` (lvb_device_priority_range): greatest <= least, the default is 0."""
+    least, greatest = C.c_int(), C.c_int()
+    api.check(api.device_priority_range(int(device), C.byref(least), C.byref(greatest)), "device_priority_range")
+    return least.value, greatest.value
 
 
 def default_options(api, **kw):

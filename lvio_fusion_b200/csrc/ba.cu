@@ -1901,6 +1901,9 @@ int lvb_ba_solve(lvb_ba* ba, const lvb_solve_options* options, lvb_solve_summary
             }
             if (!ba->pass_graph) {
                 cudaGraphExec_t ex = nullptr;
+                // no cudaGraphInstantiateFlagUseNodePriority: every node of a replay, the side-stream branches included, runs at the
+                // priority of the stream the graph is launched into, i.e. the context's (lvb_ctx_create_with_priority), and a cached
+                // graph re-targeted to another problem of the context keeps doing so
                 ce = cudaGraphInstantiate(&ex, g, 0);
                 if (ce != cudaSuccess) { cudaGraphDestroy(g); LVB_CUDA(ce); }
                 ba->pass_graph = ex; ba->graph_borrowed = !own;

@@ -241,8 +241,7 @@ void lvb_default_options(lvb_solve_options* o) {
 
 const char* lvb_last_error(void) { return g_last_error.c_str(); }
 
-int lvb_ctx_create(int device, void* cuda_stream, lvb_ctx** out) {
-    if (!out) { set_error("out is NULL"); return LVB_ERR_INVALID; }
+static int check_device(int device) {
     int count = 0;
     cudaError_t e = cudaGetDeviceCount(&count);
     if (e != cudaSuccess || count == 0) {
@@ -250,20 +249,24 @@ int lvb_ctx_create(int device, void* cuda_stream, lvb_ctx** out) {
         return LVB_ERR_CUDA;
     }
     if (device < 0 || device >= count) { set_error("device %d out of range (%d devices)", device, count); return LVB_ERR_INVALID; }
-    LVB_CUDA(cudaSetDevice(device));
-    cudaDeviceProp prop;
-    LVB_CUDA(cudaGetDeviceProperties(&prop, device));
-    if (prop.major != 9 || prop.minor != 0) { set_error("device %d is sm_%d%d; this library is built for sm_90a (H100) only", device, prop.major, prop.minor); return LVB_ERR_CUDA; }
-    lvb_ctx* c = new lvb_ctx();
-    c->device = device;
-    c->sm_count = prop.multiProcessorCount;
+    return LVB_OK;
+}
+
+// the context's streams, events and switches; on failure the caller destroys the partly made context
+static int ctx_init(lvb_ctx* c, void* cuda_stream, const int* priority) {
     if (cuda_stream) { c->stream = (cudaStream_t)cuda_stream; c->own_stream = false; }
+    else if (priority) { LVB_CUDA(cudaStreamCreateWithPriority(&c->stream, cudaStreamNonBlocking, *priority)); c->own_stream = true; }
     else { LVB_CUDA(cudaStreamCreateWithFlags(&c->stream, cudaStreamNonBlocking)); c->own_stream = true; }
     {   // keep freed device memory in the stream-ordered pool (see DevBuf)
         cudaMemPool_t pool;
-        if (cudaDeviceGetDefaultMemPool(&pool, device) == cudaSuccess) { unsigned long long thr = ~0ull; cudaMemPoolSetAttribute(pool, cudaMemPoolAttrReleaseThreshold, &thr); }
+        if (cudaDeviceGetDefaultMemPool(&pool, c->device) == cudaSuccess) { unsigned long long thr = ~0ull; cudaMemPoolSetAttribute(pool, cudaMemPoolAttrReleaseThreshold, &thr); }
     }
-    LVB_CUDA(cudaStreamCreateWithFlags(&c->side, cudaStreamNonBlocking));
+    // The side stream carries the parallel branches of an LM pass that is not replayed as a graph (a replay runs every node at the
+    // priority of the stream it is launched into), so it takes the priority the main stream actually has: the caller's stream's, or
+    // *priority as CUDA clamped it.
+    int prio = 0;
+    LVB_CUDA(cudaStreamGetPriority(c->stream, &prio));
+    LVB_CUDA(cudaStreamCreateWithPriority(&c->side, cudaStreamNonBlocking, prio));
     LVB_CUDA(cudaEventCreateWithFlags(&c->ev_fork, cudaEventDisableTiming));
     LVB_CUDA(cudaEventCreateWithFlags(&c->ev_join, cudaEventDisableTiming));
     const char* no_side = getenv("LVB_NO_SIDE");
@@ -280,7 +283,55 @@ int lvb_ctx_create(int device, void* cuda_stream, lvb_ctx** out) {
     if (pt && atof(pt) > 0) c->p2p_timeout_ns = (unsigned long long)(atof(pt) * 1e6);
     const char* ce = getenv("LVB_CHECK_EVERY");
     if (ce && atoi(ce) > 0) c->check_every = atoi(ce);
+    return LVB_OK;
+}
+
+// lvb_ctx_create (priority NULL) and lvb_ctx_create_with_priority (cuda_stream NULL)
+static int ctx_create(int device, void* cuda_stream, const int* priority, lvb_ctx** out) {
+    if (!out) { set_error("out is NULL"); return LVB_ERR_INVALID; }
+    *out = nullptr;
+    LVB_TRY(check_device(device));
+    LVB_CUDA(cudaSetDevice(device));
+    cudaDeviceProp prop;
+    LVB_CUDA(cudaGetDeviceProperties(&prop, device));
+    if (prop.major != 9 || prop.minor != 0) { set_error("device %d is sm_%d%d; this library is built for sm_90a (H100) only", device, prop.major, prop.minor); return LVB_ERR_CUDA; }
+    lvb_ctx* c = new lvb_ctx();
+    c->device = device;
+    c->sm_count = prop.multiProcessorCount;
+    const int rc = ctx_init(c, cuda_stream, priority);
+    if (rc != LVB_OK) { lvb_ctx_destroy(c); return rc; }
     *out = c;
+    return LVB_OK;
+}
+
+int lvb_ctx_create(int device, void* cuda_stream, lvb_ctx** out) { return ctx_create(device, cuda_stream, nullptr, out); }
+
+int lvb_ctx_create_with_priority(int device, int priority, lvb_ctx** out) { return ctx_create(device, nullptr, &priority, out); }
+
+int lvb_ctx_priority(lvb_ctx* ctx, int* priority) {
+    if (!ctx || !priority) { set_error("ctx or priority is NULL"); return LVB_ERR_INVALID; }
+    LVB_CUDA(cudaStreamGetPriority(ctx->stream, priority));
+    return LVB_OK;
+}
+
+int lvb_device_priority_range(int device, int* least, int* greatest) {
+    if (!least || !greatest) { set_error("least or greatest is NULL"); return LVB_ERR_INVALID; }
+    LVB_TRY(check_device(device));
+    int cur = 0;
+    LVB_CUDA(cudaGetDevice(&cur));
+    LVB_CUDA(cudaSetDevice(device));
+    int lo = 0, hi = 0;
+    const cudaError_t e = cudaDeviceGetStreamPriorityRange(&lo, &hi);
+    cudaSetDevice(cur);                                         // a query: the calling thread's current device stays as it was
+    LVB_CUDA(e);
+    *least = lo; *greatest = hi;
+    return LVB_OK;
+}
+
+int lvb_debug_ctx_stream_priorities(lvb_ctx* ctx, int priority[2]) {
+    if (!ctx || !priority) { set_error("ctx or priority is NULL"); return LVB_ERR_INVALID; }
+    LVB_CUDA(cudaStreamGetPriority(ctx->stream, &priority[0]));
+    LVB_CUDA(cudaStreamGetPriority(ctx->side, &priority[1]));
     return LVB_OK;
 }
 
